@@ -1,17 +1,18 @@
 #!/usr/bin/env python
 """bench.py — images/sec of one TRAINING step (forward + per-pixel CE + backward [+ SyncBN exchange + gradient
 all-reduce] + SGD update) of DeepLabV3+/ResNet-101, 513x513, 19 classes (BASELINE.json metric, SURVEY.md §8d config C3)
-on N B200s of one node, synthetic data, random-init weights.
+on N H100s of one node, synthetic data, random-init weights.
 
-    python bench.py --gpus 1 --steps 10 --warmup 3                     # this engine (hand-written sm_100a kernels)
+    python bench.py --gpus 1 --steps 10 --warmup 3                     # this engine (hand-written sm_90a kernels)
+    python bench.py --gpus 1 --steps 10 --warmup 3 --dump-outputs DIR  # also write the last timed step's results as .npy
     python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...
     python bench.py --impl reference --gpus 1 --steps 2 --warmup 1     # reference algorithm on the host CPU cores
 
 One JSON line on stdout (rank 0).  `value` = device-resident throughput through the fused train step; `e2e` = the same
 step driven through the reference-facing plugin surface (model(x) -> CrossEntropyLoss2d -> backward -> torch.optim.SGD,
 i.e. what train.py/trainer.py:55-71 call) with the batch copied from pinned host memory every step and the loss read
-back; `roofline` = algorithmic conv FLOPs / CUDA-event time of the tcgen05 implicit-GEMM launches inside the timed
-region, against the measured dense-bf16 peak; `cpu_baseline` = the CPU oracle port timed on this box's host cores.
+back; `roofline` = algorithmic conv FLOPs / CUDA-event time of the wgmma implicit-GEMM launches inside the timed
+region, against the dense-bf16 peak; `cpu_baseline` = the CPU oracle port timed on this box's host cores.
 """
 import argparse
 import json
@@ -61,8 +62,8 @@ def measured_peaks():
     if os.path.exists(path):
         with open(path) as f:
             d = json.load(f)
-        return d.get("bf16_tflops_sustained", 1400.0), d.get("hbm_gbs", 6650.0), "measured (MEASURED_PEAKS.json, sustained)"
-    return 1400.0, 6650.0, "fallback (B200_PROFILING.md)"
+        return d.get("bf16_tflops_sustained", 989.0), d.get("hbm_gbs", 3350.0), "measured (MEASURED_PEAKS.json, sustained)"
+    return 989.0, 3350.0, "H100 SXM data sheet (dense BF16 at 700 W; HBM3), not measured"
 
 
 class ClockSampler:
@@ -119,6 +120,33 @@ def synthetic_batch(B, seed):
     for sl in ((slice(None), slice(0, 4)), (slice(None), slice(-4, None)), (slice(None), slice(None), slice(0, 4)), (slice(None), slice(None), slice(-4, None))):
         y[sl] = CFG["ignore"]
     return x, y
+
+
+DUMP_SAMPLE = 1 << 21  # elements per sampled array: 8 MB of float32 each, well under 64 MB for the whole dump
+
+
+def _sample(flat, seed):
+    """A fixed, seeded sample of a large flat tensor (the same positions for the same size, run to run)."""
+    if flat.numel() <= DUMP_SAMPLE:
+        return flat
+    g = torch.Generator().manual_seed(seed)
+    idx = torch.randint(0, flat.numel(), (DUMP_SAMPLE,), generator=g).sort().values
+    return flat[idx.to(flat.device)]
+
+
+def dump_outputs(d, loss, model, grads):
+    """What the caller of the timed step receives from its last execution: the loss, the parameters the SGD update left, the
+    gradients it applied and the BatchNorm running statistics — float32 (loss float64) .npy files in `d`."""
+    import numpy as np
+    os.makedirs(d, exist_ok=True)
+    torch.cuda.synchronize()
+    params = torch.cat([p.detach().reshape(-1).float() for p in model.parameters()])
+    bufs = [b.detach().reshape(-1).float() for n, b in model.named_buffers() if n.endswith(("running_mean", "running_var"))]
+    out = {"loss": loss.detach().double().reshape(()), "params_sample": _sample(params, 1), "grads_sample": _sample(grads.float(), 2)}
+    if bufs:
+        out["bn_running_stats_sample"] = _sample(torch.cat(bufs), 3)
+    for name, t in out.items():
+        np.save(os.path.join(d, name + ".npy"), t.cpu().numpy())
 
 
 def host_threads():
@@ -189,10 +217,9 @@ def cpu_port_step_time(batch, steps, warmup, threads):
 
 
 def _import_reference_tree():
-    """The UNMODIFIED reference tree, packed by baseline/install_ref.sh into baseline/_ref/reference.zip (git-ignored; built in
-    the build container where /root/reference exists, shipped to the GPU box like a built .so).  Returns its `models` package or
-    None.  Shims: SURVEY.md §8c (skimage stub; UperNet's undefined module globals)."""
-    z = os.path.join(ROOT, "baseline", "_ref", "reference.zip")
+    """The UNMODIFIED reference tree, packed by oracle/install_ref.sh into oracle/_ref/reference.zip (git-ignored; built by
+    build() where a reference checkout exists).  Returns its `models` package or None.  Shims: SURVEY.md §8c (skimage stub; UperNet's undefined module globals)."""
+    z = os.path.join(ROOT, "oracle", "_ref", "reference.zip")
     if not os.path.exists(z):
         return None
     import types
@@ -254,12 +281,12 @@ def reference_gpu_step_time(batch, steps, warmup, n_gpus, budget_s=None):
                 loss = loss.mean()
             loss.backward()
             opt.step()
-        how = (f"UNMODIFIED reference tree (baseline/_ref/reference.zip): models.{CFG['arch']} wrapped as base/base_trainer.py:33-38 "
+        how = (f"UNMODIFIED reference tree (oracle/_ref/reference.zip): models.{CFG['arch']} wrapped as base/base_trainer.py:33-38 "
                f"({'convert_model + DataParallelWithCallback' if CFG['sync_bn'] else 'nn.DataParallel'}, device_ids=range({n_gpus})), fp32 NCHW, "
                f"cudnn.benchmark, utils.losses.{'CrossEntropyLoss2d' if CFG['loss'] == 'CE' else CFG['loss']}, torch.optim.SGD; one process")
     else:
         if n_gpus > 1:
-            raise RuntimeError("reference tree not shipped (run baseline/install_ref.sh in the build container)")
+            raise RuntimeError("reference tree not packed (oracle/install_ref.sh needs a reference checkout)")
         sd, fwd, bb, dec = _oracle_model(dev)
         opt = torch.optim.SGD([{"params": dec}, {"params": bb, "lr": 0.001}], lr=0.01, momentum=0.9, weight_decay=1e-4)
 
@@ -303,7 +330,7 @@ def config_dict(args, world, use_graph=None, last_loss=None):
     """`config` of the JSON line — the SAME dict for this engine's arm and for `--impl reference` (the driver compares them)."""
     B = args.batch
     c = {"workload": workload(world=world, sync_bn=CFG["sync_bn"]), "per_gpu_batch": B, "global_batch": B * world, "parallelism": f"dp{world}",
-         "l2": "per-step working set (activations ~GBs) far exceeds the 126 MB L2; no explicit flush needed",
+         "l2": "per-step working set (activations ~GBs) far exceeds the 50 MB L2; no explicit flush needed",
          "dropout": "on (the reference's nn.Dropout / nn.Dropout2d sites)"}
     if use_graph is not None:
         c["cuda_graph"] = use_graph
@@ -358,10 +385,12 @@ def main():
     ap.add_argument("--ref-gpus", type=int, default=1)
     ap.add_argument("--ref-sync-bn", type=int, default=-1, help="reference-GPU leg: 1 = convert_model + DataParallelWithCallback, 0 = nn.DataParallel, -1 = the config's")
     ap.add_argument("--bucket-mb", type=float, default=float(os.environ.get("SEG_BUCKET_MB", "0")),
-                    help="N > 1: gradient all-reduce bucket size of the fused step in MB; 0 (default) = one all-reduce after the backward — "
-                         "measured faster than 25 MB buckets overlapped on a side stream at N = 2 (28.6 vs 29.3 ms) and N = 8 (29.3 vs 30.1 ms): "
-                         "the NCCL kernels take SMs from the backward they overlap (profiles/scale_r02.txt)")
+                    help="N > 1: gradient all-reduce bucket size of the fused step in MB; 0 (default) = one all-reduce after the backward "
+                         "(buckets overlapped on a side stream let the NCCL kernels take SMs from the backward they overlap)")
     ap.add_argument("--trace", default=None, help="after the timed runs, trace 2 steps per C-ABI call and write a table here")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last one computed (loss, updated parameters, gradients, BN running "
+                         "statistics; fixed seeded samples of the large ones) to DIR/<name>.npy, for output-by-output comparison of builds")
     args = ap.parse_args()
     CFG = CONFIGS[args.config]
     if args.batch <= 0:
@@ -474,6 +503,9 @@ def main():
     e1.record()
     barrier()
     ms_total = max_over_ranks(e0.elapsed_time(e1))
+    if args.dump_outputs and rank == 0:
+        grads = stepper.flat_grad if fused else torch.cat([p.grad.reshape(-1).float() for p in model.parameters() if p.grad is not None])
+        dump_outputs(args.dump_outputs, loss, model, grads)
     launches = launches_per_step * K
     prof, ops.PROFILE = ops.PROFILE, None
     if prof is None:  # graph replay: measure the conv launches on two extra eager steps (same kernels, same shapes)
@@ -491,7 +523,7 @@ def main():
     last_loss = float(loss.item())
     value = world * B * K / (ms_total * 1e-3)
 
-    # roofline of the dominant kernel family (tcgen05 implicit-GEMM conv: fprop + dgrad + wgrad launches)
+    # roofline of the dominant kernel family (wgmma implicit-GEMM conv: fprop + dgrad + wgrad launches)
     conv_ms = sum(a.elapsed_time(b) for _, _, a, b, _ in prof)
     conv_flops = sum(f for _, f, _, _, _ in prof)
     conv_bytes = sum(nb for _, _, _, _, nb in prof)
@@ -503,18 +535,9 @@ def main():
         d[2] += 1
     peak_tf, peak_hbm, peak_src = measured_peaks()
     achieved = conv_flops / (conv_ms * 1e-3) / 1e12 if conv_ms > 0 else 0.0
-    traffic, traffic_src = None, None
-    for tname in ("roofline_traffic_r02.json", "roofline_traffic_r01.json"):
-        tpath = os.path.join(ROOT, "profiles", tname)
-        if args.config == "C3" and os.path.exists(tpath):  # dram bytes per conv launch from the committed ncu launch list of this workload
-            with open(tpath) as f:
-                tj = json.load(f)
-            traffic, traffic_src = tj.get("dram_bytes_per_launch"), f"profiles/{tname} (ncu dram__bytes_read.sum + dram__bytes_write.sum, mean over %d conv launches)" % tj.get("launches", 0)
-            break
     roofline = {
-        "bound": "tensor", "kernel": "conv_gemm_tc<BN,KIND> / conv_gemm_tc2 (tcgen05 implicit GEMM; fprop+dgrad+wgrad launches)",
+        "bound": "tensor", "kernel": "conv_gemm_tc<BN,KIND> (wgmma implicit GEMM; fprop+dgrad+wgrad launches)",
         "achieved": achieved, "peak": peak_tf, "unit": "TFLOP/s", "frac": achieved / peak_tf, "peak_source": peak_src,
-        "traffic": traffic, "traffic_unit": "bytes/launch (DRAM)", "traffic_source": traffic_src,
         "algorithmic_bytes_per_launch": conv_bytes / max(len(prof), 1), "algorithmic_flops_per_launch": conv_flops / max(len(prof), 1),
         "launches": len(prof), "conv_share_of_step": (conv_ms / conv_steps) / (ms_total / K) if ms_total else None,
         "timed_on": "the timed steps" if not use_graph else "2 eager steps after the graph-replayed timed region (identical kernels)",
@@ -638,8 +661,8 @@ def main():
             t = cpu_port_step_time(args.cpu_batch, 5, 1, threads)
             cpu_baseline = {"value": args.cpu_batch / t, "unit": "images/sec", "cores": threads, "kind": "port",
                             "sample": f"5 timed steps (after 1 warm-up) of batch {args.cpu_batch} of the same train step, fp32 oracle port, {threads} threads"}
-        # at N > 1 the reference's one-process DataParallelWithCallback + threaded SyncBN step takes SECONDS (measured: 4.9 s at
-        # N = 2, profiles/bench_r02_n2.json) — informational, so opt-in there (SEG_GPU_REF_MULTI=1) to keep scaling runs short
+        # at N > 1 the reference's one-process DataParallelWithCallback + threaded SyncBN step takes seconds — informational, so
+        # opt-in there (SEG_GPU_REF_MULTI=1) to keep scaling runs short
         if not args.no_gpu_ref and (world == 1 or os.environ.get("SEG_GPU_REF_MULTI", "0") == "1"):
             try:  # the reference's OWN GPU path on the same GPUs: the denominator of north_star's ">= 6x" (BASELINE.md §4)
                 budget = float(os.environ.get("SEG_GPU_REF_BUDGET_S", "60")) if world > 1 else None

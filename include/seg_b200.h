@@ -1,5 +1,5 @@
 /*
- * seg_b200.h — C ABI of the B200-native segmentation hot path.
+ * seg_b200.h — C ABI of the H100-native segmentation hot path.
  *
  * Drop-in boundary for the forward/backward hot path of yassouali/pytorch-segmentation
  * (dilated-ResNet encoder -> ASPP / PSP head -> bilinear upsample -> per-pixel loss).  The reference is
@@ -31,9 +31,9 @@ extern "C" {
 #define SEG_DT_F32 1
 
 /* implementation selector for the conv entry points */
-#define SEG_IMPL_AUTO 0 /* tcgen05 where the shape allows, else SIMT */
+#define SEG_IMPL_AUTO 0 /* wgmma where the shape allows, else SIMT */
 #define SEG_IMPL_SIMT 1 /* CUDA-core implicit GEMM (any shape) */
-#define SEG_IMPL_TC 2   /* tcgen05 + TMA implicit GEMM, error if shape unsupported */
+#define SEG_IMPL_TC 2   /* wgmma + TMA implicit GEMM, error if shape unsupported */
 
 typedef struct seg_conv_desc {
   int32_t N, H, W, C;   /* input  [N,H,W,C]  (C = input channels)                 */
@@ -59,7 +59,7 @@ typedef struct seg_sync_desc {
 
 const char* seg_last_error(void);
 int seg_version(void);
-/* 0 if the current device is sm_100 and kernels can be launched */
+/* 0 if the current device is sm_90 and kernels can be launched */
 int seg_device_ok(void);
 /* number of kernel launches issued by this library since the last reset (gpu_launches in bench.py) */
 int64_t seg_launch_count(void);
@@ -71,7 +71,7 @@ void seg_launch_count_reset(void);
  * stats (optional): fp64 [2*K], ZERO at launch: per-channel sum and sum of squares of the result as stored — the reduction
  * half of nn.BatchNorm2d, produced by the conv epilogue.  Every CTA adds its (fixed-order) fp32 column sums with one fp64
  * atomic per channel: a sum of fp32 values in fp64 is exact while their exponents span < 2^17, so the order of the atomics
- * cannot change the result — the statistics are bit-reproducible (round 1's fp32 atomics were not).
+ * cannot change the result — the statistics are bit-reproducible (fp32 atomics would not be).
  * sync (optional, with stats): SyncBN — the last CTA to finish also pushes the totals (as fp32) to every peer's symmetric
  * buffer and raises the flags (csrc/seg_sync.cuh); sync_ticket = one zeroed uint32.  The consumer is
  * seg_bn_apply_train(..., sync, ...). */
@@ -81,8 +81,11 @@ int seg_conv2d_fwd(const seg_conv_desc* d, const void* x, const void* w_packed, 
 /* dx[N,H,W,C] = beta*dx + conv_transpose(dy, w)   (autograd of the above w.r.t. x) */
 int seg_conv2d_dgrad(const seg_conv_desc* d, const void* dy, const void* w_packed, void* dx, float beta,
                      int impl, void* stream);
-/* dw_packed (fp32 [R*S][K][C]) += dy^T * im2col(x)   (autograd w.r.t. the weight; caller zeroes dw first) */
-int seg_conv2d_wgrad(const seg_conv_desc* d, const void* dy, const void* x, float* dw_packed, int impl,
+/* dw_packed (fp32 [R*S][K][C]) += dy^T * im2col(x)   (autograd w.r.t. the weight; caller zeroes dw first).
+ * workspace: fp32 scratch of seg_conv2d_wgrad_workspace_floats(d, impl) floats (NULL when that is 0) holding the k-split
+ * partial sums, which are added in a fixed order: the result is bit-reproducible. */
+int64_t seg_conv2d_wgrad_workspace_floats(const seg_conv_desc* d, int impl);
+int seg_conv2d_wgrad(const seg_conv_desc* d, const void* dy, const void* x, float* dw_packed, float* workspace, int impl,
                      void* stream);
 
 /* ---- depthwise 3x3 (atrous) convolution: SeparableConv2d.conv1 of the Aligned-Xception backbone
@@ -253,11 +256,12 @@ int seg_eval_metrics_nchw(const float* logits, const int64_t* target, int N, int
  * Also emits the arg-max label map (int32 [N,Ho,Wo], lowest index wins ties) when argmax != NULL. */
 int seg_upsample_ce_fwd(const float* logits_lo, const int64_t* target, int N, int Hi, int Wi, int Ho, int Wo, int C,
                         int align_corners, int64_t ignore_index, double* accum, int32_t* argmax, void* stream);
-/* d(logits_lo) of mean CE: accumulated in fp32 scratch dlo_f32 [N,Hi,Wi,C] (zeroed here), then written as bf16
- * NHWC with pitch lddx (channels C..lddx-1 zero) when dx != NULL; gscale = upstream grad (fp32 scalar on device) */
+/* d(logits_lo) of mean CE: accumulated in 64-bit fixed point in the int64 scratch dlo_fixed [N,Hi,Wi,C] (zeroed here;
+ * order-independent, hence bit-reproducible), converted to fp32 dlo_f32 [N,Hi,Wi,C], then written as bf16 NHWC with pitch
+ * lddx (channels C..lddx-1 zero) when dx != NULL; gscale = upstream grad (fp32 scalar on device) */
 int seg_upsample_ce_bwd(const float* logits_lo, const int64_t* target, int N, int Hi, int Wi, int Ho, int Wo, int C,
                         int align_corners, int64_t ignore_index, const double* accum, const float* gscale,
-                        float* dlo_f32, void* dx, int lddx, void* stream);
+                        float* dlo_f32, void* dlo_fixed, void* dx, int lddx, void* stream);
 /* loss = accum[0]/accum[1] (fp32 scalar) */
 int seg_ce_finalize(const double* accum, float* loss, void* stream);
 

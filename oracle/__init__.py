@@ -1,4 +1,4 @@
-"""CPU oracle for the B200 segmentation hot path — TEST INFRASTRUCTURE, NOT PRODUCT CODE.
+"""CPU oracle for the H100 segmentation hot path — TEST INFRASTRUCTURE, NOT PRODUCT CODE.
 
 A functional (state_dict-keyed) restatement, in plain PyTorch CPU ops, of the reference's hot path:
   models/deeplabv3_plus.py (ResNet trunk surgery :15-63, ASSP :253-297, Decoder :303-330, DeepLab.forward :356-362),

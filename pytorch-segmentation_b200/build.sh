@@ -1,10 +1,10 @@
 #!/bin/bash
-# Builds libseg_b200.so (the C-ABI shared library) for sm_100a, in-tree.
+# Builds libseg_b200.so (the C-ABI shared library) for sm_90a (H100), in-tree.
 set -e
 HERE="$(cd "$(dirname "$0")" && pwd)"
 OUT="$HERE/libseg_b200.so"
 NVCC="${NVCC:-/usr/local/cuda/bin/nvcc}"
-FLAGS="-gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -std=c++17 -Xcompiler -fPIC --expt-relaxed-constexpr"
+FLAGS="-gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 -Xcompiler -fPIC --expt-relaxed-constexpr"
 mkdir -p "$HERE/build"
 pids=()
 for f in seg_api seg_conv_tc seg_conv_simt seg_elementwise seg_loss seg_comm seg_dwconv seg_lovasz seg_data; do
@@ -16,5 +16,5 @@ for f in seg_api seg_conv_tc seg_conv_simt seg_elementwise seg_loss seg_comm seg
   fi
 done
 for p in "${pids[@]}"; do wait $p; done
-$NVCC -shared -gencode arch=compute_100a,code=sm_100a -o "$OUT" "$HERE"/build/*.o -lcudart_static -lpthread -ldl -lrt
+$NVCC -shared -gencode arch=compute_90a,code=sm_90a -o "$OUT" "$HERE"/build/*.o -lcudart_static -lpthread -ldl -lrt
 echo "built $OUT"

@@ -1,5 +1,5 @@
 // seg_api.cu — C-ABI glue: error reporting, device check, launch accounting and the convolution dispatcher
-// (tcgen05 path where the shape allows it, CUDA-core implicit GEMM otherwise).  No CPU fallback anywhere.
+// (wgmma path where the shape allows it, CUDA-core implicit GEMM otherwise).  No CPU fallback anywhere.
 #include <stdarg.h>
 #include "seg_common.cuh"
 #include "seg_sync.cuh"
@@ -21,7 +21,8 @@ bool supported(const seg_conv_desc* d);
 int conv_fwd(const seg_conv_desc* d, const void* x, const void* w, void* y, int y_dtype, const float* bias, float beta,
              double* stats, unsigned* stat_ticket, const SyncDesc* sync, cudaStream_t stream);
 int conv_dgrad(const seg_conv_desc* d, const void* dy, const void* w, void* dx, float beta, cudaStream_t stream);
-int conv_wgrad(const seg_conv_desc* d, const void* dy, const void* x, float* dw, cudaStream_t stream);
+int conv_wgrad(const seg_conv_desc* d, const void* dy, const void* x, float* dw, float* ws, cudaStream_t stream);
+int64_t wgrad_workspace_floats(const seg_conv_desc* d);
 }  // namespace tc
 namespace simt {
 int conv_fwd(const seg_conv_desc* d, const void* x, const void* w, void* y, int y_dtype, const float* bias, float beta,
@@ -63,8 +64,8 @@ int seg_device_ok(void) {
   int major = 0, minor = 0;
   cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
   cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev);
-  if (major != 10) {
-    set_error("seg_b200 kernels are built for sm_100a only; device is sm_%d%d", major, minor);
+  if (major != 9 || minor != 0) {
+    set_error("seg_b200 kernels are built for sm_90a (H100) only; device is sm_%d%d", major, minor);
     return 1;
   }
   return 0;
@@ -95,11 +96,20 @@ int seg_conv2d_dgrad(const seg_conv_desc* d, const void* dy, const void* w_packe
   return simt::conv_dgrad(d, dy, w_packed, dx, beta, ST(stream));
 }
 
-int seg_conv2d_wgrad(const seg_conv_desc* d, const void* dy, const void* x, float* dw_packed, int impl, void* stream) {
+static bool wgrad_on_tc(const seg_conv_desc* d, int impl) {
+  return impl == SEG_IMPL_TC || (impl == SEG_IMPL_AUTO && tc::supported(d) && d->ldy % 8 == 0);
+}
+
+int64_t seg_conv2d_wgrad_workspace_floats(const seg_conv_desc* d, int impl) {
+  if (check_desc(d)) return -1;
+  return wgrad_on_tc(d, impl) ? tc::wgrad_workspace_floats(d) : 0;
+}
+
+int seg_conv2d_wgrad(const seg_conv_desc* d, const void* dy, const void* x, float* dw_packed, float* workspace, int impl,
+                     void* stream) {
   if (check_desc(d)) return 1;
-  const bool tc_ok = tc::supported(d) && d->ldy % 8 == 0;
-  if (impl == SEG_IMPL_TC || (impl == SEG_IMPL_AUTO && tc_ok))
-    return tc::conv_wgrad(d, dy, x, dw_packed, ST(stream));
+  if (wgrad_on_tc(d, impl))
+    return tc::conv_wgrad(d, dy, x, dw_packed, workspace, ST(stream));
   return simt::conv_wgrad(d, dy, x, dw_packed, ST(stream));
 }
 

@@ -1,4 +1,4 @@
-// seg_common.cuh — shared helpers for the sm_100a segmentation kernels (error plumbing, bf16 vector helpers,
+// seg_common.cuh — shared helpers for the sm_90a segmentation kernels (error plumbing, bf16 vector helpers,
 // launch accounting).  Internal header; the public C ABI is include/seg_b200.h.
 #pragma once
 #include <cuda_runtime.h>
@@ -84,9 +84,8 @@ __device__ __forceinline__ float hash_uniform(uint64_t seed, uint64_t idx) {
 // scheduled, and run their prologue, while the previous kernel in the stream drains.  Every such kernel executes
 // pdl_wait() before its first global-memory access (it returns once the previous grid has COMPLETED and flushed), so the
 // data flow is unchanged; pdl_trigger() at the top lets the next kernel do the same with this one.  Both instructions
-// are no-ops in a kernel launched the ordinary way.  MEASURED (profiles/pdl_ab_r01.txt): inside the CUDA-graph replay of
-// the step the launch gaps are already hidden — PDL gave 24.54 ms vs 24.24 ms without (early trigger: 25.43 ms) — so it
-// is OFF by default; SEG_PDL=1 in the environment turns it on.
+// are no-ops in a kernel launched the ordinary way.  Inside the CUDA-graph replay of the step the launch gaps are already
+// hidden, so it is OFF by default; SEG_PDL=1 in the environment turns it on.
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
@@ -121,7 +120,7 @@ inline int num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return n;
 }

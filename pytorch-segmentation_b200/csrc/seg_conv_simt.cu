@@ -1,5 +1,5 @@
 // seg_conv_simt.cu — CUDA-core implicit-GEMM convolution (forward / dgrad / wgrad) for every shape the
-// tcgen05 path does not take (stride-2 data gradients, channel counts that are not a multiple of 8) and as an
+// wgmma path does not take (stride-2 data gradients, channel counts that are not a multiple of 8) and as an
 // on-device cross-check of the tensor-core kernels.  64x64 tiles, 16-deep k-slices staged in shared memory,
 // 256 threads x (4x4) fp32 accumulators.  Same semantics as seg_conv_tc.cu (reference: nn.Conv2d call sites listed there).
 #include "seg_common.cuh"
@@ -188,7 +188,7 @@ int conv_fwd(const seg_conv_desc* d, const void* x, const void* w, void* y, int 
   dim3 grid((unsigned)ceil_div64(p.M, TM), (unsigned)ceil_div(p.Ncols, TN), 1);
   igemm_simt<FWD><<<grid, 256, 0, stream>>>(p);
   if (check_launch("igemm_simt<FWD>")) return 1;
-  // statistics of the output AS STORED, by the deterministic column reduction (same workspace contract as the tcgen05 path)
+  // statistics of the output AS STORED, by the deterministic column reduction (same workspace contract as the wgmma path)
   if (stats) return bn_stats_launch(y, p.M, d->K, d->ldy, stats, sync, stat_ticket, stream);
   return 0;
 }

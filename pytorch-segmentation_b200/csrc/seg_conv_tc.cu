@@ -1,21 +1,21 @@
-// seg_conv_tc.cu — tcgen05 + TMA implicit-GEMM convolution for sm_100a (forward, data-gradient, weight-gradient).
+// seg_conv_tc.cu — wgmma + TMA implicit-GEMM convolution for sm_90a (forward, data-gradient, weight-gradient).
 //
 // Replaces what the reference dispatches to cuDNN for every nn.Conv2d on the hot path (dense 3x3 / dilated 3x3 /
 // 1x1; SURVEY.md §2.3): models/deeplabv3_plus.py:256 (ASPP d=6/12/18), :312-315 (decoder 3x3), torchvision
 // Bottleneck conv1/conv2/conv3 (layer4 conv2 dilated at deeplabv3_plus.py:47-53), models/resnet.py:43-48.
 //
-// One CTA computes a 128 x BN fp32 tile held in TMEM.  Warp roles (192 threads):
-//   warp 0  : TMA producer.  The activation operand is fetched with an IM2COL-mode tensor map: one instruction
-//             brings 128 output pixels x 64 channels of one filter tap (tap displacement passed as the im2col
-//             offset, padding = the bounding-box corners, out-of-image taps zero-filled by the TMA unit) straight into
-//             the 128B-swizzled K-major layout tcgen05 consumes — the im2col gather happens in the copy engine, never
-//             in HBM.  Weights come through a tiled 2-D map over the packed [tap][K][C] matrix.
-//   warp 1  : TMEM allocator + single-thread tcgen05.mma issuer (4 x K=16 per 64-wide k-block).
-//   warps 2-5: epilogue; tcgen05.ld 32 lanes x 32 columns -> optional bias -> staged through (now idle) pipeline
-//             shared memory with an XOR swizzle -> fully coalesced 16-byte global stores (optionally beta-accumulate,
-//             optionally onto a strided sub-grid of the output) ; per-channel sum / sum-of-squares of the fp32
-//             accumulators (BatchNorm statistics) reduced per warp by a 31-shuffle transpose-reduce, then per CTA in
-//             shared memory, one atomicAdd per channel per CTA.
+// One CTA computes a 128 x BN fp32 tile held in registers.  Warpgroup roles (384 threads):
+//   warpgroup 0  : TMA producer (one thread).  The activation operand is fetched with an IM2COL-mode tensor map: one
+//                  instruction brings 128 output pixels x 64 channels of one filter tap (tap displacement passed as the
+//                  im2col offset, padding = the bounding-box corners, out-of-image taps zero-filled by the TMA unit)
+//                  straight into the 128B-swizzled K-major layout wgmma consumes — the im2col gather happens in the copy
+//                  engine, never in HBM.  Weights come through a tiled 2-D map over the packed [tap][K][C] matrix.
+//   warpgroups 1-2: wgmma consumers; warpgroup 1 + c owns rows 64c..64c+63 of the tile (4 x m64nBNk16 per 64-wide
+//                  k-block, one group kept in flight), then the epilogue: accumulators (+ bias) -> XOR-swizzled staging
+//                  tile in the (now idle) pipeline shared memory -> per-channel sum / sum of squares of the values as
+//                  stored (BatchNorm statistics, fixed order inside the CTA, one fp64 atomic per channel per CTA) ->
+//                  fully coalesced 16-byte global stores (optionally beta-accumulate, optionally onto a strided
+//                  sub-grid of the output).
 // Operand-major variants of the same pipeline:
 //   KK (fprop) : A = activations (K-major),  B = weights  [tap*K + k][c]   (K-major)
 //   KM (dgrad) : A = dY im2col  (K-major),  B = weights  [tap*K + k][c]   (MN-major: c contiguous).  Stride 1: taps
@@ -23,7 +23,8 @@
 //                gather over dY with only the taps whose parity matches, written to its strided sub-grid of dX —
 //                no wasted MACs on inserted zeros.
 //   MM (wgrad) : A = dY [pixel][k] (MN-major), B = X im2col [pixel][c] (MN-major), contraction over pixels,
-//                split-K over pixel blocks with fp32 atomics into dW[tap][k][c].
+//                split-K over pixel blocks: each split stores its partial tile to a workspace [split][tap][k][c] and a
+//                second kernel adds the splits to dW[tap][k][c] in split order — bit-reproducible, unlike atomics.
 #include <cuda.h>
 #include <mutex>
 #include <stdlib.h>
@@ -40,7 +41,8 @@ constexpr int BM = 128;
 constexpr int BK = 64;  // elements per k-block = 128 bytes of bf16
 constexpr int A_BYTES = BM * 128;
 constexpr int KIND_KK = 0, KIND_KM = 1, KIND_MM = 2;
-constexpr int NTHREADS = 192;
+constexpr int NTHREADS = 384;
+constexpr int NCONS = 256;  // consumer threads (warpgroups 1 and 2)
 constexpr int MAXT = 49;
 
 struct TcParams {
@@ -73,16 +75,20 @@ struct TcParams {
   int kblocks_total, kblocks_per_split;
   float* dw;
   int dw_K, dw_C;
-  CUtensorMap mapC;  // v2 TMA epilogue: the destination as a 2-D map with [32 rows][64 columns] boxes
-  int dbg;  // tuning experiments only (env SEG_TC_DBG): 1 skip global stores/loads, 2 skip statistics, 4 skip TMEM drain
+  float* ws;  // split-K partials [split][tap][dw_K][dw_C]; null with one split (the tile is added to dW directly)
 };
 
-template <int BN, int STAGES_>
+// Pipeline stages per tile width: one CTA per SM (384 threads, up to 128 accumulator registers per consumer thread), so
+// the ring takes most of the 227 KB; the fp32 staging tile of the epilogue (128 x BN x 4 B) reuses it.
+template <int BN>
 struct Cfg {
   static constexpr int B_BYTES = BN * 128;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGES = STAGES_;
-  static constexpr int SMEM = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+  static constexpr int STAGES = BN == 64 ? 6 : (BN == 128 ? 5 : 4);
+  static constexpr int STAT_BYTES = 2 * 2 * BN * 4;  // [row group][sum, sum of squares][column] fp32
+  static constexpr int SMEM = STAGES * STAGE_BYTES + STAT_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+  static_assert(STAGES * STAGE_BYTES >= BM * BN * 4, "staging tile must fit in the pipeline ring");
+  static_assert(SMEM <= 227 * 1024, "shared memory per block");
 };
 
 __device__ __forceinline__ void row_to_coords(int m, int PQ, int Q, int stride, int lower_h, int lower_w, int& n, int& h,
@@ -95,24 +101,29 @@ __device__ __forceinline__ void row_to_coords(int m, int PQ, int Q, int stride, 
   w = lower_w + qq * stride;
 }
 
-template <int BN, int STAGES, int KIND>
-__global__ void __launch_bounds__(NTHREADS) conv_gemm_tc(const __grid_constant__ TcParams p) {
-  using C = Cfg<BN, STAGES>;
+template <int BN, int TA, int TB>
+__device__ __forceinline__ void wgmma_tile(float* acc, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  if constexpr (BN == 64) wgmma_m64n64k16<TA, TB>(acc, adesc, bdesc, accumulate);
+  else if constexpr (BN == 128) wgmma_m64n128k16<TA, TB>(acc, adesc, bdesc, accumulate);
+  else wgmma_m64n256k16<TA, TB>(acc, adesc, bdesc, accumulate);
+}
+
+__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+
+template <int BN, int KIND>
+__global__ void __launch_bounds__(NTHREADS, 1) conv_gemm_tc(const __grid_constant__ TcParams p) {
+  using C = Cfg<BN>;
+  constexpr int STAGES = C::STAGES;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
   const uint32_t smem0 = (raw_addr + 1023u) & ~1023u;  // 1024-B alignment for SWIZZLE_128B atoms
   uint8_t* smem_gen = smem_raw + (smem0 - raw_addr);
-  const uint32_t bar0 = smem0 + C::STAGES * C::STAGE_BYTES;
-  // barrier block: full[STAGES], empty[STAGES], tmem_full, then tmem base pointer
+  float* stat_sm = reinterpret_cast<float*>(smem_gen + STAGES * C::STAGE_BYTES);
+  const uint32_t bar0 = smem0 + STAGES * C::STAGE_BYTES + C::STAT_BYTES;
   auto full_bar = [&](int s) { return bar0 + 8u * s; };
-  auto empty_bar = [&](int s) { return bar0 + 8u * (C::STAGES + s); };
-  const uint32_t tmem_full_bar = bar0 + 8u * (2 * C::STAGES);
-  volatile uint32_t* tmem_ptr_gen =
-      reinterpret_cast<volatile uint32_t*>(smem_gen + C::STAGES * C::STAGE_BYTES + 8 * (2 * C::STAGES + 1));
-  const uint32_t tmem_ptr_addr = bar0 + 8u * (2 * C::STAGES + 1);
+  auto empty_bar = [&](int s) { return bar0 + 8u * (STAGES + s); };
+  volatile int* flag_sm = reinterpret_cast<volatile int*>(smem_gen + STAGES * C::STAGE_BYTES + C::STAT_BYTES + 8 * 2 * STAGES);
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
   const int m0 = blockIdx.x * BM;
   const int n0 = blockIdx.y * BN;
 
@@ -128,29 +139,21 @@ __global__ void __launch_bounds__(NTHREADS) conv_gemm_tc(const __grid_constant__
     num_iters = p.taps * p.kchunks;
   }
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&p.mapA);
     prefetch_tmap(&p.mapB);
-    for (int s = 0; s < C::STAGES; ++s) {
+    for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
+      mbar_init(empty_bar(s), 8);  // one arrival per consumer warp
     }
-    mbar_init(tmem_full_bar, 1);
     fence_mbar_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_ptr_addr, BN);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_gen;
   pdl_wait();  // setup above overlapped the previous kernel's tail; global memory is touched only from here on
 
-  if (warp == 0) {
+  if (threadIdx.x < 128) {
     // =============================== TMA producer ===============================
-    if (lane == 0 && num_iters > 0) {
+    if (threadIdx.x == 0 && num_iters > 0) {
       if (KIND != KIND_MM) {
         int n_img = 0, h0 = 0, w0 = 0;
         if (p.x_im2col) row_to_coords(m0, p.PQ, p.Q, p.stride, p.lower_h, p.lower_w, n_img, h0, w0);
@@ -159,9 +162,9 @@ __global__ void __launch_bounds__(NTHREADS) conv_gemm_tc(const __grid_constant__
           const int wtap = p.tap_wt[tap];
           const uint16_t oh = (uint16_t)p.tap_oh[tap], ow = (uint16_t)p.tap_ow[tap];
           for (int kc = 0; kc < p.kchunks; ++kc, ++it) {
-            const int st = it % C::STAGES;
-            const uint32_t ph = (it / C::STAGES) & 1;
-            mbar_wait(empty_bar(st), ph ^ 1u);
+            const int st = it % STAGES;
+            const uint32_t ph = (it / STAGES) & 1;
+            mbar_wait_nocall(empty_bar(st), ph ^ 1u);
             const uint32_t a_dst = smem0 + st * C::STAGE_BYTES;
             const uint32_t b_dst = a_dst + A_BYTES;
             mbar_arrive_expect_tx(full_bar(st), C::STAGE_BYTES);
@@ -182,9 +185,9 @@ __global__ void __launch_bounds__(NTHREADS) conv_gemm_tc(const __grid_constant__
         const uint16_t oh = (uint16_t)p.tap_oh[tap_mm], ow = (uint16_t)p.tap_ow[tap_mm];
         int it = 0;
         for (int kb = kb_begin; kb < kb_end; ++kb, ++it) {
-          const int st = it % C::STAGES;
-          const uint32_t ph = (it / C::STAGES) & 1;
-          mbar_wait(empty_bar(st), ph ^ 1u);
+          const int st = it % STAGES;
+          const uint32_t ph = (it / STAGES) & 1;
+          mbar_wait_nocall(empty_bar(st), ph ^ 1u);
           const uint32_t a_dst = smem0 + st * C::STAGE_BYTES;
           const uint32_t b_dst = a_dst + A_BYTES;
           const int pix0 = kb * BK;
@@ -204,224 +207,205 @@ __global__ void __launch_bounds__(NTHREADS) conv_gemm_tc(const __grid_constant__
         }
       }
     }
-  } else if (warp == 1) {
-    // =============================== MMA issuer ===============================
-    if (lane == 0 && num_iters > 0) {
-      constexpr int A_MN = (KIND == KIND_MM) ? 1 : 0;
-      constexpr int B_MN = (KIND == KIND_KK) ? 0 : 1;
-      constexpr uint32_t idesc = make_idesc_bf16(BN, A_MN, B_MN);
-      for (int it = 0; it < num_iters; ++it) {
-        const int st = it % C::STAGES;
-        const uint32_t ph = (it / C::STAGES) & 1;
-        mbar_wait(full_bar(st), ph);
-        tc_fence_after();
-        const uint32_t a_addr = smem0 + st * C::STAGE_BYTES;
-        const uint32_t b_addr = a_addr + A_BYTES;
-        // K-major: 8-row atoms 1024 B apart, K advance = 32 B inside the swizzle atom.
-        // MN-major: 64-wide MN blocks one box (8192 B) apart, 8-row K groups 1024 B apart, K advance = 16 rows.
-        const uint64_t adesc0 = A_MN ? make_smem_desc_sw128(a_addr, 8192, 1024) : make_smem_desc_sw128(a_addr, 16, 1024);
-        const uint64_t bdesc0 = B_MN ? make_smem_desc_sw128(b_addr, 8192, 1024) : make_smem_desc_sw128(b_addr, 16, 1024);
-#pragma unroll
-        for (int k = 0; k < BK / 16; ++k) {
-          const uint64_t adesc = adesc0 + (uint64_t)(A_MN ? (k * 2048 >> 4) : (k * 32 >> 4));
-          const uint64_t bdesc = bdesc0 + (uint64_t)(B_MN ? (k * 2048 >> 4) : (k * 32 >> 4));
-          umma_bf16(tmem_base, adesc, bdesc, idesc, (it > 0 || k > 0) ? 1u : 0u);
-        }
-        umma_commit(empty_bar(st));  // frees the smem slot when these MMAs retire
-      }
-      umma_commit(tmem_full_bar);  // accumulator complete
-      pdl_trigger();               // loads and MMAs of this CTA are issued: dependents may be scheduled
-    }
-  } else {
-    // =============================== epilogue (warps 2..5) ===============================
-    const int lg = warp & 3;  // TMEM lane group this warp may access
-    const int trow = lg * 32 + lane;
-    const int row = m0 + trow;
-    if (num_iters > 0) {
-      mbar_wait(tmem_full_bar, 0);
-      tc_fence_after();
-    }
-    float v[32];
-    if (KIND == KIND_MM) {
-      for (int ch = 0; ch < BN / 32; ++ch) {
-        const int col0 = n0 + ch * 32;
-        if (col0 >= p.Ncols) break;  // warp-uniform
-        if (num_iters > 0) {
-          tmem_ld_32x32(tmem_base + ((uint32_t)(lg * 32) << 16) + (uint32_t)(ch * 32), v);
-          tmem_ld_wait();
-          if (row < p.M) {
-            float* dst = p.dw + ((size_t)tap_mm * p.dw_K + row) * p.dw_C + col0;
-            if (col0 + 32 <= p.Ncols && ((reinterpret_cast<uintptr_t>(dst) & 15) == 0)) {
-              // 128-bit vector reductions: 8 RED.F32x4 instead of 32 scalar atomics per thread
-#pragma unroll
-              for (int i = 0; i < 32; i += 4)
-                asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst + i), "f"(v[i]), "f"(v[i + 1]),
-                             "f"(v[i + 2]), "f"(v[i + 3])
-                             : "memory");
-            } else {
-#pragma unroll
-              for (int i = 0; i < 32; ++i)
-                if (col0 + i < p.Ncols) atomicAdd(dst + i, v[i]);
-            }
-          }
-        }
-      }
-    } else {
-      // -------- phase 1: TMEM -> registers -> (bias, stats) -> swizzled staging tile in the idle pipeline smem ------
-      const bool out_bf16 = (p.out_dtype == SEG_DT_BF16);
-      const int esize = out_bf16 ? 2 : 4;
-      const int CPR = BN * esize / 16;  // 16-byte chunks per staged row
-      const int swz = (CPR >= 32 ? 31 : CPR - 1);
-      uint8_t* stage = smem_gen;  // 128 rows x BN*esize bytes
-      float* stat_sm = reinterpret_cast<float*>(smem_gen + BM * BN * esize);  // [4 warps][2][BN], right after the staging tile
-      const bool row_ok = row < p.M;
-      for (int ch = 0; ch < BN / 32; ++ch) {
-        const int col0 = n0 + ch * 32;
-        if (col0 >= p.Ncols) break;  // warp-uniform
-        if (num_iters > 0) {
-          tmem_ld_32x32(tmem_base + ((uint32_t)(lg * 32) << 16) + (uint32_t)(ch * 32), v);
-          tmem_ld_wait();
-        } else {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) v[i] = 0.f;
-        }
-        if (p.bias) {
-#pragma unroll
-          for (int i = 0; i < 32; ++i)
-            if (col0 + i < p.Ncols) v[i] += __ldg(p.bias + col0 + i);
-        }
-        if (out_bf16) {
-#pragma unroll
-          for (int g = 0; g < 4; ++g) {
-            const int c16 = ch * 4 + g;
-            *reinterpret_cast<bf16x8*>(stage + (size_t)trow * (BN * 2) + ((c16 ^ (trow & swz)) << 4)) = pack8(v + g * 8);
-          }
-        } else {
-#pragma unroll
-          for (int g = 0; g < 8; ++g) {
-            const int c16 = ch * 8 + g;
-            *reinterpret_cast<float4*>(stage + (size_t)trow * (BN * 4) + ((c16 ^ (trow & swz)) << 4)) =
-                make_float4(v[g * 4], v[g * 4 + 1], v[g * 4 + 2], v[g * 4 + 3]);
-          }
-        }
-        if (p.stats) {
-          // column sums over this warp's 32 rows: transpose-reduce, lane i ends with column (col0+i)
-          float s1[32], s2[32];
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            // statistics of the value AS STORED (bf16-rounded) — exactly what bn_apply normalises, and what the
-            // persistent kernel sums from its staged tile
-            const float x = row_ok ? (out_bf16 ? bf2f(f2bf(v[i])) : v[i]) : 0.f;
-            s1[i] = x;
-            s2[i] = x * x;
-          }
-#pragma unroll
-          for (int off = 16; off >= 1; off >>= 1) {
-            const bool up = (lane & off) != 0;
-#pragma unroll
-            for (int j = 0; j < off; ++j) {
-              const float send1 = up ? s1[j] : s1[j + off];
-              const float keep1 = up ? s1[j + off] : s1[j];
-              s1[j] = keep1 + __shfl_xor_sync(0xffffffffu, send1, off);
-              const float send2 = up ? s2[j] : s2[j + off];
-              const float keep2 = up ? s2[j + off] : s2[j];
-              s2[j] = keep2 + __shfl_xor_sync(0xffffffffu, send2, off);
-            }
-          }
-          stat_sm[(lg * 2 + 0) * BN + ch * 32 + lane] = s1[0];
-          stat_sm[(lg * 2 + 1) * BN + ch * 32 + lane] = s2[0];
-        }
-      }
-      __syncwarp();
-      // -------- phase 2: each warp streams ITS 32 rows out with coalesced 16-byte stores --------
-      const int ncols_tile = min(BN, p.Ncols - n0);           // valid columns of this tile
-      const int nchunks = (ncols_tile * esize + 15) >> 4;      // 16-byte chunks that hold valid data
-      const bool vec_ok = ((p.ldo * esize) & 15) == 0 && ((reinterpret_cast<uintptr_t>(p.out) + (size_t)n0 * esize) & 15) == 0;
-      for (int idx = lane; idx < 32 * CPR; idx += 32) {
-        const int rr = idx / CPR;
-        const int c16 = idx - rr * CPR;
-        if (c16 >= nchunks) continue;
-        const int tr = lg * 32 + rr;
-        const int grow = m0 + tr;
-        if (grow >= p.M) continue;
-        long long pixel = grow;
-        if (p.out_strided) {
-          const int n = grow / p.PQ;
-          const int rem = grow - n * p.PQ;
-          const int i = rem / p.Q, j = rem - i * p.Q;
-          pixel = ((long long)n * p.out_H + (i * p.osy + p.opy)) * p.out_W + (j * p.osx + p.opx);
-        }
-        const uint8_t* src = stage + (size_t)tr * (BN * esize) + ((c16 ^ (tr & swz)) << 4);
-        uint8_t* dst = reinterpret_cast<uint8_t*>(p.out) + ((size_t)pixel * p.ldo + n0) * esize + ((size_t)c16 << 4);
-        const int first_col = (c16 << 4) / esize;
-        const bool full = first_col + 16 / esize <= ncols_tile;
-        if (out_bf16) {
-          bf16x8 val = *reinterpret_cast<const bf16x8*>(src);
-          if (vec_ok && full) {
-            if (p.beta != 0.f) {
-              float a[8], b[8];
-              unpack8(val, a);
-              unpack8(*reinterpret_cast<const bf16x8*>(dst), b);
-#pragma unroll
-              for (int k = 0; k < 8; ++k) a[k] += p.beta * b[k];
-              val = pack8(a);
-            }
-            *reinterpret_cast<bf16x8*>(dst) = val;
-          } else {
-            float a[8];
-            unpack8(val, a);
-            __nv_bfloat16* d = reinterpret_cast<__nv_bfloat16*>(dst);
-            for (int k = 0; k < 8; ++k)
-              if (first_col + k < ncols_tile) {
-                float o = a[k];
-                if (p.beta != 0.f) o += p.beta * bf2f(d[k]);
-                d[k] = f2bf(o);
-              }
-          }
-        } else {
-          const float4 val = *reinterpret_cast<const float4*>(src);
-          const float a[4] = {val.x, val.y, val.z, val.w};
-          float* d = reinterpret_cast<float*>(dst);
-          if (vec_ok && full && p.beta == 0.f) {
-            *reinterpret_cast<float4*>(d) = val;
-          } else {
-            for (int k = 0; k < 4; ++k)
-              if (first_col + k < ncols_tile) d[k] = (p.beta != 0.f) ? a[k] + p.beta * d[k] : a[k];
-          }
-        }
-      }
-      // -------- phase 3: BN statistics: this CTA's column sums (fixed order inside the CTA) are added to the layer's totals
-      //          with fp64 atomics.  Each contribution is an fp32 value, so the fp64 sum of the <= few thousand partials of a
-      //          channel is EXACT (no rounding at all) whenever their exponents span less than 2^17 — then the order of the
-      //          atomics cannot matter and the statistics are bit-reproducible; round 1's fp32 atomics were not, and the
-      //          batch-2 image-pooling BatchNorm amplified that into 3-5 % logit differences between runs.  (Beyond that
-      //          span the order can move the fp64 sum by one fp64 ulp — invisible after the rounding to fp32 below.) --------
-      if (p.stats) {
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        const int e = (warp - 2) * 32 + lane;
-        for (int c = e; c < ncols_tile; c += 128) {
-          float a = 0.f, b = 0.f;
-#pragma unroll
-          for (int w = 0; w < 4; ++w) {
-            a += stat_sm[(w * 2 + 0) * BN + c];
-            b += stat_sm[(w * 2 + 1) * BN + c];
-          }
-          atomicAdd(p.stats + n0 + c, (double)a);
-          atomicAdd(p.stats + p.Ncols + n0 + c, (double)b);
-        }
-        if (p.sync.world > 0) {
-          volatile int* flag = reinterpret_cast<volatile int*>(smem_gen + C::STAGES * C::STAGE_BYTES + 128);
-          sync_push_when_last(p.sync, p.stats, 2 * p.Ncols, p.stat_ticket, gridDim.x * gridDim.y, e, 128,
-                              [] { asm volatile("bar.sync 1, 128;" ::: "memory"); }, flag);
-        }
-      }
-    }
-    tc_fence_before();
+    return;
   }
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, BN);
+
+  // =============================== wgmma consumers ===============================
+  if (KIND == KIND_MM && num_iters == 0) return;  // an empty split adds nothing (uniform across the consumers)
+  const int ctid = threadIdx.x - 128;  // 0..255
+  const int cw = ctid >> 7;            // consumer warpgroup: rows 64*cw.. of the tile
+  const int warp = (ctid >> 5) & 3, lane = ctid & 31;
+  float acc[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  {
+    constexpr int TA = (KIND == KIND_MM) ? 1 : 0;
+    constexpr int TB = (KIND == KIND_KK) ? 0 : 1;
+    for (int it = 0; it < num_iters; ++it) {
+      const int st = it % STAGES;
+      mbar_wait_nocall(full_bar(st), (it / STAGES) & 1);
+      const uint32_t a_addr = smem0 + st * C::STAGE_BYTES + cw * 8192;  // K-major: 64 rows x 128 B; MN-major: box cw
+      const uint32_t b_addr = smem0 + st * C::STAGE_BYTES + A_BYTES;
+      // K-major: 8-row atoms 1024 B apart, K advance = 32 B inside the swizzle atom.
+      // MN-major: 64-wide MN blocks one box (8192 B) apart, 8-row K groups 1024 B apart, K advance = 16 rows.
+      const uint64_t adesc0 = make_smem_desc_sw128(a_addr, TA ? 8192 : 16, 1024);
+      const uint64_t bdesc0 = make_smem_desc_sw128(b_addr, TB ? 8192 : 16, 1024);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < BK / 16; ++k) {
+        const uint64_t adesc = adesc0 + (uint64_t)(TA ? (k * 2048 >> 4) : (k * 32 >> 4));
+        const uint64_t bdesc = bdesc0 + (uint64_t)(TB ? (k * 2048 >> 4) : (k * 32 >> 4));
+        wgmma_tile<BN, TA, TB>(acc, adesc, bdesc, 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();  // the previous k-block's MMAs have retired: its stage goes back to the producer
+      __syncwarp();
+      if (it > 0 && lane == 0) mbar_arrive(empty_bar((it - 1) % STAGES));
+    }
+    wgmma_wait<0>();
+  }
+  consumer_sync();  // both warpgroups are done reading the ring: it becomes the staging tile
+
+  // -------- phase 1: registers -> (bias) -> swizzled staging tile [128 rows][BN * esize bytes] --------
+  const bool out_f32 = (KIND == KIND_MM) || p.out_dtype != SEG_DT_BF16;
+  const int esize = out_f32 ? 4 : 2;
+  const int CPR = BN * esize / 16;  // 16-byte chunks per staged row
+  const int swz = (CPR >= 32 ? 31 : CPR - 1);
+  uint8_t* stage = smem_gen;
+  const int ncols_tile = min(BN, p.Ncols - n0);
+  {
+    const int r0 = cw * 64 + warp * 16 + (lane >> 2);
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      const int col = j * 8 + 2 * (lane & 3);
+      float b0 = 0.f, b1 = 0.f;
+      if (KIND != KIND_MM && p.bias) {
+        if (col < ncols_tile) b0 = __ldg(p.bias + n0 + col);
+        if (col + 1 < ncols_tile) b1 = __ldg(p.bias + n0 + col + 1);
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int r = r0 + 8 * h;
+        const float x0 = acc[4 * j + 2 * h] + b0, x1 = acc[4 * j + 2 * h + 1] + b1;
+        const int byte = col * esize;
+        uint8_t* dst = stage + (size_t)r * (BN * esize) + ((((byte >> 4) ^ (r & swz))) << 4) + (byte & 15);
+        if (out_f32)
+          *reinterpret_cast<float2*>(dst) = make_float2(x0, x1);
+        else
+          *reinterpret_cast<__nv_bfloat162*>(dst) = __floats2bfloat162_rn(x0, x1);
+      }
+    }
+  }
+  consumer_sync();
+
+  if (KIND == KIND_MM) {
+    // -------- wgrad tile: with one split, added to dW[tap][k][c] (once per element: order-free); with several, stored
+    //          to this split's slice of the workspace for the fixed-order reduction --------
+    float* base = p.ws ? p.ws + (size_t)(blockIdx.z / p.taps) * p.taps * p.dw_K * p.dw_C : p.dw;
+    for (int idx = ctid; idx < BM * CPR; idx += NCONS) {
+      const int tr = idx / CPR, c16 = idx - tr * CPR;
+      const int row = m0 + tr, col0 = c16 * 4;
+      if (row >= p.M || col0 >= ncols_tile) continue;
+      const float4 v = *reinterpret_cast<const float4*>(stage + (size_t)tr * (BN * 4) + ((c16 ^ (tr & swz)) << 4));
+      float* dst = base + ((size_t)tap_mm * p.dw_K + row) * p.dw_C + n0 + col0;
+      const bool vec = col0 + 4 <= ncols_tile && ((reinterpret_cast<uintptr_t>(dst) & 15) == 0);
+      const float a[4] = {v.x, v.y, v.z, v.w};
+      if (p.ws) {
+        if (vec)
+          *reinterpret_cast<float4*>(dst) = v;
+        else
+          for (int i = 0; i < 4; ++i)
+            if (col0 + i < ncols_tile) dst[i] = a[i];
+      } else if (vec) {
+        asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w)
+                     : "memory");
+      } else {
+        for (int i = 0; i < 4; ++i)
+          if (col0 + i < ncols_tile) atomicAdd(dst + i, a[i]);
+      }
+    }
+    return;
+  }
+
+  // -------- phase 2: BN statistics of the tile AS STORED (bf16-rounded for bf16 outputs — exactly what bn_apply
+  //          normalises): NG row groups of 128/NG rows per column, summed in a fixed order --------
+  if (p.stats) {
+    constexpr int NG = NCONS / BN, RPG = BM / NG;
+    const int c = ctid % BN, g = ctid / BN;
+    const int rend = min((g + 1) * RPG, p.M - m0);
+    float s1 = 0.f, s2 = 0.f;
+    const int byte = c * esize;
+    for (int r = g * RPG; r < rend; ++r) {
+      const uint8_t* src = stage + (size_t)r * (BN * esize) + ((((byte >> 4) ^ (r & swz))) << 4) + (byte & 15);
+      const float x = out_f32 ? *reinterpret_cast<const float*>(src) : bf2f(*reinterpret_cast<const __nv_bfloat16*>(src));
+      s1 += x;
+      s2 = fmaf(x, x, s2);
+    }
+    stat_sm[(g * 2 + 0) * BN + c] = s1;
+    stat_sm[(g * 2 + 1) * BN + c] = s2;
+  }
+
+  // -------- phase 3: the consumers stream the tile out with coalesced 16-byte stores --------
+  {
+    const int nchunks = (ncols_tile * esize + 15) >> 4;  // 16-byte chunks that hold valid data
+    const bool vec_ok = ((p.ldo * esize) & 15) == 0 && ((reinterpret_cast<uintptr_t>(p.out) + (size_t)n0 * esize) & 15) == 0;
+    for (int idx = ctid; idx < BM * CPR; idx += NCONS) {
+      const int tr = idx / CPR;
+      const int c16 = idx - tr * CPR;
+      if (c16 >= nchunks) continue;
+      const int grow = m0 + tr;
+      if (grow >= p.M) continue;
+      long long pixel = grow;
+      if (p.out_strided) {
+        const int n = grow / p.PQ;
+        const int rem = grow - n * p.PQ;
+        const int i = rem / p.Q, j = rem - i * p.Q;
+        pixel = ((long long)n * p.out_H + (i * p.osy + p.opy)) * p.out_W + (j * p.osx + p.opx);
+      }
+      const uint8_t* src = stage + (size_t)tr * (BN * esize) + ((c16 ^ (tr & swz)) << 4);
+      uint8_t* dst = reinterpret_cast<uint8_t*>(p.out) + ((size_t)pixel * p.ldo + n0) * esize + ((size_t)c16 << 4);
+      const int first_col = (c16 << 4) / esize;
+      const bool full = first_col + 16 / esize <= ncols_tile;
+      if (!out_f32) {
+        bf16x8 val = *reinterpret_cast<const bf16x8*>(src);
+        if (vec_ok && full) {
+          if (p.beta != 0.f) {
+            float a[8], b[8];
+            unpack8(val, a);
+            unpack8(*reinterpret_cast<const bf16x8*>(dst), b);
+#pragma unroll
+            for (int k = 0; k < 8; ++k) a[k] += p.beta * b[k];
+            val = pack8(a);
+          }
+          *reinterpret_cast<bf16x8*>(dst) = val;
+        } else {
+          float a[8];
+          unpack8(val, a);
+          __nv_bfloat16* d = reinterpret_cast<__nv_bfloat16*>(dst);
+          for (int k = 0; k < 8; ++k)
+            if (first_col + k < ncols_tile) {
+              float o = a[k];
+              if (p.beta != 0.f) o += p.beta * bf2f(d[k]);
+              d[k] = f2bf(o);
+            }
+        }
+      } else {
+        const float4 val = *reinterpret_cast<const float4*>(src);
+        const float a[4] = {val.x, val.y, val.z, val.w};
+        float* d = reinterpret_cast<float*>(dst);
+        if (vec_ok && full && p.beta == 0.f) {
+          *reinterpret_cast<float4*>(d) = val;
+        } else {
+          for (int k = 0; k < 4; ++k)
+            if (first_col + k < ncols_tile) d[k] = (p.beta != 0.f) ? a[k] + p.beta * d[k] : a[k];
+        }
+      }
+    }
+  }
+  if (num_iters > 0 && ctid == 0) pdl_trigger();
+
+  // -------- phase 4: this CTA's column sums are added to the layer's totals with fp64 atomics.  Each contribution is an
+  //          fp32 value, so the fp64 sum of the <= few thousand partials of a channel is EXACT (no rounding at all) whenever
+  //          their exponents span less than 2^17 — then the order of the atomics cannot matter and the statistics are
+  //          bit-reproducible (fp32 atomics were not, and the batch-2 image-pooling BatchNorm amplified that into 3-5 %
+  //          logit differences between runs).  (Beyond that span the order can move the fp64 sum by one fp64 ulp —
+  //          invisible after the rounding to fp32.) --------
+  if (p.stats) {
+    constexpr int NG = NCONS / BN;
+    consumer_sync();
+    for (int c = ctid; c < ncols_tile; c += NCONS) {
+      float a = 0.f, b = 0.f;
+#pragma unroll
+      for (int g = 0; g < NG; ++g) {
+        a += stat_sm[(g * 2 + 0) * BN + c];
+        b += stat_sm[(g * 2 + 1) * BN + c];
+      }
+      atomicAdd(p.stats + n0 + c, (double)a);
+      atomicAdd(p.stats + p.Ncols + n0 + c, (double)b);
+    }
+    if (p.sync.world > 0)
+      sync_push_when_last<false>(p.sync, p.stats, 2 * p.Ncols, p.stat_ticket, gridDim.x * gridDim.y, ctid, NCONS,
+                          [] { asm volatile("bar.sync 1, 256;" ::: "memory"); }, flag_sm);
   }
 }
 
@@ -501,101 +485,37 @@ static int make_map_im2col(CUtensorMap* m, const void* ptr, int N, int H, int W,
   return 0;
 }
 
-template <int BN, int STAGES, int KIND>
+template <int BN, int KIND>
 static int launch_kernel(const TcParams& p, dim3 grid, cudaStream_t stream) {
   static bool attr_set = false;
-  auto kfn = conv_gemm_tc<BN, STAGES, KIND>;
+  auto kfn = conv_gemm_tc<BN, KIND>;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BN, STAGES>::SMEM);
-    SEG_REQUIRE(e == cudaSuccess, "cudaFuncSetAttribute(smem=%d): %s", Cfg<BN, STAGES>::SMEM, cudaGetErrorString(e));
+    cudaError_t e = cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BN>::SMEM);
+    SEG_REQUIRE(e == cudaSuccess, "cudaFuncSetAttribute(smem=%d): %s", Cfg<BN>::SMEM, cudaGetErrorString(e));
     attr_set = true;
   }
-  launch_pdl(kfn, grid, dim3(NTHREADS), (size_t)Cfg<BN, STAGES>::SMEM, stream, p);
+  launch_pdl(kfn, grid, dim3(NTHREADS), (size_t)Cfg<BN>::SMEM, stream, p);
   return check_launch("conv_gemm_tc");
 }
 
-// Tile configurations: every one fits two CTAs per SM (<= 113 KB smem, <= 256 TMEM columns) so one CTA's epilogue
-// overlaps the other's main loop; the staging tile of the epilogue (128 x BN x esize) must fit in STAGES*STAGE_BYTES.
 template <int KIND>
 static int launch_bn(int bn, const TcParams& p, dim3 grid, cudaStream_t stream) {
   switch (bn) {
-    case 64: return launch_kernel<64, 4, KIND>(p, grid, stream);    // 4 x 24 KB
-    case 128: return launch_kernel<128, 3, KIND>(p, grid, stream);  // 3 x 32 KB
-    case 256: return launch_kernel<256, 2, KIND>(p, grid, stream);  // 2 x 48 KB
+    case 64: return launch_kernel<64, KIND>(p, grid, stream);
+    case 128: return launch_kernel<128, KIND>(p, grid, stream);
+    case 256: return launch_kernel<256, KIND>(p, grid, stream);
   }
   set_error("bad BN %d", bn);
   return 1;
 }
 
-static int env_dbg() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("SEG_TC_DBG");
-    v = e ? atoi(e) : 0;
-  }
-  return v;
-}
-
-}  // namespace tc
-}  // namespace seg
-#include "seg_conv_tc2.cuh"
-namespace seg {
-namespace tc {
-
-static bool long_k_rule() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("SEG_TC_LONGK");
-    v = e ? atoi(e) : 1;
-  }
-  return v != 0;
-}
-
-static bool use_v2() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("SEG_TC_V2");
-    v = e ? atoi(e) : 1;
-  }
-  return v != 0;
-}
-
-static int env_bn() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("SEG_TC_BN");
-    v = e ? atoi(e) : 0;
-  }
-  return v;
-}
-
-static int env_v2bn() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("SEG_TC_V2BN");
-    v = e ? atoi(e) : 0;
-  }
-  return v;
-}
-
-// tile width of the persistent kernel for an output of `ncols` columns and `m_tiles` row tiles
-// (profiles/conv_sweep_r02.txt: 256-wide tiles win or tie on every C3 shape with >= 256 output columns — 3x3 512->512 d2 @33^2
-//  937 -> 1336 TFLOP/s, 1x1 512->2048 722 -> 875, decoder 3x3 256->256 @129^2 1067 -> 1366 — except where the last column
-//  block would be mostly padding: dgrad of the 304-channel decoder input, 846 -> 812)
-static int pick_v2_bn(int ncols, int64_t m_tiles, bool tma_ok) {
-  if (!tma_ok || ncols < 256) return V2_BN;
-  const int forced = env_v2bn();
-  if (forced == 128 || forced == 256) return forced;
-  const int waste = ceil_div(ncols, 256) * 256 - ncols;
-  return waste < 128 ? 256 : V2_BN;
-}
-
-static int pick_bn(int ncols, int out_dtype) {
+// Tile width for an output of `ncols` columns: 128 x 256 tiles move 0.75x the operand bytes per MAC of 128 x 128 ones, so
+// they are taken where the layer has >= 256 output columns and the last column block is not mostly padding.
+static int pick_bn(int ncols) {
   if (ncols <= 64) return 64;
-  if (out_dtype == SEG_DT_F32) return 64;  // fp32 staging tile: 128 x 64 x 4 B
-  const int forced = env_bn();
-  if (forced == 64 || forced == 128 || forced == 256) return forced;
-  return 128;
+  if (ncols < 256) return 128;
+  const int waste = ceil_div(ncols, 256) * 256 - ncols;
+  return waste < 128 ? 256 : 128;
 }
 
 bool supported(const seg_conv_desc* d) {
@@ -611,7 +531,7 @@ static bool is_pointwise(const seg_conv_desc* d) { return d->R == 1 && d->S == 1
 
 int conv_fwd(const seg_conv_desc* d, const void* x, const void* w, void* y, int y_dtype, const float* bias, float beta,
              double* stats, unsigned* stat_ticket, const SyncDesc* sync, cudaStream_t stream) {
-  SEG_REQUIRE(supported(d), "tcgen05 conv fwd: unsupported shape (C=%d ldx=%d R=%d pad=%d dil=%d)", d->C, d->ldx, d->R,
+  SEG_REQUIRE(supported(d), "wgmma conv fwd: unsupported shape (C=%d ldx=%d R=%d pad=%d dil=%d)", d->C, d->ldx, d->R,
               d->pad, d->dil);
   TcParams p;
   memset(&p, 0, sizeof(p));
@@ -644,20 +564,7 @@ int conv_fwd(const seg_conv_desc* d, const void* x, const void* w, void* y, int 
     p.sync = *sync;
   }
   const int64_t m_tiles = ceil_div64(M, BM);
-  // persistent double-buffered kernel for bf16 outputs wider than 64 channels; the one-tile-per-CTA kernel otherwise
-  // (measured: with <= 2 tiles per SM and a long k-loop, two co-resident one-tile CTAs interleave better than one
-  //  persistent CTA; everywhere else — short k-loops, many tiles — the persistent kernel wins by 1.3-1.8x)
-  const int64_t tiles128 = m_tiles * ceil_div(d->K, 128);
-  // (measured, profiles/conv_longk_r02.txt: with few tiles and a long k-loop the two co-resident one-tile CTAs still win for
-  //  the 3x3s — 256->256 @33^2: 751 vs 704 TFLOP/s — but not for a 1x1 with >= 256 outputs: 2048->256 612 vs 687 on 256-wide tiles)
-  const bool wide_ok = d->K >= 256 && v2_tma_epilogue_ok(y, d->ldy, beta, false);
-  const bool long_k_few_tiles = long_k_rule() && tiles128 <= 2 * num_sms() && (int64_t)d->R * d->S * ceil_div(d->C, BK) >= 32 &&
-                                !(wide_ok && d->R * d->S == 1);
-  const bool v2 = use_v2() && y_dtype == SEG_DT_BF16 && bias == nullptr && d->K > 64 && !long_k_few_tiles;
-  // 256-wide persistent tiles (0.75x the operand bytes per flop) where the layer has >= 256 output channels, the output can
-  // go through the TMA epilogue and there are enough 128 x 256 tiles to fill the SMs (env SEG_TC_V2BN = 128 | 256 forces)
-  const int v2bn = v2 ? pick_v2_bn(d->K, m_tiles, v2_tma_epilogue_ok(y, d->ldy, beta, false)) : V2_BN;
-  const int bn = v2 ? v2bn : pick_bn(d->K, y_dtype);
+  const int bn = pick_bn(d->K);
   if (is_pointwise(d)) {
     p.x_im2col = 0;
     if (make_map_2d(&p.mapA, x, M, d->C, d->ldx, BM)) return 1;
@@ -667,7 +574,6 @@ int conv_fwd(const seg_conv_desc* d, const void* x, const void* w, void* y, int 
     if (make_map_im2col(&p.mapA, x, d->N, d->H, d->W, d->C, d->ldx, -d->pad, -d->pad, upper, upper, d->stride, BM)) return 1;
   }
   if (make_map_2d(&p.mapB, w, (int64_t)p.taps * d->K, d->C, d->C, bn)) return 1;
-  if (v2) return launch_v2<KIND_KK>(p, stream, v2bn);
   dim3 grid((unsigned)m_tiles, (unsigned)ceil_div(d->K, bn), 1);
   return launch_bn<KIND_KK>(bn, p, grid, stream);
 }
@@ -675,16 +581,10 @@ int conv_fwd(const seg_conv_desc* d, const void* x, const void* w, void* y, int 
 static int floordiv(int a, int b) { return (a >= 0) ? a / b : -((-a + b - 1) / b); }
 
 int conv_dgrad(const seg_conv_desc* d, const void* dy, const void* w, void* dx, float beta, cudaStream_t stream) {
-  SEG_REQUIRE(supported(d) && d->ldy % 8 == 0, "tcgen05 conv dgrad: unsupported shape (stride=%d K=%d ldy=%d)", d->stride,
+  SEG_REQUIRE(supported(d) && d->ldy % 8 == 0, "wgmma conv dgrad: unsupported shape (stride=%d K=%d ldy=%d)", d->stride,
               d->K, d->ldy);
   const int s = d->stride;
-  const int64_t tiles128 = ceil_div64((int64_t)d->N * d->H * d->W, BM) * ceil_div(d->C, 128) / (s * s);
-  // (measured: dgrad 256<-256 3x3 @33^2 647 TFLOP/s on the one-tile kernel, 966 on 256-wide persistent tiles)
-  const bool wide_ok = s == 1 && pick_v2_bn(d->C, 1 << 20, v2_tma_epilogue_ok(dx, d->ldx, beta, false)) == 256;
-  const bool long_k_few_tiles = long_k_rule() && !wide_ok && tiles128 <= 2 * num_sms() &&
-                                (int64_t)d->R * d->S * ceil_div(d->K, BK) / (s * s) >= 32;
-  const bool v2 = use_v2() && d->C > 64 && !long_k_few_tiles;
-  const int bn = v2 ? V2_BN : pick_bn(d->C, SEG_DT_BF16);
+  const int bn = pick_bn(d->C);
   // One launch per parity class (py, px) of the input pixels; stride 1 has the single class (0, 0).
   for (int py = 0; py < s; ++py) {
     for (int px = 0; px < s; ++px) {
@@ -755,20 +655,48 @@ int conv_dgrad(const seg_conv_desc* d, const void* dy, const void* w, void* dx, 
         if (make_map_2d(&p.mapA, w, (int64_t)d->R * d->S * d->K, d->C, d->C, BM)) return 1;
         if (make_map_2d(&p.mapB, w, (int64_t)d->R * d->S * d->K, d->C, d->C, 64)) return 1;
       }
-      if (v2 && p.taps > 0) {
-        const int v2bn = pick_v2_bn(d->C, m_tiles, v2_tma_epilogue_ok(dx, d->ldx, beta, s > 1));
-        if (launch_v2<KIND_KM>(p, stream, v2bn)) return 1;
-        continue;
-      }
-      dim3 grid((unsigned)m_tiles, (unsigned)ceil_div(d->C, v2 ? 128 : bn), 1);
-      if (launch_bn<KIND_KM>(v2 ? 128 : bn, p, grid, stream)) return 1;
+      dim3 grid((unsigned)m_tiles, (unsigned)ceil_div(d->C, bn), 1);
+      if (launch_bn<KIND_KM>(bn, p, grid, stream)) return 1;
     }
   }
   return 0;
 }
 
-int conv_wgrad(const seg_conv_desc* d, const void* dy, const void* x, float* dw, cudaStream_t stream) {
-  SEG_REQUIRE(supported(d) && d->ldy % 8 == 0, "tcgen05 conv wgrad: unsupported shape");
+// dW[i] += sum over splits s (in order) of ws[s][i]
+__global__ void wgrad_split_reduce_kernel(const float* __restrict__ ws, int splits, int64_t n, float* __restrict__ dw) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    float acc = ws[i];
+    for (int s = 1; s < splits; ++s) acc += ws[(size_t)s * n + i];
+    dw[i] += acc;
+  }
+}
+
+// tile width and number of k-splits of the wgrad of `d` (one wave: tiles * splits <= resident CTAs, one per SM)
+static void wgrad_plan(const seg_conv_desc* d, int& bn, int& splits, int& kblocks_per_split) {
+  // 256-wide tiles for the 3x3 convs with C a multiple of 256; the 1x1s keep 128-wide tiles (twice as many tiles for the
+  // one-wave split-K)
+  const bool wide = d->R * d->S >= 9 && d->C >= 256 && d->C % 256 == 0;
+  bn = (d->C <= 64) ? 64 : (wide ? 256 : 128);
+  const int kblocks_total = (int)ceil_div64((int64_t)d->N * d->P * d->Q, BK);
+  const int tiles = ceil_div(d->K, BM) * ceil_div(d->C, bn) * d->R * d->S;
+  splits = max(1, num_sms() / tiles);
+  splits = min(splits, kblocks_total);
+  splits = min(splits, 1024);
+  kblocks_per_split = ceil_div(kblocks_total, splits);
+  // recounted so that every split owns at least one k-block: the split-order reduction reads every split's workspace slice,
+  // and a split without k-blocks would leave its slice unwritten (conv_wgrad checks this)
+  splits = ceil_div(kblocks_total, kblocks_per_split);
+}
+
+int64_t wgrad_workspace_floats(const seg_conv_desc* d) {
+  if (!supported(d)) return 0;
+  int bn, splits, kps;
+  wgrad_plan(d, bn, splits, kps);
+  return splits > 1 ? (int64_t)splits * d->R * d->S * d->K * d->C : 0;
+}
+
+int conv_wgrad(const seg_conv_desc* d, const void* dy, const void* x, float* dw, float* ws, cudaStream_t stream) {
+  SEG_REQUIRE(supported(d) && d->ldy % 8 == 0, "wgmma conv wgrad: unsupported shape");
   TcParams p;
   memset(&p, 0, sizeof(p));
   const int64_t npix = (int64_t)d->N * d->P * d->Q;
@@ -789,22 +717,11 @@ int conv_wgrad(const seg_conv_desc* d, const void* dy, const void* x, float* dw,
   p.dw_K = d->K;
   p.dw_C = d->C;
   p.kblocks_total = (int)ceil_div64(npix, BK);
-  static int wgrad_bn_env = -1;
-  if (wgrad_bn_env < 0) {
-    const char* e = getenv("SEG_TC_WGRAD_BN");
-    wgrad_bn_env = e ? atoi(e) : 0;
-  }
-  // 256-wide wgrad tiles pay on the 3x3 convs with C a multiple of 256 (measured: 2048->256 d12 1231 -> 1376 TFLOP/s, decoder
-  // 256->256 @129^2 1182 -> 1332) and lose on the 1x1s (478 -> 363: half as many tiles for the one-wave split-K); env forces
-  const bool wide = wgrad_bn_env == 256 ? d->C >= 256 : (wgrad_bn_env == 128 ? false : (d->R * d->S >= 9 && d->C >= 256 && d->C % 256 == 0));
-  const int bn = (d->C <= 64) ? 64 : (wide ? 256 : 128);
-  const int tiles = ceil_div(d->K, BM) * ceil_div(d->C, bn) * p.taps;
-  // one wave: tiles * splits <= resident CTA slots (2 per SM), so no CTA waits for a second wave
-  int splits = max(1, (2 * num_sms()) / tiles);
-  splits = min(splits, p.kblocks_total);
-  splits = min(splits, 1024);
-  p.kblocks_per_split = ceil_div(p.kblocks_total, splits);
-  splits = ceil_div(p.kblocks_total, p.kblocks_per_split);
+  int bn, splits;
+  wgrad_plan(d, bn, splits, p.kblocks_per_split);
+  SEG_REQUIRE(splits == 1 || ws != nullptr, "wgmma conv wgrad: %d k-splits need the workspace (seg_conv2d_wgrad_workspace_floats)", splits);
+  SEG_REQUIRE((int64_t)(splits - 1) * p.kblocks_per_split < p.kblocks_total, "wgmma conv wgrad: split %d has no k-blocks", splits - 1);
+  if (splits > 1) p.ws = ws;
   if (make_map_2d(&p.mapA, dy, npix, d->K, d->ldy, 64)) return 1;
   if (is_pointwise(d)) {
     p.x_im2col = 0;
@@ -816,7 +733,11 @@ int conv_wgrad(const seg_conv_desc* d, const void* dy, const void* x, float* dw,
   }
   SEG_REQUIRE((unsigned)(p.taps * splits) <= 65535u, "wgrad grid.z too large");
   dim3 grid((unsigned)ceil_div(d->K, BM), (unsigned)ceil_div(d->C, bn), (unsigned)(p.taps * splits));
-  return launch_bn<KIND_MM>(bn, p, grid, stream);
+  if (launch_bn<KIND_MM>(bn, p, grid, stream)) return 1;
+  if (splits == 1) return 0;
+  const int64_t n = (int64_t)p.taps * d->K * d->C;
+  wgrad_split_reduce_kernel<<<(unsigned)std::min<int64_t>(ceil_div64(n, 256), (int64_t)num_sms() * 8), 256, 0, stream>>>(ws, splits, n, dw);
+  return check_launch("wgrad_split_reduce");
 }
 
 }  // namespace tc

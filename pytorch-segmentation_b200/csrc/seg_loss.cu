@@ -170,26 +170,44 @@ static inline float rscale(int in_size, int out_size, int ac) {
 }
 
 constexpr int MAXC = 160;  // classes supported by the fused kernel (19 / 21 / 150 on the configs)
-constexpr int TILE = 32;   // output tile edge
+constexpr int TILE = 32;   // output tile edge (the backward halves it when the 32 x 32 tile's patch does not fit in shared memory)
+
+// The backward accumulates the logits gradient in 64-bit fixed point: integer additions are associative, so the result
+// does not depend on the order in which threads and blocks add their contributions (fp32 atomics did).  Every contribution
+// is at most |g| in magnitude and the interpolation weights reaching one low-res element sum to less than
+// (2/sh + 2)(2/sw + 2), so with that bound below 2^e the scale 2^(61-e) cannot overflow; a contribution is rounded to
+// |bound| * 2^-62, far below the fp32 rounding of the result.
+__device__ __forceinline__ double ce_grad_scale(float g, float sh, float sw, int Ho, int Wo) {
+  const double ry = sh > 0.f ? 2.0 / sh : (double)Ho, rx = sw > 0.f ? 2.0 / sw : (double)Wo;
+  int e;
+  frexp(fabs((double)g) * (ry + 2.0) * (rx + 2.0), &e);
+  return ldexp(1.0, 61 - e);
+}
+__device__ __forceinline__ float ce_grad_g(const float* gscale, const double* accum) {
+  return (gscale ? *gscale : 1.f) / (float)fmax(accum[1], 1.0);
+}
+__device__ __forceinline__ unsigned long long to_fixed(float v, double scale) {
+  return (unsigned long long)__double2ll_rn((double)v * scale);
+}
 
 // one block = one 32x32 output tile; the low-res source patch (<= PATCH x PATCH pixels x C) is staged in smem
 template <bool BWD>
 __global__ void __launch_bounds__(256) upsample_ce_kernel(const float* __restrict__ lo, const int64_t* __restrict__ target,
                                                           int N, int Hi, int Wi, int Ho, int Wo, int C, int ac, float sh,
                                                           float sw, int64_t ignore, double* accum, int32_t* argmax,
-                                                          const float* __restrict__ gscale, float* __restrict__ dlo,
-                                                          int patch) {
-  extern __shared__ float sm[];
-  float* src = sm;                                   // [patch*patch][C]
-  float* dst = BWD ? sm + patch * patch * C : nullptr;  // [patch*patch][C] grad accumulators
-  const int tiles_x = (Wo + TILE - 1) / TILE, tiles_y = (Ho + TILE - 1) / TILE;
+                                                          const float* __restrict__ gscale,
+                                                          unsigned long long* __restrict__ dlo_fixed, int patch, int tile) {
+  extern __shared__ unsigned long long sm64[];
+  unsigned long long* dst = BWD ? sm64 : nullptr;  // [patch*patch][C] fixed-point grad accumulators
+  float* src = reinterpret_cast<float*>(BWD ? sm64 + patch * patch * C : sm64);  // [patch*patch][C]
+  const int tiles_x = (Wo + tile - 1) / tile, tiles_y = (Ho + tile - 1) / tile;
   int t = blockIdx.x;
   const int tx = t % tiles_x;
   t /= tiles_x;
   const int ty = t % tiles_y;
   const int n = t / tiles_y;
-  const int oy0 = ty * TILE, ox0 = tx * TILE;
-  const int oy1 = min(oy0 + TILE, Ho) - 1, ox1 = min(ox0 + TILE, Wo) - 1;
+  const int oy0 = ty * tile, ox0 = tx * tile;
+  const int oy1 = min(oy0 + tile, Ho) - 1, ox1 = min(ox0 + tile, Wo) - 1;
   const int sy0 = src_idx(oy0, sh, Hi, ac).i0, sx0 = src_idx(ox0, sw, Wi, ac).i0;
   const int sy1 = src_idx(oy1, sh, Hi, ac).i1, sx1 = src_idx(ox1, sw, Wi, ac).i1;
   const int ph = sy1 - sy0 + 1, pw = sx1 - sx0 + 1;  // <= patch by construction (checked on host)
@@ -198,14 +216,18 @@ __global__ void __launch_bounds__(256) upsample_ce_kernel(const float* __restric
     const int pp = i / C;
     const int py = pp / pw, px = pp - py * pw;
     src[i] = lo[(((int64_t)n * Hi + sy0 + py) * Wi + sx0 + px) * C + c];
-    if (BWD) dst[i] = 0.f;
+    if (BWD) dst[i] = 0ull;
   }
   __syncthreads();
   double loss = 0.0, cnt = 0.0;
   float g = 0.f;
-  if (BWD) g = (gscale ? *gscale : 1.f) / (float)fmax(accum[1], 1.0);
-  for (int e = threadIdx.x; e < TILE * TILE; e += blockDim.x) {
-    const int oy = oy0 + e / TILE, ox = ox0 + e % TILE;
+  double scale = 0.0;
+  if (BWD) {
+    g = ce_grad_g(gscale, accum);
+    scale = ce_grad_scale(g, sh, sw, Ho, Wo);
+  }
+  for (int e = threadIdx.x; e < tile * tile; e += blockDim.x) {
+    const int oy = oy0 + e / tile, ox = ox0 + e % tile;
     if (oy >= Ho || ox >= Wo) continue;
     const int64_t tg = target[((int64_t)n * Ho + oy) * Wo + ox];
     const bool valid = tg != ignore;
@@ -239,17 +261,17 @@ __global__ void __launch_bounds__(256) upsample_ce_kernel(const float* __restric
       }
     } else {
       const float inv = 1.f / se;
-      float* da = dst + ((ly.i0 - sy0) * pw + (lx.i0 - sx0)) * C;
-      float* db = dst + ((ly.i0 - sy0) * pw + (lx.i1 - sx0)) * C;
-      float* dc = dst + ((ly.i1 - sy0) * pw + (lx.i0 - sx0)) * C;
-      float* dd = dst + ((ly.i1 - sy0) * pw + (lx.i1 - sx0)) * C;
+      unsigned long long* da = dst + ((ly.i0 - sy0) * pw + (lx.i0 - sx0)) * C;
+      unsigned long long* db = dst + ((ly.i0 - sy0) * pw + (lx.i1 - sx0)) * C;
+      unsigned long long* dc = dst + ((ly.i1 - sy0) * pw + (lx.i0 - sx0)) * C;
+      unsigned long long* dd = dst + ((ly.i1 - sy0) * pw + (lx.i1 - sx0)) * C;
       for (int c = 0; c < C; ++c) {
         const float v = h0 * (w0 * pa[c] + w1 * pb[c]) + h1 * (w0 * pc[c] + w1 * pd[c]);
         const float gr = (expf(v - mx) * inv - (c == tg ? 1.f : 0.f)) * g;
-        atomicAdd(da + c, h0 * w0 * gr);
-        atomicAdd(db + c, h0 * w1 * gr);
-        atomicAdd(dc + c, h1 * w0 * gr);
-        atomicAdd(dd + c, h1 * w1 * gr);
+        atomicAdd(da + c, to_fixed(h0 * w0 * gr, scale));
+        atomicAdd(db + c, to_fixed(h0 * w1 * gr, scale));
+        atomicAdd(dc + c, to_fixed(h1 * w0 * gr, scale));
+        atomicAdd(dd + c, to_fixed(h1 * w1 * gr, scale));
       }
     }
   }
@@ -258,15 +280,23 @@ __global__ void __launch_bounds__(256) upsample_ce_kernel(const float* __restric
   } else {
     __syncthreads();
     for (int i = threadIdx.x; i < ph * pw * C; i += blockDim.x) {
-      const float v = dst[i];
-      if (v != 0.f) {
+      const unsigned long long v = dst[i];
+      if (v != 0ull) {
         const int c = i % C;
         const int pp = i / C;
         const int py = pp / pw, px = pp - py * pw;
-        atomicAdd(dlo + (((int64_t)n * Hi + sy0 + py) * Wi + sx0 + px) * C + c, v);
+        atomicAdd(dlo_fixed + (((int64_t)n * Hi + sy0 + py) * Wi + sx0 + px) * C + c, v);
       }
     }
   }
+}
+
+// fixed-point accumulators -> fp32 gradient (the scale is recomputed exactly as the accumulating kernel did)
+__global__ void ce_grad_from_fixed_kernel(const unsigned long long* __restrict__ acc, int64_t n, const float* gscale,
+                                          const double* accum, float sh, float sw, int Ho, int Wo, float* __restrict__ dlo) {
+  const double inv = 1.0 / ce_grad_scale(ce_grad_g(gscale, accum), sh, sw, Ho, Wo);
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+    dlo[i] = (float)((double)(long long)acc[i] * inv);
 }
 
 __global__ void cast_pad_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ y, int64_t M, int C, int ld) {
@@ -278,10 +308,10 @@ __global__ void cast_pad_kernel(const float* __restrict__ x, __nv_bfloat16* __re
   }
 }
 
-static int patch_for(int in_size, int out_size, int ac) {
-  // upper bound on low-res rows touched by TILE consecutive output rows
+static int patch_for(int in_size, int out_size, int ac, int tile) {
+  // upper bound on low-res rows touched by `tile` consecutive output rows
   const float sc = rscale(in_size, out_size, ac);
-  int p = (int)ceilf(sc * (TILE - 1)) + 3;
+  int p = (int)ceilf(sc * (tile - 1)) + 3;
   return p < in_size + 1 ? p : in_size + 1;
 }
 
@@ -330,7 +360,7 @@ int seg_ce_finalize(const double* accum, float* loss, void* stream) {
 int seg_upsample_ce_fwd(const float* logits_lo, const int64_t* target, int N, int Hi, int Wi, int Ho, int Wo, int C,
                         int align_corners, int64_t ignore_index, double* accum, int32_t* argmax, void* stream) {
   SEG_REQUIRE(C <= MAXC, "upsample_ce: C=%d > %d", C, MAXC);
-  const int patch = std::max(patch_for(Hi, Ho, align_corners), patch_for(Wi, Wo, align_corners));
+  const int patch = std::max(patch_for(Hi, Ho, align_corners, TILE), patch_for(Wi, Wo, align_corners, TILE));
   const size_t smem = (size_t)patch * patch * C * sizeof(float);
   SEG_REQUIRE(smem <= 200 * 1024, "upsample_ce: patch too large (%zu B)", smem);
   static size_t set_smem = 0;
@@ -341,30 +371,40 @@ int seg_upsample_ce_fwd(const float* logits_lo, const int64_t* target, int N, in
   const int blocks = N * ceil_div(Ho, TILE) * ceil_div(Wo, TILE);
   upsample_ce_kernel<false><<<blocks, 256, smem, ST(stream)>>>(
       logits_lo, target, N, Hi, Wi, Ho, Wo, C, align_corners, rscale(Hi, Ho, align_corners), rscale(Wi, Wo, align_corners),
-      ignore_index, accum, argmax, nullptr, nullptr, patch);
+      ignore_index, accum, argmax, nullptr, nullptr, patch, TILE);
   return check_launch("upsample_ce_fwd");
 }
 
-// dlo_f32: fp32 scratch [N,Hi,Wi,C] (zeroed here); dx: bf16 [N*Hi*Wi][lddx]
+// dlo_f32: fp32 [N,Hi,Wi,C]; dlo_fixed: int64 scratch [N,Hi,Wi,C] (zeroed here); dx: bf16 [N*Hi*Wi][lddx] or NULL
 int seg_upsample_ce_bwd(const float* logits_lo, const int64_t* target, int N, int Hi, int Wi, int Ho, int Wo, int C,
                         int align_corners, int64_t ignore_index, const double* accum, const float* gscale,
-                        float* dlo_f32, void* dx, int lddx, void* stream) {
+                        float* dlo_f32, void* dlo_fixed, void* dx, int lddx, void* stream) {
   SEG_REQUIRE(C <= MAXC, "upsample_ce: C=%d > %d", C, MAXC);
-  const int patch = std::max(patch_for(Hi, Ho, align_corners), patch_for(Wi, Wo, align_corners));
-  const size_t smem = (size_t)2 * patch * patch * C * sizeof(float);
-  SEG_REQUIRE(smem <= 200 * 1024, "upsample_ce: patch too large (%zu B)", smem);
+  // fixed-point accumulators (8 B) + the fp32 source patch per (patch pixel, class)
+  auto bwd_patch = [&](int t) { return std::max(patch_for(Hi, Ho, align_corners, t), patch_for(Wi, Wo, align_corners, t)); };
+  auto bwd_smem = [&](int t) { return (size_t)bwd_patch(t) * bwd_patch(t) * C * (sizeof(unsigned long long) + sizeof(float)); };
+  const int tile = bwd_smem(TILE) <= 227 * 1024 ? TILE : TILE / 2;
+  const int patch = bwd_patch(tile);
+  const size_t smem = bwd_smem(tile);
+  SEG_REQUIRE(smem <= 227 * 1024, "upsample_ce: patch too large (%zu B)", smem);
   static size_t set_smem = 0;
   if (smem > set_smem) {
     cudaFuncSetAttribute(upsample_ce_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     set_smem = smem;
   }
   const int64_t M = (int64_t)N * Hi * Wi;
-  cudaMemsetAsync(dlo_f32, 0, (size_t)M * C * sizeof(float), ST(stream));
-  const int blocks = N * ceil_div(Ho, TILE) * ceil_div(Wo, TILE);
+  unsigned long long* fixed = reinterpret_cast<unsigned long long*>(dlo_fixed);
+  cudaMemsetAsync(fixed, 0, (size_t)M * C * sizeof(unsigned long long), ST(stream));
+  const int blocks = N * ceil_div(Ho, tile) * ceil_div(Wo, tile);
+  const float sh = rscale(Hi, Ho, align_corners), sw = rscale(Wi, Wo, align_corners);
   upsample_ce_kernel<true><<<blocks, 256, smem, ST(stream)>>>(
-      logits_lo, target, N, Hi, Wi, Ho, Wo, C, align_corners, rscale(Hi, Ho, align_corners), rscale(Wi, Wo, align_corners),
-      ignore_index, const_cast<double*>(accum), nullptr, gscale, dlo_f32, patch);
+      logits_lo, target, N, Hi, Wi, Ho, Wo, C, align_corners, sh, sw, ignore_index, const_cast<double*>(accum), nullptr, gscale,
+      fixed, patch, tile);
   if (check_launch("upsample_ce_bwd")) return 1;
+  const int64_t n = M * C;
+  ce_grad_from_fixed_kernel<<<(unsigned)std::min<int64_t>(ceil_div64(n, 256), (int64_t)num_sms() * 8), 256, 0, ST(stream)>>>(
+      fixed, n, gscale, accum, sh, sw, Ho, Wo, dlo_f32);
+  if (check_launch("ce_grad_from_fixed")) return 1;
   if (dx) {
     int blocks2 = (int)std::min<int64_t>(ceil_div64(M * lddx, 256), (int64_t)num_sms() * 8);
     cast_pad_kernel<<<blocks2, 256, 0, ST(stream)>>>(dlo_f32, reinterpret_cast<__nv_bfloat16*>(dx), M, C, lddx);

@@ -1,8 +1,8 @@
 // seg_sync.cuh — SyncBN statistics exchange folded INTO the kernels that produce and consume the statistics.
 //
-// Round 1 ran one single-CTA exchange kernel per BatchNorm layer and direction (226 launches per DeepLab-R101 step), each a
-// world-wide flag barrier sitting alone between a conv epilogue and bn_apply; at 8 GPUs that cost ~33 us per exchange —
-// the limiter of the 1 -> 8 scaling curve.  Now the exchange has no launch of its own:
+// A stand-alone exchange kernel per BatchNorm layer and direction (226 launches per DeepLab-R101 step) would be a world-wide
+// flag barrier sitting alone between a conv epilogue and bn_apply, paid once per exchange.  Here the exchange has no launch
+// of its own:
 //
 //   producer  = a kernel that ends with per-channel totals: the conv epilogues / the depthwise conv / bn_stats (fp64 atomics
 //               into the layer's accumulators) and bn_bwd_reduce / the cooperative BN backward.  The LAST block to finish
@@ -100,7 +100,10 @@ __device__ __forceinline__ void sync_publish(const SyncDesc& s, uint32_t epoch, 
 // producer epilogue for kernels that accumulate their per-channel totals with fp64 atomics into `acc` (n doubles): every
 // contributing block calls this with its `nthr` cooperating threads after issuing its atomics; the LAST of `nblocks` blocks to
 // arrive (ticket) reads the finished totals and pushes them (as fp64) to every peer, then raises the flags.
-template <class Sync>
+template <bool kPrint, class Sync>
+__device__ __forceinline__ void sync_exchange_block_d(const SyncDesc& s, double* acc, int n, int tid, int nthr, Sync sync);
+// kPrint = false: time out with a bare trap — no printf call, which would make ptxas serialise a caller's wgmma pipeline
+template <bool kPrint = true, class Sync>
 __device__ __forceinline__ void sync_push_when_last(const SyncDesc& s, const double* acc, int n, unsigned* ticket, unsigned nblocks,
                                                     int tid, int nthr, Sync sync, volatile int* sm_flag) {
   __threadfence();
@@ -110,7 +113,7 @@ __device__ __forceinline__ void sync_push_when_last(const SyncDesc& s, const dou
   if (!*sm_flag) return;
   __threadfence();
   if (s.mode == 1) {  // the whole exchange here: acc becomes the world's totals, the consumer needs no SyncBN logic
-    sync_exchange_block_d(s, const_cast<double*>(acc), n, tid, nthr, sync);
+    sync_exchange_block_d<kPrint>(s, const_cast<double*>(acc), n, tid, nthr, sync);
     return;
   }
   const uint32_t epoch = sync_epoch(s);
@@ -139,7 +142,7 @@ __device__ __forceinline__ void sync_total8(const SyncDesc& s, uint32_t epoch, i
 
 // ---- mode 1: the whole exchange inside the producer's last block -----------------------------------------------------------------
 // wait for the world's flags with the `nthr` cooperating threads of ONE block (tid 0..nthr-1, `sync()` their barrier)
-template <class Sync>
+template <bool kPrint = true, class Sync>
 __device__ __forceinline__ void sync_wait_world_block(const SyncDesc& s, uint32_t epoch, int tid, Sync sync) {
   if (tid < s.world) {
     const uint32_t* mine = reinterpret_cast<const uint32_t*>(reinterpret_cast<const char*>(s.peers[s.rank]) + sync_flags_offset(s.world, s.n_max)) +
@@ -148,7 +151,8 @@ __device__ __forceinline__ void sync_wait_world_block(const SyncDesc& s, uint32_
     const long long t0 = clock64();
     while (sync_ld_acquire_sys(mine) != epoch) {
       if (clock64() - t0 > limit) {
-        printf("seg_b200: SyncBN exchange timeout (rank %d waiting for rank %d, epoch %u; raise SEG_SYNC_TIMEOUT_S)\n", s.rank, tid, epoch);
+        if constexpr (kPrint)
+          printf("seg_b200: SyncBN exchange timeout (rank %d waiting for rank %d, epoch %u; raise SEG_SYNC_TIMEOUT_S)\n", s.rank, tid, epoch);
         __trap();
       }
     }
@@ -161,12 +165,12 @@ __device__ __forceinline__ void sync_advance(const SyncDesc& s, uint32_t epoch) 
   __threadfence();
 }
 // fp64 totals acc[0..n) (this rank's, final) -> world totals, in place; called by the cooperating threads of ONE block
-template <class Sync>
+template <bool kPrint, class Sync>
 __device__ __forceinline__ void sync_exchange_block_d(const SyncDesc& s, double* acc, int n, int tid, int nthr, Sync sync) {
   const uint32_t epoch = sync_epoch(s);
   for (int i = tid; i < n; i += nthr) sync_push_value_d(s, epoch, i, __ldcg(acc + i));
   sync_publish(s, epoch, tid, sync);
-  sync_wait_world_block(s, epoch, tid, sync);
+  sync_wait_world_block<kPrint>(s, epoch, tid, sync);
   for (int i = tid; i < n; i += nthr) acc[i] = sync_total_d(s, epoch, i);
   __threadfence();
   sync();

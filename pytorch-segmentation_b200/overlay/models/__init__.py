@@ -1,6 +1,6 @@
 """Overlay for the reference's `models` registry (models/__init__.py): put this directory's PARENT
 (`pytorch-segmentation_b200/overlay`) in front of the reference tree on PYTHONPATH and `train.py` resolves
-`config['arch']['type']` == 'DeepLab' / 'PSPNet' to the B200-native classes while every other architecture keeps
+`config['arch']['type']` == 'DeepLab' / 'PSPNet' to the H100-native classes while every other architecture keeps
 coming from the reference, unmodified.  See INTEGRATION.md."""
 import importlib
 import os
@@ -35,4 +35,4 @@ if _REF_MODELS is not None:
         except Exception as _e:  # a reference model that cannot import here stays unavailable, as in the reference
             globals().setdefault("_import_errors", {})[_mod] = repr(_e)
 
-from seg_b200.nets import DeepLab, PSPNet, UperNet  # noqa: E402,F401  B200-native replacements (same names, same contract)
+from seg_b200.nets import DeepLab, PSPNet, UperNet  # noqa: E402,F401  H100-native replacements (same names, same contract)

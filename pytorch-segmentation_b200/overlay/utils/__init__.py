@@ -1,5 +1,5 @@
 """Overlay for the reference's `utils` package: everything resolves to the reference's modules except `utils.losses`,
-whose CrossEntropyLoss2d is the B200-native one.  See INTEGRATION.md."""
+whose CrossEntropyLoss2d is the H100-native one.  See INTEGRATION.md."""
 import os
 import sys
 

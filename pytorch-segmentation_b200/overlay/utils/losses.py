@@ -1,5 +1,5 @@
 """`utils.losses` overlay: the reference's loss registry (train.py:30 `getattr(losses, config['loss'])`) with
-CrossEntropyLoss2d replaced by the sm_100a kernel version; the other losses are re-exported from the reference file."""
+CrossEntropyLoss2d replaced by the sm_90a kernel version; the other losses are re-exported from the reference file."""
 import importlib.util
 import os
 

@@ -1,5 +1,5 @@
 """`utils.sync_batchnorm` overlay (imported by base/base_trainer.py:11-12): the reference's package, re-exported, with
-`convert_model` made aware of the B200-native engine models.
+`convert_model` made aware of the H100-native engine models.
 
 The reference turns `config['use_synch_bn']` into `convert_model(model)` + `DataParallelWithCallback(model, device_ids)`
 (base/base_trainer.py:33-35): every nn.BatchNorm2d is swapped for a SynchronizedBatchNorm2d whose replicas meet through

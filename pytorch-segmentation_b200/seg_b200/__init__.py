@@ -1,7 +1,7 @@
-"""seg_b200 — B200-native forward/backward engine for the data-parallel hot path of yassouali/pytorch-segmentation.
+"""seg_b200 — H100-native forward/backward engine for the data-parallel hot path of yassouali/pytorch-segmentation.
 
 Host side mirrors the reference's plugin surface (models / losses registries); all arithmetic runs in the hand-written
-sm_100a kernels of ``libseg_b200.so`` (C ABI: include/seg_b200.h).  No CPU fallback.
+sm_90a kernels of ``libseg_b200.so`` (C ABI: include/seg_b200.h).  No CPU fallback.
 
 Attributes are resolved lazily so that ``python -m seg_b200.launch`` can order sys.path (overlay before the reference
 tree) before anything imports the reference's ``base`` / ``utils`` packages.

@@ -171,7 +171,7 @@ class DeviceBatcher:
                                           want_labels=want_labels)
 
     def stage_full(self, samples):
-        """(validated on the B200 in round 2: bit-exact against the staged oracle, tests/test_data_tail_gpu.py.)  samples: sequence of
+        """(bit-exact against the staged oracle, tests/test_data_tail_gpu.py.)  samples: sequence of
         (RAW image, RAW label or None, h, w, angle or None, y0, x0, flip): resize to h x w, rotate by `angle` degrees about the
         centre (base_dataset.py:77-83), pad / crop / flip / normalise — one kernel (`seg_augment_full_batch_u8`)."""
         assert _FULL_ENTRY.itemsize == lib.load().seg_aug_full_entry_bytes()

@@ -24,7 +24,7 @@ from . import ops
 
 def _require_cuda(image):
     if not image.is_cuda:
-        raise RuntimeError("seg_b200.inference runs on a B200 only; there is no CPU fallback")
+        raise RuntimeError("seg_b200.inference runs on an H100 only; there is no CPU fallback")
 
 
 def multi_scale_predict(model, image, scales, num_classes, device=None, flip=False):

@@ -1,4 +1,4 @@
-"""Run an UNMODIFIED reference script (train.py / inference.py) with the B200-native models and losses plugged in:
+"""Run an UNMODIFIED reference script (train.py / inference.py) with the H100-native models and losses plugged in:
 
     cd /path/to/pytorch-segmentation
     PYTHONPATH=/path/to/repo/pytorch-segmentation_b200 python -m seg_b200.launch train.py -c config.json

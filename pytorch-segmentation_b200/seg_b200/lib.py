@@ -1,7 +1,7 @@
 """ctypes binding of the C-ABI shared library ``libseg_b200.so`` (declared in ``include/seg_b200.h``).
 
 Every function takes plain device pointers / sizes and a ``cudaStream_t``; torch is used only to own device memory
-and streams.  There is no CPU fallback: if the library is missing or the device is not sm_100 the import-time /
+and streams.  There is no CPU fallback: if the library is missing or the device is not sm_90 the import-time /
 first-call checks raise.
 """
 import ctypes
@@ -48,7 +48,8 @@ _SIGS = {
     "seg_launch_count_reset": (None, []),
     "seg_conv2d_fwd": (c_int, [POINTER(ConvDesc), c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_float, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
     "seg_conv2d_dgrad": (c_int, [POINTER(ConvDesc), c_void_p, c_void_p, c_void_p, c_float, c_int, c_void_p]),
-    "seg_conv2d_wgrad": (c_int, [POINTER(ConvDesc), c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
+    "seg_conv2d_wgrad_workspace_floats": (c_int64, [POINTER(ConvDesc), c_int]),
+    "seg_conv2d_wgrad": (c_int, [POINTER(ConvDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
     "seg_dwconv_scratch_floats": (c_int64, [c_int]),
     "seg_dwconv3x3_fwd": (c_int, [POINTER(ConvDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "seg_dwconv3x3_bwd_data": (c_int, [POINTER(ConvDesc), c_void_p, c_void_p, c_void_p, c_float, c_void_p]),
@@ -92,7 +93,7 @@ _SIGS = {
     "seg_eval_metrics_nchw": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "seg_ce_finalize": (c_int, [c_void_p, c_void_p, c_void_p]),
     "seg_upsample_ce_fwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int64, c_void_p, c_void_p, c_void_p]),
-    "seg_upsample_ce_bwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
+    "seg_upsample_ce_bwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
     "seg_relu_fwd": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int64, c_int, c_void_p]),
     "seg_relu_bwd": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int64, c_int, c_float, c_void_p]),
     "seg_nhwc_to_nchw_f32": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
@@ -130,7 +131,7 @@ def load():
         if not os.path.exists(LIB_PATH):
             raise RuntimeError(
                 f"{LIB_PATH} not found: build it with pytorch-segmentation_b200/build.sh (or __graft_entry__.build()); "
-                "the B200 engine has no CPU / eager fallback")
+                "the engine has no CPU / eager fallback")
         lib = ctypes.CDLL(LIB_PATH)
         for name, (res, args) in _SIGS.items():
             fn = getattr(lib, name)
@@ -176,7 +177,7 @@ def call(name, *args, meta=None):
 def require_device():
     lib = load()
     if not torch.cuda.is_available():
-        raise RuntimeError("seg_b200 needs a CUDA device (sm_100); no CPU fallback exists")
+        raise RuntimeError("seg_b200 needs a CUDA device (sm_90); no CPU fallback exists")
     if lib.seg_device_ok() != 0:
         raise RuntimeError(last_error())
 

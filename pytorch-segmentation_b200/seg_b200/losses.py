@@ -5,7 +5,7 @@
     CE_DiceLoss(smooth=1, reduction='mean', ignore_index=255, weight=None) — utils/losses.py:67-77
     LovaszSoftmax(classes='present', per_image=False, ignore_index=255)   — utils/losses.py:79-89
 
-forward(output fp32 [B,C,H,W], target int64 [B,H,W]) -> 0-dim tensor with autograd, computed by the sm_100a kernels
+forward(output fp32 [B,C,H,W], target int64 [B,H,W]) -> 0-dim tensor with autograd, computed by the sm_90a kernels
 (`seg_ce_nchw_fwd/bwd`); `.item()` works as the trainer expects (trainer.py:72,81).  CUDA tensors only.
 """
 import torch
@@ -58,7 +58,7 @@ class CrossEntropyLoss2d(nn.Module):
 
     def forward(self, output, target):
         if not output.is_cuda:
-            raise RuntimeError("seg_b200 losses run on a B200 only; there is no CPU fallback")
+            raise RuntimeError("seg_b200 losses run on an H100 only; there is no CPU fallback")
         return _CEFn.apply(output, target, self.ignore_index)
 
 
@@ -96,7 +96,7 @@ class DiceLoss(nn.Module):
 
     def forward(self, output, target):
         if not output.is_cuda:
-            raise RuntimeError("seg_b200 losses run on a B200 only; there is no CPU fallback")
+            raise RuntimeError("seg_b200 losses run on an H100 only; there is no CPU fallback")
         target = _dice_fix_target_(target, self.ignore_index)
         return _DiceFn.apply(output, target.contiguous(), float(self.smooth))
 
@@ -139,5 +139,5 @@ class LovaszSoftmax(nn.Module):
 
     def forward(self, output, target):
         if not output.is_cuda:
-            raise RuntimeError("seg_b200 losses run on a B200 only; there is no CPU fallback")
+            raise RuntimeError("seg_b200 losses run on an H100 only; there is no CPU fallback")
         return _LovaszFn.apply(output, target, self.ignore_index)

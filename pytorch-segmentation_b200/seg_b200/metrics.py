@@ -13,7 +13,7 @@ from . import ops
 
 def eval_metrics(output, target, num_class):
     if not output.is_cuda:
-        raise RuntimeError("seg_b200.eval_metrics runs on a B200 only; there is no CPU fallback")
+        raise RuntimeError("seg_b200.eval_metrics runs on an H100 only; there is no CPU fallback")
     v = ops.eval_metrics_nchw(output.detach().contiguous().float(), target.contiguous(), num_class).cpu().numpy()
     K = num_class
     correct, labeled = v[0], v[1]

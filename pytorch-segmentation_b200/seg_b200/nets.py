@@ -1,4 +1,4 @@
-"""B200-native drop-in models for the reference's plugin surface (models/__init__.py registry):
+"""H100-native drop-in models for the reference's plugin surface (models/__init__.py registry):
 
     DeepLab(num_classes, in_channels=3, backbone='xception',  pretrained=None, output_stride=16, freeze_bn=False, **_)
     PSPNet (num_classes, in_channels=3, backbone='resnet152', pretrained=None, use_aux=True,   freeze_bn=False, **_)
@@ -13,7 +13,7 @@ returns `(out, aux)` in training) as models/deeplabv3_plus.py:336-377 and models
 BaseTrainer (base/base_trainer.py:46-57), torch.optim.SGD, checkpoints and `convert_model` keep working.
 
 The nn.Conv2d / nn.BatchNorm2d children are PARAMETER HOLDERS only: forward never calls them.  `forward` runs the
-hand-written sm_100a kernels through `engine.Tape`; gradients reach the parameters through one autograd.Function.
+hand-written sm_90a kernels through `engine.Tape`; gradients reach the parameters through one autograd.Function.
 There is no CPU / eager path: a CPU input raises.
 """
 import logging
@@ -578,7 +578,7 @@ class _EngineModel(BaseModel):
 
     def _check_input(self, x):
         if not x.is_cuda:
-            raise RuntimeError("seg_b200 models run on a B200 only; there is no CPU / eager fallback")
+            raise RuntimeError("seg_b200 models run on an H100 only; there is no CPU / eager fallback")
         require_device()
 
     def forward(self, x):

@@ -2,7 +2,7 @@
 
 Activations are NHWC ``torch.bfloat16`` tensors; a tensor may be a channel slice ``buf[..., a:b]`` of a wider
 buffer (that is how concatenation is expressed — no copy).  These wrappers only compute shapes / pitches and pass
-raw pointers; all arithmetic happens in the sm_100a kernels.
+raw pointers; all arithmetic happens in the sm_90a kernels.
 """
 import ctypes
 
@@ -155,8 +155,12 @@ def conv2d_wgrad(dy, x, R, S, stride=1, pad=0, dil=1, out=None, impl=IMPL_AUTO):
         out = torch.zeros((R * S, K, C), dtype=torch.float32, device=x.device)
     d = make_conv_desc(N, H, W, C, K, R, S, stride, pad, dil, ldx=ld(x), ldy=ld(dy))
     assert (d.P, d.Q) == (dy.shape[1], dy.shape[2])
+    nws = lib.load().seg_conv2d_wgrad_workspace_floats(ctypes.byref(d), _impl(impl))
+    if nws < 0:
+        raise RuntimeError(f"seg_conv2d_wgrad_workspace_floats failed: {lib.last_error()}")
+    ws = torch.empty(nws, dtype=torch.float32, device=x.device) if nws > 0 else None
     ev = _prof("wgrad", d)
-    call("seg_conv2d_wgrad", ctypes.byref(d), ptr(dy), ptr(x), ptr(out), _impl(impl), meta=_meta(d))
+    call("seg_conv2d_wgrad", ctypes.byref(d), ptr(dy), ptr(x), ptr(out), ptr(ws), _impl(impl), meta=_meta(d))
     if ev is not None:
         ev.record()
     return out
@@ -520,9 +524,10 @@ def upsample_ce_bwd(logits_lo, target, align_corners, ignore_index, accum, ldx, 
     N, Hi, Wi, C = logits_lo.shape
     _, Ho, Wo = target.shape
     dlo = torch.empty((N, Hi, Wi, C), dtype=torch.float32, device=logits_lo.device)
+    fixed = torch.empty((N, Hi, Wi, C), dtype=torch.int64, device=logits_lo.device)
     dx = torch.empty((N, Hi, Wi, ldx), dtype=torch.bfloat16, device=logits_lo.device)
     call("seg_upsample_ce_bwd", ptr(logits_lo), ptr(target), N, Hi, Wi, Ho, Wo, C, int(align_corners), int(ignore_index),
-         ptr(accum), ptr(gscale), ptr(dlo), ptr(dx), ldx)
+         ptr(accum), ptr(gscale), ptr(dlo), ptr(fixed), ptr(dx), ldx)
     return dx, dlo
 
 

@@ -121,9 +121,8 @@ class FusedTrainStep:
         self.specs = self.wt.specs
         # gradient buckets (world > 1, bucket_mb > 0): contiguous ranges of the flat gradient buffer of ~bucket_mb each, in
         # parameter order; the backward produces them from the last to the first, and each bucket's all-reduce is launched on a
-        # side stream as soon as its last gradient is written (SURVEY.md §8e).  Built and MEASURED SLOWER than one all-reduce
-        # after the backward on NVLink 5 (N=2: 29.3 vs 28.6 ms/step, N=8: 30.1 vs 29.3): the 237 MB exchange costs ~1 ms, and the
-        # NCCL kernels take SMs from the kernels they overlap — so the default (0) is the single call
+        # side stream as soon as its last gradient is written (SURVEY.md §8e).  The NCCL kernels then take SMs from the kernels
+        # they overlap, so the default (0) is the single all-reduce after the backward
         self.bucket_mb = float(bucket_mb)
         self.buckets, self.bucket_of = [], {}
         if world > 1 and bucket_mb > 0:

@@ -8,7 +8,7 @@ bf16-rounded upstream gradient:
 
     oracle : fp32 ATen, the reference's arithmetic (torchvision Bottleneck / models/resnet.py:100-121,
              deeplabv3_plus.py:286-297 ASSP, :323-330 Decoder, pspnet.py:31-38 _PSPModule + classifier)
-    engine : the same block through seg_b200's tape — tcgen05 fprop/dgrad/wgrad, BN statistics in the conv epilogue,
+    engine : the same block through seg_b200's tape — wgmma fprop/dgrad/wgrad, BN statistics in the conv epilogue,
              bn_apply, bn_bwd_reduce / bn_bwd_apply, bilinear, adaptive pool, concat-free buffers — at exactly the shapes
              bench.py launches (M = 4*129^2, 4*65^2, 4*33^2; persistent tiles, one-wave split-K)
 

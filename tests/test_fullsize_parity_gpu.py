@@ -233,7 +233,7 @@ def test_fullsize_parity(name, gpu_out_dir):
             # is then a sum of two bf16 numbers sitting a hair BELOW an exact bf16 rounding tie, and the engine — which adds in
             # fp32 and rounds ONCE, the correctly rounded value of the fp32 result — lands on the lower neighbour where ATen's
             # bf16 path (round the BN output, then round the sum: a true tie, to even) does not: a -6e-4 shrink per residual
-            # block of this un-normalised trunk, measured op by op by tools/eval_block_probe.py (profiles/eval_block_probe_r02.txt).
+            # block of this un-normalised trunk, measured op by op by tools/eval_block_probe.py.
             # Not an error of the kernels (each op's output is the RNE rounding of the fp32 result) and gone as soon as the
             # statistics are not the initialisers' (the `eval` leg below); bounded here, not compared with the control.
             expect(e_max <= 5e-2 and e_rms <= 4e-2, f"{tag} logits error {e_max:.3e} / {e_rms:.3e}")
@@ -294,7 +294,7 @@ def test_fullsize_parity(name, gpu_out_dir):
             log(gpu_out_dir, f"{tag} ENGINE vs bf16-faithful CPU emulation of the same tape ({time.time() - t0:.1f} s): logits max-norm {em:.3e} rms {er:.3e}; "
                              f"loss {a[2]:.6f} vs {emu[2]:.6f}; grad cosine median {ge['cos_median']:.5f} min {ge['cos_min']:.5f} ({ge['cos_min_at']}); "
                              f"running stats worst {re_[wk]:.3e} ({wk})")
-            # measured: in this 100-layer batch-4 network even the fp32 summation ORDER (tcgen05 tiles vs ATen) decorrelates the
+            # measured: in this 100-layer batch-4 network even the fp32 summation ORDER (wgmma tiles vs ATen) decorrelates the
             # logits (rms ~0.9 at C3): informational — the per-block harness (tests/test_block_parity_gpu.py) is the sharp check
             expect(abs(a[2] - emu[2]) <= 0.1 * abs(emu[2]), f"{tag} engine vs emulation loss {a[2]} vs {emu[2]}")
     assert not failures, "\n".join(failures)

@@ -1,7 +1,7 @@
 """Whole-model GPU parity against the CPU oracle (pinned to the reference by tests/golden).
 
 A random-initialised ~100-layer BatchNorm network in TRAIN mode is chaotic: measured on this engine, two bf16
-implementations that differ only in fp32 summation order (tcgen05 vs CUDA-core kernels) already differ by ~2e-2 in the
+implementations that differ only in fp32 summation order (wgmma vs CUDA-core kernels) already differ by ~2e-2 in the
 logits in eval mode, and batch-statistics BN on small maps amplifies any rounding difference by ~1.3x per residual
 block.  So whole-model parity is decomposed into links that can each be checked tightly:
 
@@ -112,7 +112,7 @@ def test_frozen_bn_train_step_parity(kind, nc, backbone, seed, kw, xseed, gpu_ou
     torch.cuda.synchronize()
     tag = f"[frozen-BN {kind}/{backbone}{kw}]"
     e = relerr(out, ref_out)
-    log(gpu_out_dir, f"{tag} logits rel_err vs fp32 oracle {e:.3e}; loss B200={loss.item():.6f} oracle={ref_loss.item():.6f}")
+    log(gpu_out_dir, f"{tag} logits rel_err vs fp32 oracle {e:.3e}; loss H100={loss.item():.6f} oracle={ref_loss.item():.6f}")
     assert e < 5e-2
     assert abs(loss.item() - ref_loss.item()) < 1e-2 * abs(ref_loss.item())
     agree_all, agree_safe = argmax_report(gpu_out_dir, tag, out, ref_out.detach())
@@ -160,7 +160,7 @@ def test_batchstat_train_step(kind, nc, backbone, seed, kw, xseed, gpu_out_dir):
     torch.cuda.synchronize()
     tag = f"[batch-stat {kind}/{backbone}{kw}]"
     log(gpu_out_dir, f"{tag} logits rel_err vs fp32 oracle {relerr(out, ref_out):.3e} (chaotic regime, see module docstring); "
-                     f"loss B200={loss.item():.6f} oracle={ref_loss.item():.6f}")
+                     f"loss H100={loss.item():.6f} oracle={ref_loss.item():.6f}")
     assert abs(loss.item() - ref_loss.item()) < 0.05 * abs(ref_loss.item())
     argmax_report(gpu_out_dir, tag, out, ref_out.detach())
     cos = []
@@ -198,7 +198,7 @@ def test_batchstat_train_step_shallow_trunk(gpu_out_dir):
     torch.cuda.synchronize()
     tag = "[batch-stat deeplab/resnet14]"
     e = relerr(out, ref_out)
-    log(gpu_out_dir, f"{tag} logits rel_err vs fp32 oracle {e:.3e}; loss B200={loss.item():.6f} oracle={ref_loss.item():.6f}")
+    log(gpu_out_dir, f"{tag} logits rel_err vs fp32 oracle {e:.3e}; loss H100={loss.item():.6f} oracle={ref_loss.item():.6f}")
     assert e < 0.15 and abs(loss.item() - ref_loss.item()) < 1e-2 * abs(ref_loss.item())
     agree_all, agree_safe = argmax_report(gpu_out_dir, tag, out, ref_out.detach())
     assert agree_safe == 1.0 and agree_all > 0.9
@@ -226,7 +226,7 @@ def test_eval_forward_and_simt_tc_agree(gpu_out_dir):
         m.conv_impl = IMPL_SIMT
         out_simt = m(x.cuda())
     e1, e2, e3 = relerr(out_tc, ref), relerr(out_simt, ref), relerr(out_tc, out_simt)
-    log(gpu_out_dir, f"[eval deeplab/r50] vs fp32 oracle: tcgen05 path {e1:.3e}; CUDA-core path {e2:.3e}; tcgen05 vs CUDA-core {e3:.3e} (bf16 noise floor)")
+    log(gpu_out_dir, f"[eval deeplab/r50] vs fp32 oracle: wgmma path {e1:.3e}; CUDA-core path {e2:.3e}; wgmma vs CUDA-core {e3:.3e} (bf16 noise floor)")
     assert e1 < 5e-2 and e2 < 5e-2 and e3 < 5e-2
     agree_all, agree_safe = argmax_report(gpu_out_dir, "[eval deeplab/r50]", out_tc, ref)
     assert agree_safe == 1.0 and agree_all > 0.97
@@ -252,7 +252,7 @@ def test_overfit_one_batch(gpu_out_dir):
         l.backward()
         opt.step()
         ref_losses.append(l.item())
-    log(gpu_out_dir, "[overfit] B200 fused-step loss: " + " ".join(f"{v:.3f}" for v in losses[:12]) + f" ... {losses[-1]:.3f}")
+    log(gpu_out_dir, "[overfit] H100 fused-step loss: " + " ".join(f"{v:.3f}" for v in losses[:12]) + f" ... {losses[-1]:.3f}")
     log(gpu_out_dir, "[overfit] oracle SGD loss     : " + " ".join(f"{v:.3f}" for v in ref_losses))
     assert abs(losses[0] - ref_losses[0]) < 0.05 * ref_losses[0]
     assert losses[11] < 0.9 * losses[0] and ref_losses[11] < 0.9 * ref_losses[0]
@@ -309,10 +309,9 @@ def test_plugin_path_after_fused_steps_sees_updated_weights():
 def test_graph_replayed_steps_equal_eager_steps(frozen_bn, gpu_out_dir):
     """CUDA-graph replay of the fused step (train.py: FusedTrainStep(cuda_graph=True)) is the same training as the eager
     step: the capture's two warm-up steps are rolled back, every replay is a fresh step (device-side counters).
-    A second eager trainer is the control for run-to-run noise.  Since round 2 the BatchNorm statistics are accumulated exactly
-    (fp64), so BOTH modes are reproducible: the three loss trajectories must agree to 1e-5 (measured: identical to the last
-    printed digit; round 1's fp32-atomic statistics made two EAGER batch-statistics runs differ by 1e-3) and the three-step
-    parameter updates must be parallel (cosine > 0.9999; round 1 measured 0.74 for graph-vs-eager in batch-statistics mode)."""
+    A second eager trainer is the control for run-to-run noise.  The BatchNorm statistics are accumulated exactly (fp64), so
+    BOTH modes are reproducible: the three loss trajectories must agree to 1e-5 (fp32-atomic statistics made two EAGER
+    batch-statistics runs differ by 1e-3) and the three-step parameter updates must be parallel (cosine > 0.9999)."""
     models = [build("deeplab", 7, "resnet14", 8, output_stride=16) for _ in range(3)]
     sd = models[0][0]
     m_e, m_c, m_g = (m for _, m in models)
@@ -338,3 +337,27 @@ def test_graph_replayed_steps_equal_eager_steps(frozen_bn, gpu_out_dir):
     for (n, a), (_, b) in zip(m_e.named_buffers(), m_g.named_buffers()):
         if n.endswith("num_batches_tracked"):
             assert int(a) == int(b) == (0 if frozen_bn else 3), n
+
+
+def test_training_step_is_bit_reproducible(gpu_out_dir):
+    """Two trainers from the same state on the same batch, graph-replayed as bench.py runs them, must agree BIT FOR BIT after
+    three steps: losses, the flat gradient of the last step, the parameters and the BatchNorm running statistics.  The shape
+    is chosen so the paths whose sums could depend on arrival order all run: split-K weight gradients (few output tiles ->
+    several k-splits, summed in split order) and the fused upsample + CE backward (overlapping bilinear footprints, summed in
+    fixed point)."""
+    models = [build("deeplab", 7, "resnet14", 8, output_stride=16) for _ in range(2)]
+    for _, m in models:
+        m.engine_dropout = False
+        m.train()
+    x, y = synth.make_batch(2, 65, 65, 7, 255, seed=9011)
+    xd, yd = x.cuda(), y.cuda()
+    steppers = [FusedTrainStep(m, lr=0.005, cuda_graph=True) for _, m in models]
+    losses = [[float(s.step(xd, yd)) for _ in range(3)] for s in steppers]
+    torch.cuda.synchronize()
+    log(gpu_out_dir, f"bit-reproducibility: losses {losses[0]} / {losses[1]}")
+    assert losses[0] == losses[1]
+    assert torch.equal(steppers[0].flat_grad, steppers[1].flat_grad), "last step's gradients differ between identical runs"
+    for (n, a), (_, b) in zip(models[0][1].named_parameters(), models[1][1].named_parameters()):
+        assert torch.equal(a, b), n
+    for (n, a), (_, b) in zip(models[0][1].named_buffers(), models[1][1].named_buffers()):
+        assert torch.equal(a, b), n

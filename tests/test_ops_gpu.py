@@ -89,7 +89,7 @@ def test_conv_fwd(shape, impl, gpu_out_dir):
     x, w = conv_inputs(shape)
     ref = F.conv2d(x, w, None, stride, pad, dil)
     wp = ops.pack_weight(w.to(DEV))
-    # fp32 output + statistics: tcgen05 path only (the CUDA-core path reduces the stored bf16 output)
+    # fp32 output + statistics: wgmma path only (the CUDA-core path reduces the stored bf16 output)
     stats = ops.new_stats(K, DEV) if impl == IMPL_TC else None  # zeroed fp64 accumulators
     y = ops.conv2d_fwd(to_nhwc_dev(x), wp, K, ks, ks, stride, pad, dil, out_dtype=torch.float32, stats=stats, impl=impl)
     torch.cuda.synchronize()

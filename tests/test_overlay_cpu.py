@@ -1,19 +1,21 @@
 """The drop-in overlay: with `seg_b200.launch` ordering sys.path as [overlay, reference root], the
-reference's own registries resolve DeepLab / PSPNet / CrossEntropyLoss2d to the B200-native classes and everything else
-to the reference's.  Needs the reference checkout (build container only; skipped on the GPU box)."""
+reference's own registries resolve DeepLab / PSPNet / CrossEntropyLoss2d to the H100-native classes and everything else
+to the reference's.  Runs against the unmodified reference tree that build() packs into oracle/_ref/reference.zip
+(oracle/install_ref.sh), extracted to a temporary directory; skipped where build() had no reference checkout to pack."""
 import os
 import subprocess
 import sys
+import zipfile
 
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = "/root/reference"
+REF_ZIP = os.path.join(ROOT, "oracle", "_ref", "reference.zip")
 
 CODE = r"""
 import sys
 from seg_b200 import launch
-launch.setup_paths('/root/reference')
+launch.setup_paths(sys.argv[1])
 import models, seg_b200
 from utils import losses, lr_scheduler, helpers, metrics
 assert metrics.eval_metrics is seg_b200.eval_metrics and metrics.AverageMeter is seg_b200.AverageMeter
@@ -27,7 +29,8 @@ m = models.DeepLab(19, backbone='resnet50', pretrained=False, freeze_bn=False, f
 assert isinstance(m, BaseModel)
 # exactly what train.py:14-16,26,30 and base_trainer.py:46-57 do
 import json
-cfg = json.load(open('/root/reference/config.json'))
+import os
+cfg = json.load(open(os.path.join(sys.argv[1], 'config.json')))
 cfg['arch']['args']['pretrained'] = False
 cfg['arch']['type'], cfg['arch']['args']['backbone'] = 'PSPNet', 'resnet50'
 model = getattr(models, cfg['arch']['type'])(21, **cfg['arch']['args'])
@@ -49,11 +52,15 @@ print('OVERLAY_OK')
 """
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason="reference checkout not present")
-def test_overlay_resolves_registries():
+@pytest.mark.skipif(not os.path.isfile(REF_ZIP), reason="oracle/_ref/reference.zip not built (build() found no reference checkout)")
+def test_overlay_resolves_registries(tmp_path):
+    ref = tmp_path / "reference"
+    with zipfile.ZipFile(REF_ZIP) as z:
+        z.extractall(ref)
     env = dict(os.environ)
     env["PYTHONPATH"] = os.path.join(ROOT, "pytorch-segmentation_b200")
-    r = subprocess.run([sys.executable, "-W", "ignore", "-c", CODE], env=env, cwd=REF, capture_output=True, text=True, timeout=600)
+    r = subprocess.run([sys.executable, "-W", "ignore", "-c", CODE, str(ref)], env=env, cwd=str(ref), capture_output=True, text=True,
+                       timeout=600)
     assert "OVERLAY_OK" in r.stdout, r.stdout[-2000:] + r.stderr[-4000:]
     assert "Nbr of trainable parameters: 51446762" in r.stdout
 

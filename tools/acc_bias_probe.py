@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Does the tcgen05 fp32 accumulator (TMEM) round or truncate?  Positive bf16 operands, 1x1 conv = GEMM with growing
+"""Does the wgmma fp32 accumulator round or truncate?  Positive bf16 operands, 1x1 conv = GEMM with growing
 reduction length; the engine's fp32 output and cuBLAS's (bf16 operands, fp32 output) are compared with a float64
 product of the same bf16 values: mean SIGNED relative error (a systematic shrink shows up as a negative mean that grows
 with the reduction length) and the rms relative error.
@@ -34,6 +34,6 @@ for signed in (False, True):
         except Exception:
             yt = (a.cuda().float() @ b.cuda().float().t()).double().cpu()
         scale = ref.abs().mean()
-        for name, v in (("tcgen05 (engine)", y), ("cuBLAS bf16->fp32", yt)):
+        for name, v in (("wgmma (engine)", y), ("cuBLAS bf16->fp32", yt)):
             err = (v - ref) / scale
             print(f"signed={int(signed)} K={Kdim:6d} {name:18s}: mean signed rel err {err.mean().item():+.3e}  rms {err.pow(2).mean().sqrt().item():.3e}  (fp32 eps 6e-8)")

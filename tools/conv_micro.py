@@ -52,7 +52,7 @@ def run(shape, kind, iters, stats, impl, beta=0.0):
         e1.record()
         torch.cuda.synchronize()
         us = e0.elapsed_time(e1) * 1e3 / iters
-        print(f"{k:6s} shape={shape} stats={int(bool(stats))} beta={beta} dbg={os.environ.get("SEG_TC_DBG", "0")}: {us:8.2f} us  {flops / us / 1e6:8.1f} TFLOP/s  {byt[k] / us / 1e3:8.1f} GB/s")
+        print(f"{k:6s} shape={shape} stats={int(bool(stats))} beta={beta}: {us:8.2f} us  {flops / us / 1e6:8.1f} TFLOP/s  {byt[k] / us / 1e3:8.1f} GB/s")
 
 
 if __name__ == "__main__":

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Measurement of the §8(f) "next" rows on one B200 (CUDA events, warm-up, synchronised on both sides):
+"""Measurement of the §8(f) "next" rows on one H100 (CUDA events, warm-up, synchronised on both sides):
 
   * input-pipeline tail: `seg_augment_batch_u8` achieved GB/s (algorithmic bytes: uint8 image + label read once, fp32
     image + int64 label written once) next to the reference's CPU tail (oracle/data.py restatement) on the host cores;
