@@ -4,27 +4,31 @@
 // 1x1; SURVEY.md §2.3): models/deeplabv3_plus.py:256 (ASPP d=6/12/18), :312-315 (decoder 3x3), torchvision
 // Bottleneck conv1/conv2/conv3 (layer4 conv2 dilated at deeplabv3_plus.py:47-53), models/resnet.py:43-48.
 //
-// One CTA computes a 128 x BN fp32 tile held in registers.  Warpgroup roles (384 threads):
-//   warpgroup 0  : TMA producer (one thread).  The activation operand is fetched with an IM2COL-mode tensor map: one
-//                  instruction brings 128 output pixels x 64 channels of one filter tap (tap displacement passed as the
-//                  im2col offset, padding = the bounding-box corners, out-of-image taps zero-filled by the TMA unit)
-//                  straight into the 128B-swizzled K-major layout wgmma consumes — the im2col gather happens in the copy
-//                  engine, never in HBM.  Weights come through a tiled 2-D map over the packed [tap][K][C] matrix.
-//   warpgroups 1-2: wgmma consumers; warpgroup 1 + c owns rows 64c..64c+63 of the tile (4 x m64nBNk16 per 64-wide
-//                  k-block, one group kept in flight), then the epilogue: accumulators (+ bias) -> XOR-swizzled staging
-//                  tile in the (now idle) pipeline shared memory -> per-channel sum / sum of squares of the values as
-//                  stored (BatchNorm statistics, fixed order inside the CTA, one fp64 atomic per channel per CTA) ->
-//                  fully coalesced 16-byte global stores (optionally beta-accumulate, optionally onto a strided
-//                  sub-grid of the output).
-// Operand-major variants of the same pipeline:
+// Two kernels share one pipeline: a TMA producer warpgroup feeding an mbarrier ring, wgmma consumer warpgroups with fp32
+// accumulators in registers.  The activation operand is fetched with an IM2COL-mode tensor map: one instruction brings 128
+// output pixels x 64 channels of one filter tap (tap displacement passed as the im2col offset, padding = the bounding-box
+// corners, out-of-image taps zero-filled by the TMA unit) straight into the 128B-swizzled K-major layout wgmma consumes —
+// the im2col gather happens in the copy engine, never in HBM.  Weights come through a tiled 2-D map over the packed
+// [tap][K][C] matrix.
+//
+// conv_gemm_pp<BN, KIND> — fprop (KK) and dgrad (KM): persistent, warp-specialised "ping-pong" kernel.  One CTA per SM walks
+// the 128 x BN output tiles t = blockIdx.x, blockIdx.x + gridDim.x, ...  (384 threads):
+//   warpgroup 0   : TMA producer (one thread) — loads the k-blocks of the CTA's tiles into the ring, tile after tile.
+//   warpgroups 1-2: consumers that take alternate tiles; each owns a whole 128 x BN tile (two m64 wgmma row blocks).  An
+//                   ordered pair of named barriers lets one warpgroup issue MMAs at a time while the other runs the epilogue
+//                   of its previous tile: accumulators (+ bias) -> its private XOR-swizzled staging tile -> per-channel sum /
+//                   sum of squares of the values as stored (BatchNorm statistics, fixed order, one fp64 atomic per channel
+//                   per tile) -> fully coalesced 16-byte global stores (optionally beta-accumulate, optionally onto a strided
+//                   sub-grid of the output).  The epilogue of tile i thus hides under the main loop of tile i + 1.
 //   KK (fprop) : A = activations (K-major),  B = weights  [tap*K + k][c]   (K-major)
 //   KM (dgrad) : A = dY im2col  (K-major),  B = weights  [tap*K + k][c]   (MN-major: c contiguous).  Stride 1: taps
 //                flipped.  Stride s > 1: the input pixels are split into s*s parity classes; each class is a stride-1
 //                gather over dY with only the taps whose parity matches, written to its strided sub-grid of dX —
 //                no wasted MACs on inserted zeros.
-//   MM (wgrad) : A = dY [pixel][k] (MN-major), B = X im2col [pixel][c] (MN-major), contraction over pixels,
-//                split-K over pixel blocks: each split stores its partial tile to a workspace [split][tap][k][c] and a
-//                second kernel adds the splits to dW[tap][k][c] in split order — bit-reproducible, unlike atomics.
+// conv_gemm_wgrad<BN> — wgrad (MM): one 128 x BN tile per CTA, the two consumer warpgroups splitting its rows.
+//   A = dY [pixel][k] (MN-major), B = X im2col [pixel][c] (MN-major), contraction over pixels, split-K over pixel blocks
+//   sized to one wave: each split stores its partial tile to a workspace [split][tap][k][c] and a second kernel adds the
+//   splits to dW[tap][k][c] in split order — bit-reproducible, unlike atomics.
 #include <cuda.h>
 #include <mutex>
 #include <stdlib.h>
@@ -40,10 +44,15 @@ using namespace ptx;
 constexpr int BM = 128;
 constexpr int BK = 64;  // elements per k-block = 128 bytes of bf16
 constexpr int A_BYTES = BM * 128;
-constexpr int KIND_KK = 0, KIND_KM = 1, KIND_MM = 2;
+constexpr int KIND_KK = 0, KIND_KM = 1;
 constexpr int NTHREADS = 384;
 constexpr int NCONS = 256;  // consumer threads (warpgroups 1 and 2)
 constexpr int MAXT = 49;
+
+// named barriers (0 is __syncthreads)
+constexpr int BAR_CONSUMERS = 1;  // both consumer warpgroups (256 threads)
+constexpr int BAR_ORDER = 2;      // 2 + c: consumer c may issue its MMAs (ping-pong kernel)
+constexpr int BAR_WG = 4;         // 4 + c: the 128 threads of consumer c (ping-pong kernel)
 
 struct TcParams {
   CUtensorMap mapA;  // KK/KM: activation-side operand ; MM: dY 2-D
@@ -67,28 +76,21 @@ struct TcParams {
   const float* bias;
   double* stats;     // [2*Ncols] or null, ZERO at launch: per-channel sum / sum of squares of the output (BatchNorm batch
                      // statistics), accumulated with fp64 atomics (see the epilogue)
+  int stat_rows;     // rows per group of the statistics fold (32, 64 or 128; see stat_rows_for)
   unsigned* stat_ticket;   // SyncBN only: one zeroed word counting finished CTAs
   SyncDesc sync;           // world > 0: SyncBN — the last CTA pushes the finished totals to every peer (seg_sync.cuh)
   // strided sub-grid output (stride>1 dgrad): row (n,i,j) -> pixel (n, i*osy+opy, j*osx+opx) of an out_H x out_W map
   int out_strided, out_H, out_W, osy, osx, opy, opx;
+  // KK/KM: tile t covers rows (t / n_tiles) * BM and columns (t % n_tiles) * BN — the column block runs fastest, so the
+  // CTAs working at the same time share their activation rows in L2 and each row block comes from HBM once, however many
+  // column blocks the layer has (with the row block fastest, every column block would stream the whole activation
+  // operand again — 71 MB for layer 4's 2048-channel 1x1 convs, more than the 50 MB L2)
+  int n_tiles, tiles;
   // MM only
   int kblocks_total, kblocks_per_split;
   float* dw;
   int dw_K, dw_C;
   float* ws;  // split-K partials [split][tap][dw_K][dw_C]; null with one split (the tile is added to dW directly)
-};
-
-// Pipeline stages per tile width: one CTA per SM (384 threads, up to 128 accumulator registers per consumer thread), so
-// the ring takes most of the 227 KB; the fp32 staging tile of the epilogue (128 x BN x 4 B) reuses it.
-template <int BN>
-struct Cfg {
-  static constexpr int B_BYTES = BN * 128;
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGES = BN == 64 ? 6 : (BN == 128 ? 5 : 4);
-  static constexpr int STAT_BYTES = 2 * 2 * BN * 4;  // [row group][sum, sum of squares][column] fp32
-  static constexpr int SMEM = STAGES * STAGE_BYTES + STAT_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
-  static_assert(STAGES * STAGE_BYTES >= BM * BN * 4, "staging tile must fit in the pipeline ring");
-  static_assert(SMEM <= 227 * 1024, "shared memory per block");
 };
 
 __device__ __forceinline__ void row_to_coords(int m, int PQ, int Q, int stride, int lower_h, int lower_w, int& n, int& h,
@@ -108,36 +110,341 @@ __device__ __forceinline__ void wgmma_tile(float* acc, uint64_t adesc, uint64_t 
   else wgmma_m64n256k16<TA, TB>(acc, adesc, bdesc, accumulate);
 }
 
-__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+// The TMA loads of one k-block (ring stage `st`) of a KK / KM tile.
+template <int BN, int KIND>
+__device__ __forceinline__ void load_kblock(const TcParams& p, uint32_t a_dst, uint32_t bar, int kc, int wtap, uint16_t oh,
+                                            uint16_t ow, int n_img, int h0, int w0, int m0, int n0) {
+  const uint32_t b_dst = a_dst + A_BYTES;
+  if (p.x_im2col)
+    tma_load_im2col_4d(a_dst, &p.mapA, bar, kc * BK, w0, h0, n_img, ow, oh);
+  else
+    tma_load_2d(a_dst, &p.mapA, bar, kc * BK, m0);
+  if (KIND == KIND_KK) {
+    tma_load_2d(b_dst, &p.mapB, bar, kc * BK, wtap * p.brows_per_tap + n0);  // box [BN][64]
+  } else {
+#pragma unroll
+    for (int j = 0; j < BN / 64; ++j)  // boxes [64 k-rows][64 cols]
+      tma_load_2d(b_dst + j * 8192, &p.mapB, bar, n0 + j * 64, wtap * p.brows_per_tap + kc * BK);
+  }
+}
+
+// The accumulators of one m64 x BN wgmma row block (+ bias) -> rows rbase.. of the XOR-swizzled staging tile
+// [128 rows][BN * esize bytes]; with acc1, also those of the row block below it (rows rbase + 64..).  `bias`: the tile's BN
+// bias values in shared memory, zero past the layer's last column (or null).
+template <int BN>
+__device__ __forceinline__ void stage_acc(const float* acc, const float* acc1, uint8_t* stage, int rbase, int warp, int lane,
+                                          const float* bias, bool out_f32) {
+  const int esize = out_f32 ? 4 : 2;
+  const int CPR = BN * esize / 16;  // 16-byte chunks per staged row
+  const int swz = (CPR >= 32 ? 31 : CPR - 1);
+  const int r0 = rbase + warp * 16 + (lane >> 2);
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    const int col = j * 8 + 2 * (lane & 3);
+    float b0 = 0.f, b1 = 0.f;
+    if (bias) {
+      b0 = bias[col];
+      b1 = bias[col + 1];
+    }
+#pragma unroll
+    for (int h = 0; h < 4; ++h) {
+      if (h >= 2 && !acc1) break;
+      const float* a = h < 2 ? acc : acc1;
+      const int r = r0 + 8 * (h & 1) + 32 * (h & 2);
+      const float x0 = a[4 * j + 2 * (h & 1)] + b0, x1 = a[4 * j + 2 * (h & 1) + 1] + b1;
+      const int byte = col * esize;
+      uint8_t* dst = stage + (size_t)r * (BN * esize) + ((((byte >> 4) ^ (r & swz))) << 4) + (byte & 15);
+      if (out_f32)
+        *reinterpret_cast<float2*>(dst) = make_float2(x0, x1);
+      else
+        *reinterpret_cast<__nv_bfloat162*>(dst) = __floats2bfloat162_rn(x0, x1);
+    }
+  }
+}
+
+// ================================ fprop / dgrad: persistent ping-pong kernel ================================
+
+// Ring depth per tile width.  Each consumer has a private staging tile of 128 rows x 256 B (BN * esize <= 256: fp32 outputs
+// take BN = 64) and a private statistics scratch, because the ring never idles and cannot double as the staging area.
+template <int BN>
+struct PPCfg {
+  static_assert(BN == 64 || BN == 128, "ping-pong tile width");
+  static constexpr int B_BYTES = BN * 128;
+  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+  static constexpr int STAGES = BN == 64 ? 6 : 4;
+  static constexpr int RING = STAGES * STAGE_BYTES;
+  static constexpr int STG_BYTES = BM * 256;
+  static constexpr int MAXG = BM / 32;                  // statistics row groups per tile (stat_rows >= 32)
+  static constexpr int STAT_BYTES = MAXG * 2 * BN * 4 + BN * 4;  // [group][sum, sum of squares][column] fp32 + [column] bias
+  static constexpr int SMEM = RING + 2 * (STG_BYTES + STAT_BYTES) + 1024 /*align slack*/ + 256 /*barriers*/;
+  static_assert(16 * STAGES + 8 <= 256, "barrier area");
+  static_assert(SMEM <= 227 * 1024, "shared memory per block");
+};
 
 template <int BN, int KIND>
-__global__ void __launch_bounds__(NTHREADS, 1) conv_gemm_tc(const __grid_constant__ TcParams p) {
+__global__ void __launch_bounds__(NTHREADS, 1) conv_gemm_pp(const __grid_constant__ TcParams p) {
+  using C = PPCfg<BN>;
+  constexpr int STAGES = C::STAGES;
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t raw_addr = smem_u32(smem_raw);
+  const uint32_t smem0 = (raw_addr + 1023u) & ~1023u;  // 1024-B alignment for SWIZZLE_128B atoms
+  uint8_t* smem_gen = smem_raw + (smem0 - raw_addr);
+  const uint32_t bar0 = smem0 + C::RING + 2 * (C::STG_BYTES + C::STAT_BYTES);
+  auto full_bar = [&](int s) { return bar0 + 8u * s; };
+  auto empty_bar = [&](int s) { return bar0 + 8u * (STAGES + s); };
+  volatile int* flag_sm = reinterpret_cast<volatile int*>(smem_gen + (bar0 - smem0) + 16 * STAGES);
+
+  const int num_iters = p.taps * p.kchunks;  // k-blocks per tile (0: a parity class no tap reaches — zeros are written)
+  const int grid = gridDim.x;
+  const int ntiles = (p.tiles - (int)blockIdx.x + grid - 1) / grid;  // this CTA's tiles: blockIdx.x + j * grid
+
+  if (threadIdx.x == 0) {
+    prefetch_tmap(&p.mapA);
+    prefetch_tmap(&p.mapB);
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(full_bar(s), 1);
+      mbar_init(empty_bar(s), 4);  // each stage is consumed by one warpgroup: one arrival per warp
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+  pdl_wait();  // setup above overlapped the previous kernel's tail; global memory is touched only from here on
+
+  if (threadIdx.x < 128) {
+    // =============================== TMA producer ===============================
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0 && num_iters > 0) {
+      int it = 0;
+      for (int j = 0; j < ntiles; ++j) {
+        const int t = blockIdx.x + j * grid;
+        const int m0 = (t / p.n_tiles) * BM, n0 = (t % p.n_tiles) * BN;
+        int n_img = 0, h0 = 0, w0 = 0;
+        if (p.x_im2col) row_to_coords(m0, p.PQ, p.Q, p.stride, p.lower_h, p.lower_w, n_img, h0, w0);
+        for (int tap = 0; tap < p.taps; ++tap) {
+          const int wtap = p.tap_wt[tap];
+          const uint16_t oh = (uint16_t)p.tap_oh[tap], ow = (uint16_t)p.tap_ow[tap];
+          for (int kc = 0; kc < p.kchunks; ++kc, ++it) {
+            const int st = it % STAGES;
+            mbar_wait_nocall(empty_bar(st), ((it / STAGES) & 1) ^ 1u);
+            mbar_arrive_expect_tx(full_bar(st), C::STAGE_BYTES);
+            load_kblock<BN, KIND>(p, smem0 + st * C::STAGE_BYTES, full_bar(st), kc, wtap, oh, ow, n_img, h0, w0, m0, n0);
+          }
+        }
+      }
+    }
+    return;
+  }
+
+  // =============================== wgmma consumers ===============================
+  setmaxnreg_inc<232>();
+  const int cw = (threadIdx.x - 128) >> 7;  // consumer warpgroup: local tiles j = cw, cw + 2, ...
+  const int tid = threadIdx.x & 127;
+  const int warp = tid >> 5, lane = tid & 31;
+  uint8_t* stage = smem_gen + C::RING + cw * C::STG_BYTES;
+  float* stat_sm = reinterpret_cast<float*>(smem_gen + C::RING + 2 * C::STG_BYTES + cw * C::STAT_BYTES);
+  float* bias_sm = stat_sm + C::MAXG * 2 * BN;
+  const bool out_f32 = p.out_dtype != SEG_DT_BF16;
+  const int esize = out_f32 ? 4 : 2;
+  const int CPR = BN * esize / 16;  // 16-byte chunks per staged row
+  const int swz = (CPR >= 32 ? 31 : CPR - 1);
+  auto wg_sync = [&] { named_sync(BAR_WG + cw, 128); };
+
+  for (int j = cw; j < ntiles; j += 2) {
+    const int t = blockIdx.x + j * grid;
+    const int m0 = (t / p.n_tiles) * BM, n0 = (t % p.n_tiles) * BN;
+    float acc0[BN / 2], acc1[BN / 2];  // rows 0..63 and 64..127 of the tile
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc0[i] = acc1[i] = 0.f;
+
+    // ---- main loop: only after the other consumer has issued every MMA of local tile j - 1 ----
+    if (j > 0) named_sync(BAR_ORDER + cw, NCONS);
+    {
+      constexpr int TB = (KIND == KIND_KK) ? 0 : 1;
+      const int it0 = j * num_iters;  // ring position of this tile's first k-block: the producer loads tiles in order
+      for (int i = 0; i < num_iters; ++i) {
+        const int it = it0 + i;
+        const int st = it % STAGES;
+        mbar_wait_nocall(full_bar(st), (it / STAGES) & 1);
+        const uint32_t a_addr = smem0 + st * C::STAGE_BYTES;  // K-major: 128 rows x 128 B, rows 64.. at +8192
+        const uint32_t b_addr = a_addr + A_BYTES;
+        // K-major: 8-row atoms 1024 B apart, K advance = 32 B inside the swizzle atom.
+        // MN-major: 64-wide MN blocks one box (8192 B) apart, 8-row K groups 1024 B apart, K advance = 16 rows.
+        const uint64_t adesc0 = make_smem_desc_sw128(a_addr, 16, 1024);
+        const uint64_t adesc1 = make_smem_desc_sw128(a_addr + 8192, 16, 1024);
+        const uint64_t bdesc0 = make_smem_desc_sw128(b_addr, TB ? 8192 : 16, 1024);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k) {
+          const uint64_t bdesc = bdesc0 + (uint64_t)(TB ? (k * 2048 >> 4) : (k * 32 >> 4));
+          wgmma_tile<BN, 0, TB>(acc0, adesc0 + (uint64_t)(k * 32 >> 4), bdesc, 1u);
+          wgmma_tile<BN, 0, TB>(acc1, adesc1 + (uint64_t)(k * 32 >> 4), bdesc, 1u);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();  // the previous k-block's MMAs have retired: its stage goes back to the producer
+        __syncwarp();
+        if (i > 0 && lane == 0) mbar_arrive(empty_bar((it - 1) % STAGES));
+      }
+      if (j + 1 < ntiles) named_arrive(BAR_ORDER + (cw ^ 1), NCONS);  // the other consumer may start its main loop
+      wgmma_wait<0>();
+      __syncwarp();
+      if (num_iters > 0 && lane == 0) mbar_arrive(empty_bar((it0 + num_iters - 1) % STAGES));
+    }
+
+    // -------- phase 1: registers -> (bias) -> swizzled staging tile --------
+    const int ncols_tile = min(BN, p.Ncols - n0);
+    if (p.bias && tid < BN) bias_sm[tid] = tid < ncols_tile ? __ldg(p.bias + n0 + tid) : 0.f;  // read in phase 1 only
+    wg_sync();  // the previous tile's epilogue is done with the staging tile and the statistics scratch
+    stage_acc<BN>(acc0, acc1, stage, 0, warp, lane, p.bias ? bias_sm : nullptr, out_f32);
+    wg_sync();
+
+    // -------- phase 2: BN statistics of the tile AS STORED (bf16-rounded for bf16 outputs — exactly what bn_apply
+    //          normalises): per column, fp32 sums over groups of stat_rows rows, the groups added in order in phase 4.
+    //          The grouping depends on the layer (stat_rows), never on the tile width, and a column's groups are shared
+    //          by up to 128 / BN threads. --------
+    const int ngroups = BM / p.stat_rows;
+    if (p.stats) {
+      const int parts = min(128 / BN, ngroups);  // threads per column
+      const int rpp = BM / parts;                // rows per thread
+      const int c = tid % BN, part = tid / BN;
+      const int rvalid = min(BM, p.M - m0);
+      if (part < parts) {
+        const int byte = c * esize;
+        int g = part * rpp / p.stat_rows;
+        for (int rg = part * rpp; rg < (part + 1) * rpp; rg += p.stat_rows, ++g) {
+          float s1 = 0.f, s2 = 0.f;
+          const int rend = min(rg + p.stat_rows, rvalid);
+          for (int r = rg; r < rend; ++r) {
+            const uint8_t* src = stage + (size_t)r * (BN * esize) + ((((byte >> 4) ^ (r & swz))) << 4) + (byte & 15);
+            const float x = out_f32 ? *reinterpret_cast<const float*>(src) : bf2f(*reinterpret_cast<const __nv_bfloat16*>(src));
+            s1 += x;
+            s2 = fmaf(x, x, s2);
+          }
+          stat_sm[(g * 2 + 0) * BN + c] = s1;
+          stat_sm[(g * 2 + 1) * BN + c] = s2;
+        }
+      }
+    }
+
+    // -------- phase 3: coalesced 16-byte stores of the staged tile --------
+    {
+      const int nchunks = (ncols_tile * esize + 15) >> 4;  // 16-byte chunks that hold valid data
+      const bool vec_ok = ((p.ldo * esize) & 15) == 0 && ((reinterpret_cast<uintptr_t>(p.out) + (size_t)n0 * esize) & 15) == 0;
+      for (int idx = tid; idx < BM * CPR; idx += 128) {
+        const int tr = idx / CPR;
+        const int c16 = idx - tr * CPR;
+        if (c16 >= nchunks) continue;
+        const int grow = m0 + tr;
+        if (grow >= p.M) continue;
+        long long pixel = grow;
+        if (p.out_strided) {
+          const int n = grow / p.PQ;
+          const int rem = grow - n * p.PQ;
+          const int i = rem / p.Q, jj = rem - i * p.Q;
+          pixel = ((long long)n * p.out_H + (i * p.osy + p.opy)) * p.out_W + (jj * p.osx + p.opx);
+        }
+        const uint8_t* src = stage + (size_t)tr * (BN * esize) + ((c16 ^ (tr & swz)) << 4);
+        uint8_t* dst = reinterpret_cast<uint8_t*>(p.out) + ((size_t)pixel * p.ldo + n0) * esize + ((size_t)c16 << 4);
+        const int first_col = (c16 << 4) / esize;
+        const bool full = first_col + 16 / esize <= ncols_tile;
+        if (!out_f32) {
+          bf16x8 val = *reinterpret_cast<const bf16x8*>(src);
+          if (vec_ok && full) {
+            if (p.beta != 0.f) {
+              float a[8], b[8];
+              unpack8(val, a);
+              unpack8(*reinterpret_cast<const bf16x8*>(dst), b);
+#pragma unroll
+              for (int k = 0; k < 8; ++k) a[k] += p.beta * b[k];
+              val = pack8(a);
+            }
+            *reinterpret_cast<bf16x8*>(dst) = val;
+          } else {
+            float a[8];
+            unpack8(val, a);
+            __nv_bfloat16* d = reinterpret_cast<__nv_bfloat16*>(dst);
+            for (int k = 0; k < 8; ++k)
+              if (first_col + k < ncols_tile) {
+                float o = a[k];
+                if (p.beta != 0.f) o += p.beta * bf2f(d[k]);
+                d[k] = f2bf(o);
+              }
+          }
+        } else {
+          const float4 val = *reinterpret_cast<const float4*>(src);
+          const float a[4] = {val.x, val.y, val.z, val.w};
+          float* d = reinterpret_cast<float*>(dst);
+          if (vec_ok && full && p.beta == 0.f) {
+            *reinterpret_cast<float4*>(d) = val;
+          } else {
+            for (int k = 0; k < 4; ++k)
+              if (first_col + k < ncols_tile) d[k] = (p.beta != 0.f) ? a[k] + p.beta * d[k] : a[k];
+          }
+        }
+      }
+    }
+    if (j == ntiles - 1 && tid == 0) pdl_trigger();  // the CTA's last tile is stored
+
+    // -------- phase 4: this tile's column sums are added to the layer's totals with fp64 atomics.  Each contribution is an
+    //          fp32 value, so the fp64 sum of the <= few thousand partials of a channel is EXACT (no rounding at all) whenever
+    //          their exponents span less than 2^17 — then the order of the atomics cannot matter and the statistics are
+    //          bit-reproducible (fp32 atomics were not, and the batch-2 image-pooling BatchNorm amplified that into 3-5 %
+    //          logit differences between runs).  (Beyond that span the order can move the fp64 sum by one fp64 ulp —
+    //          invisible after the rounding to fp32.) --------
+    if (p.stats) {
+      wg_sync();
+      if (tid < ncols_tile) {
+        float a = 0.f, b = 0.f;
+        for (int g = 0; g < ngroups; ++g) {
+          a += stat_sm[(g * 2 + 0) * BN + tid];
+          b += stat_sm[(g * 2 + 1) * BN + tid];
+        }
+        atomicAdd(p.stats + n0 + tid, (double)a);
+        atomicAdd(p.stats + p.Ncols + n0 + tid, (double)b);
+      }
+    }
+  }
+
+  // SyncBN: one ticket per CTA, taken after both consumers' atomics of every tile of the CTA
+  if (p.stats && p.sync.world > 0)
+    sync_push_when_last<false>(p.sync, p.stats, 2 * p.Ncols, p.stat_ticket, gridDim.x, threadIdx.x - 128, NCONS,
+                               [] { named_sync(BAR_CONSUMERS, NCONS); }, flag_sm);
+}
+
+// ================================ wgrad: one tile per CTA ================================
+
+// Pipeline stages per tile width: one CTA per SM (384 threads, up to 128 accumulator registers per consumer thread), so
+// the ring takes most of the 227 KB; the fp32 staging tile of the epilogue (128 x BN x 4 B) reuses it.
+template <int BN>
+struct Cfg {
+  static constexpr int B_BYTES = BN * 128;
+  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+  static constexpr int STAGES = BN == 64 ? 6 : (BN == 128 ? 5 : 4);
+  static constexpr int SMEM = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+  static_assert(STAGES * STAGE_BYTES >= BM * BN * 4, "staging tile must fit in the pipeline ring");
+  static_assert(SMEM <= 227 * 1024, "shared memory per block");
+};
+
+template <int BN>
+__global__ void __launch_bounds__(NTHREADS, 1) conv_gemm_wgrad(const __grid_constant__ TcParams p) {
   using C = Cfg<BN>;
   constexpr int STAGES = C::STAGES;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
   const uint32_t smem0 = (raw_addr + 1023u) & ~1023u;  // 1024-B alignment for SWIZZLE_128B atoms
   uint8_t* smem_gen = smem_raw + (smem0 - raw_addr);
-  float* stat_sm = reinterpret_cast<float*>(smem_gen + STAGES * C::STAGE_BYTES);
-  const uint32_t bar0 = smem0 + STAGES * C::STAGE_BYTES + C::STAT_BYTES;
+  const uint32_t bar0 = smem0 + STAGES * C::STAGE_BYTES;
   auto full_bar = [&](int s) { return bar0 + 8u * s; };
   auto empty_bar = [&](int s) { return bar0 + 8u * (STAGES + s); };
-  volatile int* flag_sm = reinterpret_cast<volatile int*>(smem_gen + STAGES * C::STAGE_BYTES + C::STAT_BYTES + 8 * 2 * STAGES);
 
   const int m0 = blockIdx.x * BM;
   const int n0 = blockIdx.y * BN;
 
   // ---- iteration space of the k loop ----
-  int tap_mm = 0, kb_begin = 0, kb_end = 0, num_iters;
-  if (KIND == KIND_MM) {
-    tap_mm = blockIdx.z % p.taps;
-    const int split = blockIdx.z / p.taps;
-    kb_begin = split * p.kblocks_per_split;
-    kb_end = min(kb_begin + p.kblocks_per_split, p.kblocks_total);
-    num_iters = max(kb_end - kb_begin, 0);
-  } else {
-    num_iters = p.taps * p.kchunks;
-  }
+  const int tap_mm = blockIdx.z % p.taps;
+  const int split = blockIdx.z / p.taps;
+  const int kb_begin = split * p.kblocks_per_split;
+  const int kb_end = min(kb_begin + p.kblocks_per_split, p.kblocks_total);
+  const int num_iters = max(kb_end - kb_begin, 0);
 
   if (threadIdx.x == 0) {
     prefetch_tmap(&p.mapA);
@@ -154,56 +461,27 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_gemm_tc(const __grid_constan
   if (threadIdx.x < 128) {
     // =============================== TMA producer ===============================
     if (threadIdx.x == 0 && num_iters > 0) {
-      if (KIND != KIND_MM) {
-        int n_img = 0, h0 = 0, w0 = 0;
-        if (p.x_im2col) row_to_coords(m0, p.PQ, p.Q, p.stride, p.lower_h, p.lower_w, n_img, h0, w0);
-        int it = 0;
-        for (int tap = 0; tap < p.taps; ++tap) {
-          const int wtap = p.tap_wt[tap];
-          const uint16_t oh = (uint16_t)p.tap_oh[tap], ow = (uint16_t)p.tap_ow[tap];
-          for (int kc = 0; kc < p.kchunks; ++kc, ++it) {
-            const int st = it % STAGES;
-            const uint32_t ph = (it / STAGES) & 1;
-            mbar_wait_nocall(empty_bar(st), ph ^ 1u);
-            const uint32_t a_dst = smem0 + st * C::STAGE_BYTES;
-            const uint32_t b_dst = a_dst + A_BYTES;
-            mbar_arrive_expect_tx(full_bar(st), C::STAGE_BYTES);
-            if (p.x_im2col)
-              tma_load_im2col_4d(a_dst, &p.mapA, full_bar(st), kc * BK, w0, h0, n_img, ow, oh);
-            else
-              tma_load_2d(a_dst, &p.mapA, full_bar(st), kc * BK, m0);
-            if (KIND == KIND_KK) {
-              tma_load_2d(b_dst, &p.mapB, full_bar(st), kc * BK, wtap * p.brows_per_tap + n0);  // box [BN][64]
-            } else {
+      const uint16_t oh = (uint16_t)p.tap_oh[tap_mm], ow = (uint16_t)p.tap_ow[tap_mm];
+      int it = 0;
+      for (int kb = kb_begin; kb < kb_end; ++kb, ++it) {
+        const int st = it % STAGES;
+        const uint32_t ph = (it / STAGES) & 1;
+        mbar_wait_nocall(empty_bar(st), ph ^ 1u);
+        const uint32_t a_dst = smem0 + st * C::STAGE_BYTES;
+        const uint32_t b_dst = a_dst + A_BYTES;
+        const int pix0 = kb * BK;
+        mbar_arrive_expect_tx(full_bar(st), C::STAGE_BYTES);
+        tma_load_2d(a_dst, &p.mapA, full_bar(st), m0, pix0);  // dY box [64 pixels][64 k]
+        tma_load_2d(a_dst + 8192, &p.mapA, full_bar(st), m0 + 64, pix0);
+        if (p.x_im2col) {
+          int n_img, h0, w0;
+          row_to_coords(pix0, p.PQ, p.Q, p.stride, p.lower_h, p.lower_w, n_img, h0, w0);
 #pragma unroll
-              for (int j = 0; j < BN / 64; ++j)  // boxes [64 k-rows][64 cols]
-                tma_load_2d(b_dst + j * 8192, &p.mapB, full_bar(st), n0 + j * 64, wtap * p.brows_per_tap + kc * BK);
-            }
-          }
-        }
-      } else {
-        const uint16_t oh = (uint16_t)p.tap_oh[tap_mm], ow = (uint16_t)p.tap_ow[tap_mm];
-        int it = 0;
-        for (int kb = kb_begin; kb < kb_end; ++kb, ++it) {
-          const int st = it % STAGES;
-          const uint32_t ph = (it / STAGES) & 1;
-          mbar_wait_nocall(empty_bar(st), ph ^ 1u);
-          const uint32_t a_dst = smem0 + st * C::STAGE_BYTES;
-          const uint32_t b_dst = a_dst + A_BYTES;
-          const int pix0 = kb * BK;
-          mbar_arrive_expect_tx(full_bar(st), C::STAGE_BYTES);
-          tma_load_2d(a_dst, &p.mapA, full_bar(st), m0, pix0);  // dY box [64 pixels][64 k]
-          tma_load_2d(a_dst + 8192, &p.mapA, full_bar(st), m0 + 64, pix0);
-          if (p.x_im2col) {
-            int n_img, h0, w0;
-            row_to_coords(pix0, p.PQ, p.Q, p.stride, p.lower_h, p.lower_w, n_img, h0, w0);
+          for (int j = 0; j < BN / 64; ++j)
+            tma_load_im2col_4d(b_dst + j * 8192, &p.mapB, full_bar(st), n0 + j * 64, w0, h0, n_img, ow, oh);
+        } else {
 #pragma unroll
-            for (int j = 0; j < BN / 64; ++j)
-              tma_load_im2col_4d(b_dst + j * 8192, &p.mapB, full_bar(st), n0 + j * 64, w0, h0, n_img, ow, oh);
-          } else {
-#pragma unroll
-            for (int j = 0; j < BN / 64; ++j) tma_load_2d(b_dst + j * 8192, &p.mapB, full_bar(st), n0 + j * 64, pix0);
-          }
+          for (int j = 0; j < BN / 64; ++j) tma_load_2d(b_dst + j * 8192, &p.mapB, full_bar(st), n0 + j * 64, pix0);
         }
       }
     }
@@ -211,201 +489,65 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_gemm_tc(const __grid_constan
   }
 
   // =============================== wgmma consumers ===============================
-  if (KIND == KIND_MM && num_iters == 0) return;  // an empty split adds nothing (uniform across the consumers)
+  if (num_iters == 0) return;  // an empty split adds nothing (uniform across the consumers)
   const int ctid = threadIdx.x - 128;  // 0..255
   const int cw = ctid >> 7;            // consumer warpgroup: rows 64*cw.. of the tile
   const int warp = (ctid >> 5) & 3, lane = ctid & 31;
   float acc[BN / 2];
 #pragma unroll
   for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-  {
-    constexpr int TA = (KIND == KIND_MM) ? 1 : 0;
-    constexpr int TB = (KIND == KIND_KK) ? 0 : 1;
-    for (int it = 0; it < num_iters; ++it) {
-      const int st = it % STAGES;
-      mbar_wait_nocall(full_bar(st), (it / STAGES) & 1);
-      const uint32_t a_addr = smem0 + st * C::STAGE_BYTES + cw * 8192;  // K-major: 64 rows x 128 B; MN-major: box cw
-      const uint32_t b_addr = smem0 + st * C::STAGE_BYTES + A_BYTES;
-      // K-major: 8-row atoms 1024 B apart, K advance = 32 B inside the swizzle atom.
-      // MN-major: 64-wide MN blocks one box (8192 B) apart, 8-row K groups 1024 B apart, K advance = 16 rows.
-      const uint64_t adesc0 = make_smem_desc_sw128(a_addr, TA ? 8192 : 16, 1024);
-      const uint64_t bdesc0 = make_smem_desc_sw128(b_addr, TB ? 8192 : 16, 1024);
-      wgmma_fence();
+  for (int it = 0; it < num_iters; ++it) {
+    const int st = it % STAGES;
+    mbar_wait_nocall(full_bar(st), (it / STAGES) & 1);
+    const uint32_t a_addr = smem0 + st * C::STAGE_BYTES + cw * 8192;  // MN-major: box cw
+    const uint32_t b_addr = smem0 + st * C::STAGE_BYTES + A_BYTES;
+    // MN-major: 64-wide MN blocks one box (8192 B) apart, 8-row K groups 1024 B apart, K advance = 16 rows.
+    const uint64_t adesc0 = make_smem_desc_sw128(a_addr, 8192, 1024);
+    const uint64_t bdesc0 = make_smem_desc_sw128(b_addr, 8192, 1024);
+    wgmma_fence();
 #pragma unroll
-      for (int k = 0; k < BK / 16; ++k) {
-        const uint64_t adesc = adesc0 + (uint64_t)(TA ? (k * 2048 >> 4) : (k * 32 >> 4));
-        const uint64_t bdesc = bdesc0 + (uint64_t)(TB ? (k * 2048 >> 4) : (k * 32 >> 4));
-        wgmma_tile<BN, TA, TB>(acc, adesc, bdesc, 1u);
-      }
-      wgmma_commit();
-      wgmma_wait<1>();  // the previous k-block's MMAs have retired: its stage goes back to the producer
-      __syncwarp();
-      if (it > 0 && lane == 0) mbar_arrive(empty_bar((it - 1) % STAGES));
-    }
-    wgmma_wait<0>();
+    for (int k = 0; k < BK / 16; ++k)
+      wgmma_tile<BN, 1, 1>(acc, adesc0 + (uint64_t)(k * 2048 >> 4), bdesc0 + (uint64_t)(k * 2048 >> 4), 1u);
+    wgmma_commit();
+    wgmma_wait<1>();  // the previous k-block's MMAs have retired: its stage goes back to the producer
+    __syncwarp();
+    if (it > 0 && lane == 0) mbar_arrive(empty_bar((it - 1) % STAGES));
   }
-  consumer_sync();  // both warpgroups are done reading the ring: it becomes the staging tile
+  wgmma_wait<0>();
+  named_sync(BAR_CONSUMERS, NCONS);  // both warpgroups are done reading the ring: it becomes the staging tile
 
-  // -------- phase 1: registers -> (bias) -> swizzled staging tile [128 rows][BN * esize bytes] --------
-  const bool out_f32 = (KIND == KIND_MM) || p.out_dtype != SEG_DT_BF16;
-  const int esize = out_f32 ? 4 : 2;
-  const int CPR = BN * esize / 16;  // 16-byte chunks per staged row
-  const int swz = (CPR >= 32 ? 31 : CPR - 1);
+  // -------- registers -> swizzled fp32 staging tile [128 rows][BN * 4 bytes] --------
   uint8_t* stage = smem_gen;
   const int ncols_tile = min(BN, p.Ncols - n0);
-  {
-    const int r0 = cw * 64 + warp * 16 + (lane >> 2);
-#pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
-      const int col = j * 8 + 2 * (lane & 3);
-      float b0 = 0.f, b1 = 0.f;
-      if (KIND != KIND_MM && p.bias) {
-        if (col < ncols_tile) b0 = __ldg(p.bias + n0 + col);
-        if (col + 1 < ncols_tile) b1 = __ldg(p.bias + n0 + col + 1);
-      }
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int r = r0 + 8 * h;
-        const float x0 = acc[4 * j + 2 * h] + b0, x1 = acc[4 * j + 2 * h + 1] + b1;
-        const int byte = col * esize;
-        uint8_t* dst = stage + (size_t)r * (BN * esize) + ((((byte >> 4) ^ (r & swz))) << 4) + (byte & 15);
-        if (out_f32)
-          *reinterpret_cast<float2*>(dst) = make_float2(x0, x1);
-        else
-          *reinterpret_cast<__nv_bfloat162*>(dst) = __floats2bfloat162_rn(x0, x1);
-      }
-    }
-  }
-  consumer_sync();
+  stage_acc<BN>(acc, nullptr, stage, cw * 64, warp, lane, nullptr, true);
+  named_sync(BAR_CONSUMERS, NCONS);
 
-  if (KIND == KIND_MM) {
-    // -------- wgrad tile: with one split, added to dW[tap][k][c] (once per element: order-free); with several, stored
-    //          to this split's slice of the workspace for the fixed-order reduction --------
-    float* base = p.ws ? p.ws + (size_t)(blockIdx.z / p.taps) * p.taps * p.dw_K * p.dw_C : p.dw;
-    for (int idx = ctid; idx < BM * CPR; idx += NCONS) {
-      const int tr = idx / CPR, c16 = idx - tr * CPR;
-      const int row = m0 + tr, col0 = c16 * 4;
-      if (row >= p.M || col0 >= ncols_tile) continue;
-      const float4 v = *reinterpret_cast<const float4*>(stage + (size_t)tr * (BN * 4) + ((c16 ^ (tr & swz)) << 4));
-      float* dst = base + ((size_t)tap_mm * p.dw_K + row) * p.dw_C + n0 + col0;
-      const bool vec = col0 + 4 <= ncols_tile && ((reinterpret_cast<uintptr_t>(dst) & 15) == 0);
-      const float a[4] = {v.x, v.y, v.z, v.w};
-      if (p.ws) {
-        if (vec)
-          *reinterpret_cast<float4*>(dst) = v;
-        else
-          for (int i = 0; i < 4; ++i)
-            if (col0 + i < ncols_tile) dst[i] = a[i];
-      } else if (vec) {
-        asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w)
-                     : "memory");
-      } else {
+  // -------- wgrad tile: with one split, added to dW[tap][k][c] (once per element: order-free); with several, stored
+  //          to this split's slice of the workspace for the fixed-order reduction --------
+  const int CPR = BN * 4 / 16;
+  const int swz = (CPR >= 32 ? 31 : CPR - 1);
+  float* base = p.ws ? p.ws + (size_t)split * p.taps * p.dw_K * p.dw_C : p.dw;
+  for (int idx = ctid; idx < BM * CPR; idx += NCONS) {
+    const int tr = idx / CPR, c16 = idx - tr * CPR;
+    const int row = m0 + tr, col0 = c16 * 4;
+    if (row >= p.M || col0 >= ncols_tile) continue;
+    const float4 v = *reinterpret_cast<const float4*>(stage + (size_t)tr * (BN * 4) + ((c16 ^ (tr & swz)) << 4));
+    float* dst = base + ((size_t)tap_mm * p.dw_K + row) * p.dw_C + n0 + col0;
+    const bool vec = col0 + 4 <= ncols_tile && ((reinterpret_cast<uintptr_t>(dst) & 15) == 0);
+    const float a[4] = {v.x, v.y, v.z, v.w};
+    if (p.ws) {
+      if (vec)
+        *reinterpret_cast<float4*>(dst) = v;
+      else
         for (int i = 0; i < 4; ++i)
-          if (col0 + i < ncols_tile) atomicAdd(dst + i, a[i]);
-      }
+          if (col0 + i < ncols_tile) dst[i] = a[i];
+    } else if (vec) {
+      asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w)
+                   : "memory");
+    } else {
+      for (int i = 0; i < 4; ++i)
+        if (col0 + i < ncols_tile) atomicAdd(dst + i, a[i]);
     }
-    return;
-  }
-
-  // -------- phase 2: BN statistics of the tile AS STORED (bf16-rounded for bf16 outputs — exactly what bn_apply
-  //          normalises): NG row groups of 128/NG rows per column, summed in a fixed order --------
-  if (p.stats) {
-    constexpr int NG = NCONS / BN, RPG = BM / NG;
-    const int c = ctid % BN, g = ctid / BN;
-    const int rend = min((g + 1) * RPG, p.M - m0);
-    float s1 = 0.f, s2 = 0.f;
-    const int byte = c * esize;
-    for (int r = g * RPG; r < rend; ++r) {
-      const uint8_t* src = stage + (size_t)r * (BN * esize) + ((((byte >> 4) ^ (r & swz))) << 4) + (byte & 15);
-      const float x = out_f32 ? *reinterpret_cast<const float*>(src) : bf2f(*reinterpret_cast<const __nv_bfloat16*>(src));
-      s1 += x;
-      s2 = fmaf(x, x, s2);
-    }
-    stat_sm[(g * 2 + 0) * BN + c] = s1;
-    stat_sm[(g * 2 + 1) * BN + c] = s2;
-  }
-
-  // -------- phase 3: the consumers stream the tile out with coalesced 16-byte stores --------
-  {
-    const int nchunks = (ncols_tile * esize + 15) >> 4;  // 16-byte chunks that hold valid data
-    const bool vec_ok = ((p.ldo * esize) & 15) == 0 && ((reinterpret_cast<uintptr_t>(p.out) + (size_t)n0 * esize) & 15) == 0;
-    for (int idx = ctid; idx < BM * CPR; idx += NCONS) {
-      const int tr = idx / CPR;
-      const int c16 = idx - tr * CPR;
-      if (c16 >= nchunks) continue;
-      const int grow = m0 + tr;
-      if (grow >= p.M) continue;
-      long long pixel = grow;
-      if (p.out_strided) {
-        const int n = grow / p.PQ;
-        const int rem = grow - n * p.PQ;
-        const int i = rem / p.Q, j = rem - i * p.Q;
-        pixel = ((long long)n * p.out_H + (i * p.osy + p.opy)) * p.out_W + (j * p.osx + p.opx);
-      }
-      const uint8_t* src = stage + (size_t)tr * (BN * esize) + ((c16 ^ (tr & swz)) << 4);
-      uint8_t* dst = reinterpret_cast<uint8_t*>(p.out) + ((size_t)pixel * p.ldo + n0) * esize + ((size_t)c16 << 4);
-      const int first_col = (c16 << 4) / esize;
-      const bool full = first_col + 16 / esize <= ncols_tile;
-      if (!out_f32) {
-        bf16x8 val = *reinterpret_cast<const bf16x8*>(src);
-        if (vec_ok && full) {
-          if (p.beta != 0.f) {
-            float a[8], b[8];
-            unpack8(val, a);
-            unpack8(*reinterpret_cast<const bf16x8*>(dst), b);
-#pragma unroll
-            for (int k = 0; k < 8; ++k) a[k] += p.beta * b[k];
-            val = pack8(a);
-          }
-          *reinterpret_cast<bf16x8*>(dst) = val;
-        } else {
-          float a[8];
-          unpack8(val, a);
-          __nv_bfloat16* d = reinterpret_cast<__nv_bfloat16*>(dst);
-          for (int k = 0; k < 8; ++k)
-            if (first_col + k < ncols_tile) {
-              float o = a[k];
-              if (p.beta != 0.f) o += p.beta * bf2f(d[k]);
-              d[k] = f2bf(o);
-            }
-        }
-      } else {
-        const float4 val = *reinterpret_cast<const float4*>(src);
-        const float a[4] = {val.x, val.y, val.z, val.w};
-        float* d = reinterpret_cast<float*>(dst);
-        if (vec_ok && full && p.beta == 0.f) {
-          *reinterpret_cast<float4*>(d) = val;
-        } else {
-          for (int k = 0; k < 4; ++k)
-            if (first_col + k < ncols_tile) d[k] = (p.beta != 0.f) ? a[k] + p.beta * d[k] : a[k];
-        }
-      }
-    }
-  }
-  if (num_iters > 0 && ctid == 0) pdl_trigger();
-
-  // -------- phase 4: this CTA's column sums are added to the layer's totals with fp64 atomics.  Each contribution is an
-  //          fp32 value, so the fp64 sum of the <= few thousand partials of a channel is EXACT (no rounding at all) whenever
-  //          their exponents span less than 2^17 — then the order of the atomics cannot matter and the statistics are
-  //          bit-reproducible (fp32 atomics were not, and the batch-2 image-pooling BatchNorm amplified that into 3-5 %
-  //          logit differences between runs).  (Beyond that span the order can move the fp64 sum by one fp64 ulp —
-  //          invisible after the rounding to fp32.) --------
-  if (p.stats) {
-    constexpr int NG = NCONS / BN;
-    consumer_sync();
-    for (int c = ctid; c < ncols_tile; c += NCONS) {
-      float a = 0.f, b = 0.f;
-#pragma unroll
-      for (int g = 0; g < NG; ++g) {
-        a += stat_sm[(g * 2 + 0) * BN + c];
-        b += stat_sm[(g * 2 + 1) * BN + c];
-      }
-      atomicAdd(p.stats + n0 + c, (double)a);
-      atomicAdd(p.stats + p.Ncols + n0 + c, (double)b);
-    }
-    if (p.sync.world > 0)
-      sync_push_when_last<false>(p.sync, p.stats, 2 * p.Ncols, p.stat_ticket, gridDim.x * gridDim.y, ctid, NCONS,
-                          [] { asm volatile("bar.sync 1, 256;" ::: "memory"); }, flag_sm);
   }
 }
 
@@ -485,37 +627,71 @@ static int make_map_im2col(CUtensorMap* m, const void* ptr, int N, int H, int W,
   return 0;
 }
 
+// fprop / dgrad: the persistent grid, one CTA per SM (one per tile when there are fewer tiles).  Fills p.n_tiles / p.tiles.
 template <int BN, int KIND>
-static int launch_kernel(const TcParams& p, dim3 grid, cudaStream_t stream) {
+static int launch_pp(TcParams& p, cudaStream_t stream) {
   static bool attr_set = false;
-  auto kfn = conv_gemm_tc<BN, KIND>;
+  auto kfn = conv_gemm_pp<BN, KIND>;
+  if (!attr_set) {
+    cudaError_t e = cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, PPCfg<BN>::SMEM);
+    SEG_REQUIRE(e == cudaSuccess, "cudaFuncSetAttribute(smem=%d): %s", PPCfg<BN>::SMEM, cudaGetErrorString(e));
+    attr_set = true;
+  }
+  const int n_tiles = ceil_div(p.Ncols, BN);
+  const int64_t tiles = ceil_div64(p.M, BM) * n_tiles;
+  SEG_REQUIRE(tiles < (1ll << 31), "too many output tiles");
+  p.n_tiles = n_tiles;
+  p.tiles = (int)tiles;
+  const dim3 grid((unsigned)std::min<int64_t>(tiles, num_sms()));
+  launch_pdl(kfn, grid, dim3(NTHREADS), (size_t)PPCfg<BN>::SMEM, stream, p);
+  return check_launch("conv_gemm_pp");
+}
+
+template <int KIND>
+static int launch_pp_bn(int bn, TcParams& p, cudaStream_t stream) {
+  switch (bn) {
+    case 64: return launch_pp<64, KIND>(p, stream);
+    case 128: return launch_pp<128, KIND>(p, stream);
+  }
+  set_error("bad BN %d", bn);
+  return 1;
+}
+
+template <int BN>
+static int launch_wgrad(const TcParams& p, dim3 grid, cudaStream_t stream) {
+  static bool attr_set = false;
+  auto kfn = conv_gemm_wgrad<BN>;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BN>::SMEM);
     SEG_REQUIRE(e == cudaSuccess, "cudaFuncSetAttribute(smem=%d): %s", Cfg<BN>::SMEM, cudaGetErrorString(e));
     attr_set = true;
   }
   launch_pdl(kfn, grid, dim3(NTHREADS), (size_t)Cfg<BN>::SMEM, stream, p);
-  return check_launch("conv_gemm_tc");
+  return check_launch("conv_gemm_wgrad");
 }
 
-template <int KIND>
-static int launch_bn(int bn, const TcParams& p, dim3 grid, cudaStream_t stream) {
+static int launch_wgrad_bn(int bn, const TcParams& p, dim3 grid, cudaStream_t stream) {
   switch (bn) {
-    case 64: return launch_kernel<64, KIND>(p, grid, stream);
-    case 128: return launch_kernel<128, KIND>(p, grid, stream);
-    case 256: return launch_kernel<256, KIND>(p, grid, stream);
+    case 64: return launch_wgrad<64>(p, grid, stream);
+    case 128: return launch_wgrad<128>(p, grid, stream);
+    case 256: return launch_wgrad<256>(p, grid, stream);
   }
   set_error("bad BN %d", bn);
   return 1;
 }
 
-// Tile width for an output of `ncols` columns: 128 x 256 tiles move 0.75x the operand bytes per MAC of 128 x 128 ones, so
-// they are taken where the layer has >= 256 output columns and the last column block is not mostly padding.
-static int pick_bn(int ncols) {
-  if (ncols <= 64) return 64;
-  if (ncols < 256) return 128;
-  const int waste = ceil_div(ncols, 256) * 256 - ncols;
-  return waste < 128 ? 256 : 128;
+// Tile width of fprop / dgrad: a consumer warpgroup holds a whole 128 x BN tile in registers (BN / 2 fp32 accumulators per
+// thread and m64 row block), so BN <= 128; fp32 outputs take 64 (the staging tile is 128 rows x 256 B).
+static int pick_bn(int ncols, bool out_f32) { return (ncols <= 64 || out_f32) ? 64 : 128; }
+
+// Rows per group of the statistics fold of a layer with `ncols` output channels: 32 up to 64 channels, 128 from 256 channels
+// on where the last 256-column block is not mostly padding, 64 otherwise.  A function of the layer only, never of the tile
+// width, so the statistics do not depend on the picker.  These are the groups of the earlier one-tile-per-CTA kernel (its
+// 128-row tile summed in 256 / BN groups, BN in {64, 128, 256} chosen by this rule), so its statistics are reproduced bit for bit.
+static int stat_rows_for(int ncols) {
+  if (ncols <= 64) return 32;
+  if (ncols < 256) return 64;
+  return ceil_div(ncols, 256) * 256 - ncols < 128 ? 128 : 64;
 }
 
 bool supported(const seg_conv_desc* d) {
@@ -563,8 +739,8 @@ int conv_fwd(const seg_conv_desc* d, const void* x, const void* w, void* y, int 
     SEG_REQUIRE(4 * d->K <= sync->n_max, "conv fwd: 2*K = %d fp64 statistics exceed the SyncBN buffer (%d floats)", 2 * d->K, sync->n_max);
     p.sync = *sync;
   }
-  const int64_t m_tiles = ceil_div64(M, BM);
-  const int bn = pick_bn(d->K);
+  const int bn = pick_bn(d->K, y_dtype != SEG_DT_BF16);
+  p.stat_rows = stat_rows_for(d->K);
   if (is_pointwise(d)) {
     p.x_im2col = 0;
     if (make_map_2d(&p.mapA, x, M, d->C, d->ldx, BM)) return 1;
@@ -574,8 +750,7 @@ int conv_fwd(const seg_conv_desc* d, const void* x, const void* w, void* y, int 
     if (make_map_im2col(&p.mapA, x, d->N, d->H, d->W, d->C, d->ldx, -d->pad, -d->pad, upper, upper, d->stride, BM)) return 1;
   }
   if (make_map_2d(&p.mapB, w, (int64_t)p.taps * d->K, d->C, d->C, bn)) return 1;
-  dim3 grid((unsigned)m_tiles, (unsigned)ceil_div(d->K, bn), 1);
-  return launch_bn<KIND_KK>(bn, p, grid, stream);
+  return launch_pp_bn<KIND_KK>(bn, p, stream);
 }
 
 static int floordiv(int a, int b) { return (a >= 0) ? a / b : -((-a + b - 1) / b); }
@@ -584,7 +759,7 @@ int conv_dgrad(const seg_conv_desc* d, const void* dy, const void* w, void* dx, 
   SEG_REQUIRE(supported(d) && d->ldy % 8 == 0, "wgmma conv dgrad: unsupported shape (stride=%d K=%d ldy=%d)", d->stride,
               d->K, d->ldy);
   const int s = d->stride;
-  const int bn = pick_bn(d->C);
+  const int bn = pick_bn(d->C, false);
   // One launch per parity class (py, px) of the input pixels; stride 1 has the single class (0, 0).
   for (int py = 0; py < s; ++py) {
     for (int px = 0; px < s; ++px) {
@@ -636,7 +811,7 @@ int conv_dgrad(const seg_conv_desc* d, const void* dy, const void* w, void* dx, 
         p.opy = py;
         p.opx = px;
       }
-      const int64_t m_tiles = ceil_div64(M, BM);
+      p.stat_rows = BM;  // no statistics
       if (p.taps > 0) {
         const bool plain = (s == 1 && is_pointwise(d));
         if (plain) {
@@ -655,8 +830,7 @@ int conv_dgrad(const seg_conv_desc* d, const void* dy, const void* w, void* dx, 
         if (make_map_2d(&p.mapA, w, (int64_t)d->R * d->S * d->K, d->C, d->C, BM)) return 1;
         if (make_map_2d(&p.mapB, w, (int64_t)d->R * d->S * d->K, d->C, d->C, 64)) return 1;
       }
-      dim3 grid((unsigned)m_tiles, (unsigned)ceil_div(d->C, bn), 1);
-      if (launch_bn<KIND_KM>(bn, p, grid, stream)) return 1;
+      if (launch_pp_bn<KIND_KM>(bn, p, stream)) return 1;
     }
   }
   return 0;
@@ -733,7 +907,7 @@ int conv_wgrad(const seg_conv_desc* d, const void* dy, const void* x, float* dw,
   }
   SEG_REQUIRE((unsigned)(p.taps * splits) <= 65535u, "wgrad grid.z too large");
   dim3 grid((unsigned)ceil_div(d->K, BM), (unsigned)ceil_div(d->C, bn), (unsigned)(p.taps * splits));
-  if (launch_bn<KIND_MM>(bn, p, grid, stream)) return 1;
+  if (launch_wgrad_bn(bn, p, grid, stream)) return 1;
   if (splits == 1) return 0;
   const int64_t n = (int64_t)p.taps * d->K * d->C;
   wgrad_split_reduce_kernel<<<(unsigned)std::min<int64_t>(ceil_div64(n, 256), (int64_t)num_sms() * 8), 256, 0, stream>>>(ws, splits, n, dw);

@@ -155,7 +155,7 @@ __global__ void __launch_bounds__(256) im2col_kernel(seg_conv_desc d, const void
 // Column-reduction skeleton shared by bn_stats and bn_bwd_reduce: a 256-thread block owns GB = min(G,256) channel
 // groups (8 channels each) and 256/GB row lanes; rows are grid-strided.  The block's sums (fixed order inside the block)
 // are added to acc[NACC][C] (fp64, ZERO at launch) with one fp64 atomic per channel: exact accumulation of fp32 partials,
-// hence order-independent and bit-reproducible (see conv_gemm_tc's statistics epilogue for the argument).
+// hence order-independent and bit-reproducible (see conv_gemm_pp's statistics epilogue for the argument).
 constexpr int RED_SLOTS = 8;  // accumulator copies the blocks spread their atomics over (contention: blocks / 8 per address)
 template <int NACC, int SLOTS = 1, class F>
 __device__ __forceinline__ void column_reduce(int64_t M, int C, double* acc_out /*[SLOTS][NACC][C]*/, F f) {

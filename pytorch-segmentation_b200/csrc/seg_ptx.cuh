@@ -79,6 +79,21 @@ __device__ __forceinline__ void tma_load_im2col_4d(uint32_t dst, const CUtensorM
       : "memory");
 }
 
+// ---------------- warp specialisation ----------------
+// Per-warpgroup register budget: every thread of the warpgroup executes it.  `dec` hands registers back to the SM's pool,
+// `inc` waits until the pool can grant them.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+// Named barriers: `sync` waits until `count` threads have arrived at barrier `id`; `arrive` counts without waiting.
+__device__ __forceinline__ void named_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+__device__ __forceinline__ void named_arrive(int id, int count) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+
 // ---------------- wgmma ----------------
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
