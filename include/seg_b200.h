@@ -31,7 +31,8 @@ extern "C" {
 #define SEG_DT_F32 1
 
 /* implementation selector for the conv entry points */
-#define SEG_IMPL_AUTO 0 /* wgmma where the shape allows, else SIMT */
+#define SEG_IMPL_AUTO 0 /* wgmma where the shape and the operand base addresses allow (the TMA-read operands —
+                         * fprop x, dgrad dy, wgrad dy and x, packed weights — 16-byte aligned), else SIMT */
 #define SEG_IMPL_SIMT 1 /* CUDA-core implicit GEMM (any shape) */
 #define SEG_IMPL_TC 2   /* wgmma + TMA implicit GEMM, error if shape unsupported */
 
@@ -74,16 +75,21 @@ void seg_launch_count_reset(void);
  * cannot change the result — the statistics are bit-reproducible (fp32 atomics would not be).
  * sync (optional, with stats): SyncBN — the last CTA to finish also pushes the totals (as fp32) to every peer's symmetric
  * buffer and raises the flags (csrc/seg_sync.cuh); sync_ticket = one zeroed uint32.  The consumer is
- * seg_bn_apply_train(..., sync, ...). */
+ * seg_bn_apply_train(..., sync, ...).  stats requires beta == 0 (an error otherwise, on both implementations).
+ * beta != 0 with a bf16 y: the wgmma epilogue rounds the convolution (+bias) to bf16 before it adds beta*y, so the result
+ * is rounded twice; the SIMT kernel adds in fp32 and rounds once. */
 int seg_conv2d_fwd(const seg_conv_desc* d, const void* x, const void* w_packed, void* y, int y_dtype,
                    const float* bias, float beta, double* stats, const seg_sync_desc* sync, void* sync_ticket,
                    int impl, void* stream);
-/* dx[N,H,W,C] = beta*dx + conv_transpose(dy, w)   (autograd of the above w.r.t. x) */
+/* dx[N,H,W,C] = beta*dx + conv_transpose(dy, w)   (autograd of the above w.r.t. x).  Input pixels that no filter tap
+ * reaches (a parity class of a strided convolution with no matching tap) become beta*dx.  beta != 0 with the wgmma path:
+ * the convolution is rounded to bf16 before beta*dx is added, as in seg_conv2d_fwd. */
 int seg_conv2d_dgrad(const seg_conv_desc* d, const void* dy, const void* w_packed, void* dx, float beta,
                      int impl, void* stream);
 /* dw_packed (fp32 [R*S][K][C]) += dy^T * im2col(x)   (autograd w.r.t. the weight; caller zeroes dw first).
  * workspace: fp32 scratch of seg_conv2d_wgrad_workspace_floats(d, impl) floats (NULL when that is 0) holding the k-split
- * partial sums, which are added in a fixed order: the result is bit-reproducible. */
+ * partial sums, which are added in a fixed order: the result is bit-reproducible.  The SIMT kernel (no workspace) adds
+ * its k-splits with fp32 atomics, so its result may differ in the last bits from run to run. */
 int64_t seg_conv2d_wgrad_workspace_floats(const seg_conv_desc* d, int impl);
 int seg_conv2d_wgrad(const seg_conv_desc* d, const void* dy, const void* x, float* dw_packed, float* workspace, int impl,
                      void* stream);

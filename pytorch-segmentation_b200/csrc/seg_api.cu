@@ -42,6 +42,10 @@ static int check_desc(const seg_conv_desc* d) {
   return 0;
 }
 
+// The wgmma path reads its operands through TMA tensor maps, whose base addresses must be 16-byte aligned.  A channel
+// slice at an offset that is not a multiple of 8 bf16 elements is not; AUTO sends such a call to the CUDA-core kernel.
+static bool tma_base_ok(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
 }  // namespace seg
 
 using namespace seg;
@@ -75,7 +79,8 @@ int seg_conv2d_fwd(const seg_conv_desc* d, const void* x, const void* w_packed, 
                    float beta, double* stats, const seg_sync_desc* sync, void* sync_ticket, int impl, void* stream) {
   if (check_desc(d)) return 1;
   SEG_REQUIRE(!sync || (stats && sync_ticket), "seg_conv2d_fwd: SyncBN needs stats and a zeroed ticket word");
-  const bool tc_ok = tc::supported(d);
+  SEG_REQUIRE(!stats || beta == 0.f, "seg_conv2d_fwd: BatchNorm statistics need beta = 0 (got beta = %g)", (double)beta);
+  const bool tc_ok = tc::supported(d) && tma_base_ok(x) && tma_base_ok(w_packed);
   unsigned* tk = reinterpret_cast<unsigned*>(sync_ticket);
   if (impl == SEG_IMPL_TC || (impl == SEG_IMPL_AUTO && tc_ok)) {
     SyncDesc sd{nullptr, 0, 0, 0, 0, 0};
@@ -90,7 +95,7 @@ int seg_conv2d_fwd(const seg_conv_desc* d, const void* x, const void* w_packed, 
 int seg_conv2d_dgrad(const seg_conv_desc* d, const void* dy, const void* w_packed, void* dx, float beta, int impl,
                      void* stream) {
   if (check_desc(d)) return 1;
-  const bool tc_ok = tc::supported(d) && d->ldy % 8 == 0;
+  const bool tc_ok = tc::supported(d) && d->ldy % 8 == 0 && tma_base_ok(dy) && tma_base_ok(w_packed);
   if (impl == SEG_IMPL_TC || (impl == SEG_IMPL_AUTO && tc_ok))
     return tc::conv_dgrad(d, dy, w_packed, dx, beta, ST(stream));
   return simt::conv_dgrad(d, dy, w_packed, dx, beta, ST(stream));
@@ -108,7 +113,9 @@ int64_t seg_conv2d_wgrad_workspace_floats(const seg_conv_desc* d, int impl) {
 int seg_conv2d_wgrad(const seg_conv_desc* d, const void* dy, const void* x, float* dw_packed, float* workspace, int impl,
                      void* stream) {
   if (check_desc(d)) return 1;
-  if (wgrad_on_tc(d, impl))
+  // the workspace query sees no pointers: a call it sized for the wgmma path may still run on the CUDA cores, which
+  // leave the workspace unused
+  if (wgrad_on_tc(d, impl) && (impl == SEG_IMPL_TC || (tma_base_ok(dy) && tma_base_ok(x))))
     return tc::conv_wgrad(d, dy, x, dw_packed, workspace, ST(stream));
   return simt::conv_wgrad(d, dy, x, dw_packed, ST(stream));
 }

@@ -825,8 +825,9 @@ int conv_dgrad(const seg_conv_desc* d, const void* dy, const void* w, void* dx, 
         }
         if (make_map_2d(&p.mapB, w, (int64_t)d->R * d->S * d->K, d->C, d->C, 64)) return 1;
       } else {
-        if (beta != 0.f) continue;  // nothing to add to this class
-        // no tap reaches this class: the kernel writes zeros (num_iters == 0); maps unused but must be valid objects
+        if (beta == 1.f) continue;  // dx = 1 * dx + 0: the class keeps its values
+        // no tap reaches this class: the kernel (num_iters == 0) writes 0 + beta * dx, i.e. zeros for beta = 0 and the
+        // scaled old values otherwise; maps unused but must be valid objects
         if (make_map_2d(&p.mapA, w, (int64_t)d->R * d->S * d->K, d->C, d->C, BM)) return 1;
         if (make_map_2d(&p.mapB, w, (int64_t)d->R * d->S * d->K, d->C, d->C, 64)) return 1;
       }
