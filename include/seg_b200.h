@@ -271,6 +271,33 @@ int seg_upsample_ce_bwd(const float* logits_lo, const int64_t* target, int N, in
 /* loss = accum[0]/accum[1] (fp32 scalar) */
 int seg_ce_finalize(const double* accum, float* loss, void* stream);
 
+/* Class-weighted cross-entropy and focal loss (utils/losses.py:24-31 CrossEntropyLoss2d(weight, reduction),
+ * :52-65 FocalLoss(gamma, alpha, size_average), :67-77 CE_DiceLoss(weight, reduction)).  With nll = lse(z) - z_t at a
+ * pixel labelled t != ignore_index and w = weight (fp32 [C], finite and >= 0; NULL = all ones):
+ *   focal = 0:  per-pixel loss w_t*nll;                          accum[1] += w_t over valid pixels
+ *   focal = 1:  per-pixel loss (1-pt)^gamma * L, L = w_t*nll, pt = exp(-L);  accum[1] += 1 over EVERY pixel
+ * (the reference's .mean() over the unreduced loss counts ignored pixels).  accum[0] += the per-pixel losses; accum is
+ * fp64 [2], zeroed by the caller.  mean = 1: loss = accum[0]/accum[1], or 0 when accum[1] == 0 (ATen gives NaN there);
+ * mean = 0 ('sum', size_average=False): loss = accum[0].  gamma >= 0, finite.
+ * Backward: dL/dz_c = g * w_t (p_c - delta_ct) * F'(L), F' = u^gamma (1 + gamma r), u = -expm1(-L), r = L/expm1(L)
+ * (1 at L = 0), so 0 <= F' <= 1 + gamma and a pixel whose pt rounds to 1 gets the finite limit (0 for gamma > 0; the
+ * reference's autograd gives NaN for 0 < gamma < 1); g = gscale/accum[1] (0 when accum[1] == 0) or gscale for a sum. */
+int seg_loss_nchw_fwd(const float* logits, const int64_t* target, int N, int C, int H, int W, int64_t ignore_index,
+                      const float* weight, int focal, float gamma, double* accum, void* stream);
+int seg_loss_nchw_bwd(const float* logits, const int64_t* target, int N, int C, int H, int W, int64_t ignore_index,
+                      const float* weight, int focal, float gamma, int mean, const double* accum, const float* gscale,
+                      float* dlogits, void* stream);
+int seg_loss_finalize(const double* accum, int mean, float* loss, void* stream);
+/* The same losses fused with the bilinear upsample, as seg_upsample_ce_fwd / seg_upsample_ce_bwd (same buffers, same
+ * 64-bit fixed-point accumulation, C <= 160); the fixed-point scale is derived from |g| * max(w) * (1 + gamma). */
+int seg_upsample_loss_fwd(const float* logits_lo, const int64_t* target, int N, int Hi, int Wi, int Ho, int Wo, int C,
+                          int align_corners, int64_t ignore_index, const float* weight, int focal, float gamma, double* accum,
+                          int32_t* argmax, void* stream);
+int seg_upsample_loss_bwd(const float* logits_lo, const int64_t* target, int N, int Hi, int Wi, int Ho, int Wo, int C,
+                          int align_corners, int64_t ignore_index, const float* weight, int focal, float gamma, int mean,
+                          const double* accum, const float* gscale, float* dlo_f32, void* dlo_fixed, void* dx, int lddx,
+                          void* stream);
+
 /* ---- misc ---- */
 /* standalone ReLU on NHWC bf16 (F.relu, deeplabv3_plus.py:210) and its backward dx = beta*dx + dy*(y>0) */
 int seg_relu_fwd(const void* x, int ldx, void* y, int ldy, int64_t M, int C, void* stream);

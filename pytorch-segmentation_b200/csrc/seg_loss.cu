@@ -31,12 +31,56 @@ __device__ __forceinline__ void block_accum2(double a, double b, double* out) {
   }
 }
 
+// Per-pixel loss variants (utils/losses.py:24-31,52-65,67-77).  With nll = lse(z) - z_t at a pixel labelled t:
+//   LOSS_CE     nll                       denominator: valid pixels      (today's unweighted mean CE, unchanged)
+//   LOSS_WCE    L = w_t * nll             denominator: sum of valid w_t  (nn.CrossEntropyLoss(weight); w = 1 without one)
+//   LOSS_FOCAL  (1 - pt)^gamma * L, pt = exp(-L)   denominator: every pixel, ignored ones included (FocalLoss's .mean())
+// accum[1] holds the denominator; the 'sum' reductions ignore it.  dL/dz_c = w_t (p_c - delta_ct) F'(L) with the focal
+// factor F'(L) = u^gamma (1 + gamma r), u = -expm1(-L), r = L / expm1(L) (r = 1 at L = 0): u and r lie in [0, 1], so
+// 0 <= F' <= 1 + gamma, and no 0 * inf is formed where pt rounds to 1 (F' -> 0 there for gamma > 0).
+enum LossKind { LOSS_CE = 0, LOSS_WCE = 1, LOSS_FOCAL = 2 };
+struct LossArgs {
+  const float* weight;  // fp32 [C] (finite, >= 0) or NULL = all ones; unused by LOSS_CE
+  float gamma;          // LOSS_FOCAL only
+  int mean;             // 1: divide by accum[1]; 0: 'sum' / size_average=False
+};
+
+__device__ __forceinline__ float class_weight(const LossArgs& a, int64_t t, int C) {
+  return a.weight ? ((t >= 0 && t < C) ? a.weight[t] : 0.f) : 1.f;
+}
+template <int K>
+__device__ __forceinline__ float pixel_loss(float nll, float w, float gamma) {
+  if (K == LOSS_CE) return nll;
+  const float L = w * nll;
+  if (K == LOSS_WCE) return L;
+  return powf(-expm1f(-L), gamma) * L;
+}
+// the factor w_t F'(L) the softmax gradient (p - onehot) of a pixel is multiplied by
+template <int K>
+__device__ __forceinline__ float pixel_grad_factor(float nll, float w, float gamma) {
+  if (K != LOSS_FOCAL) return w;
+  const float L = w * nll;
+  const float r = L > 0.f ? L / expm1f(L) : 1.f;
+  return w * powf(-expm1f(-L), gamma) * (1.f + gamma * r);
+}
+// d loss / d (per-pixel loss sum): gscale / accum[1] for a mean.  A weighted or focal mean with accum[1] == 0 (nothing
+// valid, or only zero-weight classes present) has loss 0 and gradient 0; accum[1] < 1 is legitimate there.
+template <int K>
+__device__ __forceinline__ float loss_grad_g(const float* gscale, const double* accum, int mean) {
+  const float gs = gscale ? *gscale : 1.f;
+  if (K == LOSS_CE) return gs / (float)fmax(accum[1], 1.0);
+  if (!mean) return gs;
+  return accum[1] > 0.0 ? (float)((double)gs / accum[1]) : 0.f;
+}
+
+template <int K>
 __global__ void __launch_bounds__(256) ce_nchw_fwd_kernel(const float* __restrict__ logits, const int64_t* __restrict__ target,
-                                                          int N, int C, int H, int W, int64_t ignore, double* accum) {
+                                                          int N, int C, int H, int W, int64_t ignore, LossArgs la, double* accum) {
   const int64_t HW = (int64_t)H * W, total = (int64_t)N * HW;
   double loss = 0.0, cnt = 0.0;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
     const int64_t t = target[i];
+    if (K == LOSS_FOCAL) cnt += 1.0;
     if (t == ignore) continue;
     const int n = (int)(i / HW);
     const float* l = logits + (int64_t)n * C * HW + (i - (int64_t)n * HW);
@@ -45,18 +89,21 @@ __global__ void __launch_bounds__(256) ce_nchw_fwd_kernel(const float* __restric
     float se = 0.f;
     for (int c = 0; c < C; ++c) se += expf(l[(int64_t)c * HW] - mx);
     const float lt = (t >= 0 && t < C) ? l[t * HW] : 0.f;
-    loss += (double)(mx + logf(se) - lt);
-    cnt += 1.0;
+    const float w = K == LOSS_CE ? 1.f : class_weight(la, t, C);
+    loss += (double)pixel_loss<K>(mx + logf(se) - lt, w, la.gamma);
+    if (K == LOSS_CE) cnt += 1.0;
+    if (K == LOSS_WCE) cnt += (double)w;
   }
   block_accum2(loss, cnt, accum);
 }
 
+template <int K>
 __global__ void __launch_bounds__(256) ce_nchw_bwd_kernel(const float* __restrict__ logits, const int64_t* __restrict__ target,
-                                                          int N, int C, int H, int W, int64_t ignore,
+                                                          int N, int C, int H, int W, int64_t ignore, LossArgs la,
                                                           const double* __restrict__ accum, const float* __restrict__ gscale,
                                                           float* __restrict__ dl) {
   const int64_t HW = (int64_t)H * W, total = (int64_t)N * HW;
-  const float g = (gscale ? *gscale : 1.f) / (float)fmax(accum[1], 1.0);
+  const float g = loss_grad_g<K>(gscale, accum, la.mean);
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
     const int64_t t = target[i];
     const int n = (int)(i / HW);
@@ -72,9 +119,14 @@ __global__ void __launch_bounds__(256) ce_nchw_bwd_kernel(const float* __restric
     float se = 0.f;
     for (int c = 0; c < C; ++c) se += expf(l[(int64_t)c * HW] - mx);
     const float inv = 1.f / se;
+    float gp = g;
+    if (K != LOSS_CE) {
+      const float lt = (t >= 0 && t < C) ? l[t * HW] : 0.f;
+      gp = g * pixel_grad_factor<K>(mx + logf(se) - lt, class_weight(la, t, C), la.gamma);
+    }
     for (int c = 0; c < C; ++c) {
       const float p = expf(l[(int64_t)c * HW] - mx) * inv;
-      d[(int64_t)c * HW] = (p - (c == t ? 1.f : 0.f)) * g;
+      d[(int64_t)c * HW] = (p - (c == t ? 1.f : 0.f)) * gp;
     }
   }
 }
@@ -143,6 +195,10 @@ __global__ void dice_finalize_kernel(const double* accum, float smooth, float* l
 __global__ void ce_finalize_kernel(const double* accum, float* loss) {
   if (threadIdx.x == 0 && blockIdx.x == 0) *loss = (float)(accum[0] / fmax(accum[1], 1.0));
 }
+// weighted / focal: a mean with a zero denominator is 0 (see loss_grad_g); a sum is accum[0]
+__global__ void loss_finalize_kernel(const double* accum, int mean, float* loss) {
+  if (threadIdx.x == 0 && blockIdx.x == 0) *loss = (float)(!mean ? accum[0] : accum[1] > 0.0 ? accum[0] / accum[1] : 0.0);
+}
 
 // ---------------------------------------------------------------- fused upsample + CE
 struct Lerp2 {
@@ -174,27 +230,38 @@ constexpr int TILE = 32;   // output tile edge (the backward halves it when the 
 
 // The backward accumulates the logits gradient in 64-bit fixed point: integer additions are associative, so the result
 // does not depend on the order in which threads and blocks add their contributions (fp32 atomics did).  Every contribution
-// is at most |g| in magnitude and the interpolation weights reaching one low-res element sum to less than
+// is at most gmax = |g| * max(w) * (1 + gamma) in magnitude (|p_c - delta_ct| <= 1, w_t <= max(w), 0 <= F' <= 1 + gamma;
+// unweighted CE: gmax = |g|) and the interpolation weights reaching one low-res element sum to less than
 // (2/sh + 2)(2/sw + 2), so with that bound below 2^e the scale 2^(61-e) cannot overflow; a contribution is rounded to
 // |bound| * 2^-62, far below the fp32 rounding of the result.
-__device__ __forceinline__ double ce_grad_scale(float g, float sh, float sw, int Ho, int Wo) {
+__device__ __forceinline__ double ce_grad_scale(double gmax, float sh, float sw, int Ho, int Wo) {
   const double ry = sh > 0.f ? 2.0 / sh : (double)Ho, rx = sw > 0.f ? 2.0 / sw : (double)Wo;
   int e;
-  frexp(fabs((double)g) * (ry + 2.0) * (rx + 2.0), &e);
+  frexp(fabs(gmax) * (ry + 2.0) * (rx + 2.0), &e);
   return ldexp(1.0, 61 - e);
 }
-__device__ __forceinline__ float ce_grad_g(const float* gscale, const double* accum) {
-  return (gscale ? *gscale : 1.f) / (float)fmax(accum[1], 1.0);
+// max over the class weights (1 without weights), on every lane of the calling warp (all 32 lanes must be active)
+__device__ __forceinline__ float warp_weight_max(const float* w, int C) {
+  float m = w ? 0.f : 1.f;
+  if (w)
+    for (int c = threadIdx.x & 31; c < C; c += 32) m = fmaxf(m, w[c]);
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  return m;
+}
+template <int K>
+__device__ __forceinline__ double loss_grad_bound(float g, const LossArgs& la, int C) {
+  if (K == LOSS_CE) return (double)g;
+  return (double)g * (double)warp_weight_max(la.weight, C) * (K == LOSS_FOCAL ? 1.0 + (double)la.gamma : 1.0);
 }
 __device__ __forceinline__ unsigned long long to_fixed(float v, double scale) {
   return (unsigned long long)__double2ll_rn((double)v * scale);
 }
 
 // one block = one 32x32 output tile; the low-res source patch (<= PATCH x PATCH pixels x C) is staged in smem
-template <bool BWD>
+template <bool BWD, int K>
 __global__ void __launch_bounds__(256) upsample_ce_kernel(const float* __restrict__ lo, const int64_t* __restrict__ target,
                                                           int N, int Hi, int Wi, int Ho, int Wo, int C, int ac, float sh,
-                                                          float sw, int64_t ignore, double* accum, int32_t* argmax,
+                                                          float sw, int64_t ignore, LossArgs la, double* accum, int32_t* argmax,
                                                           const float* __restrict__ gscale,
                                                           unsigned long long* __restrict__ dlo_fixed, int patch, int tile) {
   extern __shared__ unsigned long long sm64[];
@@ -223,14 +290,15 @@ __global__ void __launch_bounds__(256) upsample_ce_kernel(const float* __restric
   float g = 0.f;
   double scale = 0.0;
   if (BWD) {
-    g = ce_grad_g(gscale, accum);
-    scale = ce_grad_scale(g, sh, sw, Ho, Wo);
+    g = loss_grad_g<K>(gscale, accum, la.mean);
+    scale = ce_grad_scale(loss_grad_bound<K>(g, la, C), sh, sw, Ho, Wo);
   }
   for (int e = threadIdx.x; e < tile * tile; e += blockDim.x) {
     const int oy = oy0 + e / tile, ox = ox0 + e % tile;
     if (oy >= Ho || ox >= Wo) continue;
     const int64_t tg = target[((int64_t)n * Ho + oy) * Wo + ox];
     const bool valid = tg != ignore;
+    if (K == LOSS_FOCAL && !BWD) cnt += 1.0;
     if (!valid && (BWD || argmax == nullptr)) continue;
     const Lerp2 ly = src_idx(oy, sh, Hi, ac), lx = src_idx(ox, sw, Wi, ac);
     const float h1 = ly.l1, h0 = 1.f - h1, w1 = lx.l1, w0 = 1.f - w1;
@@ -256,18 +324,21 @@ __global__ void __launch_bounds__(256) upsample_ce_kernel(const float* __restric
     if (!BWD) {
       if (argmax) argmax[((int64_t)n * Ho + oy) * Wo + ox] = am;
       if (valid) {
-        loss += (double)(mx + logf(se) - lt);
-        cnt += 1.0;
+        const float w = K == LOSS_CE ? 1.f : class_weight(la, tg, C);
+        loss += (double)pixel_loss<K>(mx + logf(se) - lt, w, la.gamma);
+        if (K == LOSS_CE) cnt += 1.0;
+        if (K == LOSS_WCE) cnt += (double)w;
       }
     } else {
       const float inv = 1.f / se;
+      const float gp = K == LOSS_CE ? g : g * pixel_grad_factor<K>(mx + logf(se) - lt, class_weight(la, tg, C), la.gamma);
       unsigned long long* da = dst + ((ly.i0 - sy0) * pw + (lx.i0 - sx0)) * C;
       unsigned long long* db = dst + ((ly.i0 - sy0) * pw + (lx.i1 - sx0)) * C;
       unsigned long long* dc = dst + ((ly.i1 - sy0) * pw + (lx.i0 - sx0)) * C;
       unsigned long long* dd = dst + ((ly.i1 - sy0) * pw + (lx.i1 - sx0)) * C;
       for (int c = 0; c < C; ++c) {
         const float v = h0 * (w0 * pa[c] + w1 * pb[c]) + h1 * (w0 * pc[c] + w1 * pd[c]);
-        const float gr = (expf(v - mx) * inv - (c == tg ? 1.f : 0.f)) * g;
+        const float gr = (expf(v - mx) * inv - (c == tg ? 1.f : 0.f)) * gp;
         atomicAdd(da + c, to_fixed(h0 * w0 * gr, scale));
         atomicAdd(db + c, to_fixed(h0 * w1 * gr, scale));
         atomicAdd(dc + c, to_fixed(h1 * w0 * gr, scale));
@@ -292,9 +363,11 @@ __global__ void __launch_bounds__(256) upsample_ce_kernel(const float* __restric
 }
 
 // fixed-point accumulators -> fp32 gradient (the scale is recomputed exactly as the accumulating kernel did)
+template <int K>
 __global__ void ce_grad_from_fixed_kernel(const unsigned long long* __restrict__ acc, int64_t n, const float* gscale,
-                                          const double* accum, float sh, float sw, int Ho, int Wo, float* __restrict__ dlo) {
-  const double inv = 1.0 / ce_grad_scale(ce_grad_g(gscale, accum), sh, sw, Ho, Wo);
+                                          const double* accum, LossArgs la, int C, float sh, float sw, int Ho, int Wo,
+                                          float* __restrict__ dlo) {
+  const double inv = 1.0 / ce_grad_scale(loss_grad_bound<K>(loss_grad_g<K>(gscale, accum, la.mean), la, C), sh, sw, Ho, Wo);
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
     dlo[i] = (float)((double)(long long)acc[i] * inv);
 }
@@ -320,21 +393,114 @@ static int patch_for(int in_size, int out_size, int ac, int tile) {
 using namespace seg;
 #define ST(s) reinterpret_cast<cudaStream_t>(s)
 
+namespace seg {
+template <int K>
+static int ce_nchw_fwd(const float* logits, const int64_t* target, int N, int C, int H, int W, int64_t ignore_index,
+                       LossArgs la, double* accum, cudaStream_t stream) {
+  const int64_t total = (int64_t)N * H * W;
+  int blocks = (int)std::min<int64_t>(ceil_div64(total, 256), (int64_t)num_sms() * 8);
+  ce_nchw_fwd_kernel<K><<<blocks, 256, 0, stream>>>(logits, target, N, C, H, W, ignore_index, la, accum);
+  return check_launch("ce_nchw_fwd");
+}
+template <int K>
+static int ce_nchw_bwd(const float* logits, const int64_t* target, int N, int C, int H, int W, int64_t ignore_index,
+                       LossArgs la, const double* accum, const float* gscale, float* dlogits, cudaStream_t stream) {
+  const int64_t total = (int64_t)N * H * W;
+  int blocks = (int)std::min<int64_t>(ceil_div64(total, 256), (int64_t)num_sms() * 8);
+  ce_nchw_bwd_kernel<K><<<blocks, 256, 0, stream>>>(logits, target, N, C, H, W, ignore_index, la, accum, gscale, dlogits);
+  return check_launch("ce_nchw_bwd");
+}
+
+template <int K>
+static int upsample_ce_fwd(const float* logits_lo, const int64_t* target, int N, int Hi, int Wi, int Ho, int Wo, int C,
+                           int align_corners, int64_t ignore_index, LossArgs la, double* accum, int32_t* argmax,
+                           cudaStream_t stream) {
+  SEG_REQUIRE(C <= MAXC, "upsample_ce: C=%d > %d", C, MAXC);
+  const int patch = std::max(patch_for(Hi, Ho, align_corners, TILE), patch_for(Wi, Wo, align_corners, TILE));
+  const size_t smem = (size_t)patch * patch * C * sizeof(float);
+  SEG_REQUIRE(smem <= 200 * 1024, "upsample_ce: patch too large (%zu B)", smem);
+  static size_t set_smem = 0;
+  if (smem > set_smem) {
+    cudaFuncSetAttribute(upsample_ce_kernel<false, K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    set_smem = smem;
+  }
+  const int blocks = N * ceil_div(Ho, TILE) * ceil_div(Wo, TILE);
+  upsample_ce_kernel<false, K><<<blocks, 256, smem, stream>>>(
+      logits_lo, target, N, Hi, Wi, Ho, Wo, C, align_corners, rscale(Hi, Ho, align_corners), rscale(Wi, Wo, align_corners),
+      ignore_index, la, accum, argmax, nullptr, nullptr, patch, TILE);
+  return check_launch("upsample_ce_fwd");
+}
+
+template <int K>
+static int upsample_ce_bwd(const float* logits_lo, const int64_t* target, int N, int Hi, int Wi, int Ho, int Wo, int C,
+                           int align_corners, int64_t ignore_index, LossArgs la, const double* accum, const float* gscale,
+                           float* dlo_f32, void* dlo_fixed, void* dx, int lddx, cudaStream_t stream) {
+  SEG_REQUIRE(C <= MAXC, "upsample_ce: C=%d > %d", C, MAXC);
+  // fixed-point accumulators (8 B) + the fp32 source patch per (patch pixel, class)
+  auto bwd_patch = [&](int t) { return std::max(patch_for(Hi, Ho, align_corners, t), patch_for(Wi, Wo, align_corners, t)); };
+  auto bwd_smem = [&](int t) { return (size_t)bwd_patch(t) * bwd_patch(t) * C * (sizeof(unsigned long long) + sizeof(float)); };
+  const int tile = bwd_smem(TILE) <= 227 * 1024 ? TILE : TILE / 2;
+  const int patch = bwd_patch(tile);
+  const size_t smem = bwd_smem(tile);
+  SEG_REQUIRE(smem <= 227 * 1024, "upsample_ce: patch too large (%zu B)", smem);
+  static size_t set_smem = 0;
+  if (smem > set_smem) {
+    cudaFuncSetAttribute(upsample_ce_kernel<true, K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    set_smem = smem;
+  }
+  const int64_t M = (int64_t)N * Hi * Wi;
+  unsigned long long* fixed = reinterpret_cast<unsigned long long*>(dlo_fixed);
+  cudaMemsetAsync(fixed, 0, (size_t)M * C * sizeof(unsigned long long), stream);
+  const int blocks = N * ceil_div(Ho, tile) * ceil_div(Wo, tile);
+  const float sh = rscale(Hi, Ho, align_corners), sw = rscale(Wi, Wo, align_corners);
+  upsample_ce_kernel<true, K><<<blocks, 256, smem, stream>>>(
+      logits_lo, target, N, Hi, Wi, Ho, Wo, C, align_corners, sh, sw, ignore_index, la, const_cast<double*>(accum), nullptr,
+      gscale, fixed, patch, tile);
+  if (check_launch("upsample_ce_bwd")) return 1;
+  const int64_t n = M * C;
+  ce_grad_from_fixed_kernel<K><<<(unsigned)std::min<int64_t>(ceil_div64(n, 256), (int64_t)num_sms() * 8), 256, 0, stream>>>(
+      fixed, n, gscale, accum, la, C, sh, sw, Ho, Wo, dlo_f32);
+  if (check_launch("ce_grad_from_fixed")) return 1;
+  if (dx) {
+    int blocks2 = (int)std::min<int64_t>(ceil_div64(M * lddx, 256), (int64_t)num_sms() * 8);
+    cast_pad_kernel<<<blocks2, 256, 0, stream>>>(dlo_f32, reinterpret_cast<__nv_bfloat16*>(dx), M, C, lddx);
+    return check_launch("cast_pad");
+  }
+  return 0;
+}
+
+// the weighted / focal entry points: focal selects LOSS_FOCAL (weight optional), otherwise LOSS_WCE (NULL weight = ones)
+static int loss_args(const float* weight, int focal, float gamma, int mean, int C, LossArgs* la) {
+  SEG_REQUIRE(C > 0, "loss: C=%d", C);
+  SEG_REQUIRE(!focal || (gamma >= 0.f && isfinite(gamma)), "loss: focal gamma must be finite and >= 0 (got %g)", (double)gamma);
+  *la = LossArgs{weight, gamma, mean ? 1 : 0};
+  return 0;
+}
+#define SEG_LOSS_DISPATCH(focal, fn, ...) ((focal) ? fn<LOSS_FOCAL>(__VA_ARGS__) : fn<LOSS_WCE>(__VA_ARGS__))
+}  // namespace seg
+
 extern "C" {
 
 int seg_ce_nchw_fwd(const float* logits, const int64_t* target, int N, int C, int H, int W, int64_t ignore_index,
                     double* accum, void* stream) {
-  const int64_t total = (int64_t)N * H * W;
-  int blocks = (int)std::min<int64_t>(ceil_div64(total, 256), (int64_t)num_sms() * 8);
-  ce_nchw_fwd_kernel<<<blocks, 256, 0, ST(stream)>>>(logits, target, N, C, H, W, ignore_index, accum);
-  return check_launch("ce_nchw_fwd");
+  return ce_nchw_fwd<LOSS_CE>(logits, target, N, C, H, W, ignore_index, LossArgs{}, accum, ST(stream));
 }
 int seg_ce_nchw_bwd(const float* logits, const int64_t* target, int N, int C, int H, int W, int64_t ignore_index,
                     const double* accum, const float* gscale, float* dlogits, void* stream) {
-  const int64_t total = (int64_t)N * H * W;
-  int blocks = (int)std::min<int64_t>(ceil_div64(total, 256), (int64_t)num_sms() * 8);
-  ce_nchw_bwd_kernel<<<blocks, 256, 0, ST(stream)>>>(logits, target, N, C, H, W, ignore_index, accum, gscale, dlogits);
-  return check_launch("ce_nchw_bwd");
+  return ce_nchw_bwd<LOSS_CE>(logits, target, N, C, H, W, ignore_index, LossArgs{}, accum, gscale, dlogits, ST(stream));
+}
+int seg_loss_nchw_fwd(const float* logits, const int64_t* target, int N, int C, int H, int W, int64_t ignore_index,
+                      const float* weight, int focal, float gamma, double* accum, void* stream) {
+  LossArgs la;
+  if (loss_args(weight, focal, gamma, 1, C, &la)) return 1;
+  return SEG_LOSS_DISPATCH(focal, ce_nchw_fwd, logits, target, N, C, H, W, ignore_index, la, accum, ST(stream));
+}
+int seg_loss_nchw_bwd(const float* logits, const int64_t* target, int N, int C, int H, int W, int64_t ignore_index,
+                      const float* weight, int focal, float gamma, int mean, const double* accum, const float* gscale,
+                      float* dlogits, void* stream) {
+  LossArgs la;
+  if (loss_args(weight, focal, gamma, mean, C, &la)) return 1;
+  return SEG_LOSS_DISPATCH(focal, ce_nchw_bwd, logits, target, N, C, H, W, ignore_index, la, accum, gscale, dlogits, ST(stream));
 }
 int seg_dice_nchw_fwd(const float* logits, const int64_t* target, int N, int C, int H, int W, float smooth, double* accum,
                       float* loss, void* stream) {
@@ -356,61 +522,40 @@ int seg_ce_finalize(const double* accum, float* loss, void* stream) {
   ce_finalize_kernel<<<1, 32, 0, ST(stream)>>>(accum, loss);
   return check_launch("ce_finalize");
 }
+int seg_loss_finalize(const double* accum, int mean, float* loss, void* stream) {
+  loss_finalize_kernel<<<1, 32, 0, ST(stream)>>>(accum, mean, loss);
+  return check_launch("loss_finalize");
+}
 
 int seg_upsample_ce_fwd(const float* logits_lo, const int64_t* target, int N, int Hi, int Wi, int Ho, int Wo, int C,
                         int align_corners, int64_t ignore_index, double* accum, int32_t* argmax, void* stream) {
-  SEG_REQUIRE(C <= MAXC, "upsample_ce: C=%d > %d", C, MAXC);
-  const int patch = std::max(patch_for(Hi, Ho, align_corners, TILE), patch_for(Wi, Wo, align_corners, TILE));
-  const size_t smem = (size_t)patch * patch * C * sizeof(float);
-  SEG_REQUIRE(smem <= 200 * 1024, "upsample_ce: patch too large (%zu B)", smem);
-  static size_t set_smem = 0;
-  if (smem > set_smem) {
-    cudaFuncSetAttribute(upsample_ce_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    set_smem = smem;
-  }
-  const int blocks = N * ceil_div(Ho, TILE) * ceil_div(Wo, TILE);
-  upsample_ce_kernel<false><<<blocks, 256, smem, ST(stream)>>>(
-      logits_lo, target, N, Hi, Wi, Ho, Wo, C, align_corners, rscale(Hi, Ho, align_corners), rscale(Wi, Wo, align_corners),
-      ignore_index, accum, argmax, nullptr, nullptr, patch, TILE);
-  return check_launch("upsample_ce_fwd");
+  return upsample_ce_fwd<LOSS_CE>(logits_lo, target, N, Hi, Wi, Ho, Wo, C, align_corners, ignore_index, LossArgs{}, accum,
+                                  argmax, ST(stream));
+}
+int seg_upsample_loss_fwd(const float* logits_lo, const int64_t* target, int N, int Hi, int Wi, int Ho, int Wo, int C,
+                          int align_corners, int64_t ignore_index, const float* weight, int focal, float gamma, double* accum,
+                          int32_t* argmax, void* stream) {
+  LossArgs la;
+  if (loss_args(weight, focal, gamma, 1, C, &la)) return 1;
+  return SEG_LOSS_DISPATCH(focal, upsample_ce_fwd, logits_lo, target, N, Hi, Wi, Ho, Wo, C, align_corners, ignore_index, la, accum,
+                           argmax, ST(stream));
 }
 
 // dlo_f32: fp32 [N,Hi,Wi,C]; dlo_fixed: int64 scratch [N,Hi,Wi,C] (zeroed here); dx: bf16 [N*Hi*Wi][lddx] or NULL
 int seg_upsample_ce_bwd(const float* logits_lo, const int64_t* target, int N, int Hi, int Wi, int Ho, int Wo, int C,
                         int align_corners, int64_t ignore_index, const double* accum, const float* gscale,
                         float* dlo_f32, void* dlo_fixed, void* dx, int lddx, void* stream) {
-  SEG_REQUIRE(C <= MAXC, "upsample_ce: C=%d > %d", C, MAXC);
-  // fixed-point accumulators (8 B) + the fp32 source patch per (patch pixel, class)
-  auto bwd_patch = [&](int t) { return std::max(patch_for(Hi, Ho, align_corners, t), patch_for(Wi, Wo, align_corners, t)); };
-  auto bwd_smem = [&](int t) { return (size_t)bwd_patch(t) * bwd_patch(t) * C * (sizeof(unsigned long long) + sizeof(float)); };
-  const int tile = bwd_smem(TILE) <= 227 * 1024 ? TILE : TILE / 2;
-  const int patch = bwd_patch(tile);
-  const size_t smem = bwd_smem(tile);
-  SEG_REQUIRE(smem <= 227 * 1024, "upsample_ce: patch too large (%zu B)", smem);
-  static size_t set_smem = 0;
-  if (smem > set_smem) {
-    cudaFuncSetAttribute(upsample_ce_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    set_smem = smem;
-  }
-  const int64_t M = (int64_t)N * Hi * Wi;
-  unsigned long long* fixed = reinterpret_cast<unsigned long long*>(dlo_fixed);
-  cudaMemsetAsync(fixed, 0, (size_t)M * C * sizeof(unsigned long long), ST(stream));
-  const int blocks = N * ceil_div(Ho, tile) * ceil_div(Wo, tile);
-  const float sh = rscale(Hi, Ho, align_corners), sw = rscale(Wi, Wo, align_corners);
-  upsample_ce_kernel<true><<<blocks, 256, smem, ST(stream)>>>(
-      logits_lo, target, N, Hi, Wi, Ho, Wo, C, align_corners, sh, sw, ignore_index, const_cast<double*>(accum), nullptr, gscale,
-      fixed, patch, tile);
-  if (check_launch("upsample_ce_bwd")) return 1;
-  const int64_t n = M * C;
-  ce_grad_from_fixed_kernel<<<(unsigned)std::min<int64_t>(ceil_div64(n, 256), (int64_t)num_sms() * 8), 256, 0, ST(stream)>>>(
-      fixed, n, gscale, accum, sh, sw, Ho, Wo, dlo_f32);
-  if (check_launch("ce_grad_from_fixed")) return 1;
-  if (dx) {
-    int blocks2 = (int)std::min<int64_t>(ceil_div64(M * lddx, 256), (int64_t)num_sms() * 8);
-    cast_pad_kernel<<<blocks2, 256, 0, ST(stream)>>>(dlo_f32, reinterpret_cast<__nv_bfloat16*>(dx), M, C, lddx);
-    return check_launch("cast_pad");
-  }
-  return 0;
+  return upsample_ce_bwd<LOSS_CE>(logits_lo, target, N, Hi, Wi, Ho, Wo, C, align_corners, ignore_index, LossArgs{}, accum,
+                                  gscale, dlo_f32, dlo_fixed, dx, lddx, ST(stream));
+}
+int seg_upsample_loss_bwd(const float* logits_lo, const int64_t* target, int N, int Hi, int Wi, int Ho, int Wo, int C,
+                          int align_corners, int64_t ignore_index, const float* weight, int focal, float gamma, int mean,
+                          const double* accum, const float* gscale, float* dlo_f32, void* dlo_fixed, void* dx, int lddx,
+                          void* stream) {
+  LossArgs la;
+  if (loss_args(weight, focal, gamma, mean, C, &la)) return 1;
+  return SEG_LOSS_DISPATCH(focal, upsample_ce_bwd, logits_lo, target, N, Hi, Wi, Ho, Wo, C, align_corners, ignore_index, la, accum,
+                           gscale, dlo_f32, dlo_fixed, dx, lddx, ST(stream));
 }
 
 }  // extern "C"

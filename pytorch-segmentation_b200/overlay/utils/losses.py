@@ -1,5 +1,6 @@
 """`utils.losses` overlay: the reference's loss registry (train.py:30 `getattr(losses, config['loss'])`) with
-CrossEntropyLoss2d replaced by the sm_90a kernel version; the other losses are re-exported from the reference file."""
+every loss class it defines (CrossEntropyLoss2d, DiceLoss, FocalLoss, CE_DiceLoss, LovaszSoftmax) replaced by the sm_90a
+kernel version; the file's other names are re-exported from the reference file."""
 import importlib.util
 import os
 
@@ -13,4 +14,4 @@ if REFERENCE_UTILS is not None:
         if not _n.startswith("_"):
             globals()[_n] = getattr(_ref, _n)
 
-from seg_b200.losses import CE_DiceLoss, CrossEntropyLoss2d, DiceLoss, LovaszSoftmax  # noqa: E402,F401
+from seg_b200.losses import CE_DiceLoss, CrossEntropyLoss2d, DiceLoss, FocalLoss, LovaszSoftmax  # noqa: E402,F401

@@ -12,6 +12,7 @@ _LAZY = {
     "UperNet": ("nets", "UperNet"),
     "CrossEntropyLoss2d": ("losses", "CrossEntropyLoss2d"),
     "DiceLoss": ("losses", "DiceLoss"),
+    "FocalLoss": ("losses", "FocalLoss"),
     "CE_DiceLoss": ("losses", "CE_DiceLoss"),
     "LovaszSoftmax": ("losses", "LovaszSoftmax"),
     "eval_metrics": ("metrics", "eval_metrics"),

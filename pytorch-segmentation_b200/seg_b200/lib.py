@@ -94,6 +94,11 @@ _SIGS = {
     "seg_ce_finalize": (c_int, [c_void_p, c_void_p, c_void_p]),
     "seg_upsample_ce_fwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int64, c_void_p, c_void_p, c_void_p]),
     "seg_upsample_ce_bwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
+    "seg_loss_nchw_fwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int64, c_void_p, c_int, c_float, c_void_p, c_void_p]),
+    "seg_loss_nchw_bwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int64, c_void_p, c_int, c_float, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "seg_loss_finalize": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
+    "seg_upsample_loss_fwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int64, c_void_p, c_int, c_float, c_void_p, c_void_p, c_void_p]),
+    "seg_upsample_loss_bwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int64, c_void_p, c_int, c_float, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
     "seg_relu_fwd": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int64, c_int, c_void_p]),
     "seg_relu_bwd": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int64, c_int, c_float, c_void_p]),
     "seg_nhwc_to_nchw_f32": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),

@@ -458,6 +458,31 @@ def ce_nchw_bwd(logits, target, ignore_index, accum, gscale=None):
     return dl
 
 
+def loss_nchw_fwd(logits, target, ignore_index, weight=None, gamma=None, mean=True, reduce_fn=None):
+    """Class-weighted CE (gamma None) or focal loss (gamma >= 0), weight: fp32 [C] device tensor or None (all ones).
+    Returns (loss, accum); accum = fp64 (per-pixel loss sum, denominator), reduce_fn(accum) as in ce_nchw_fwd.  mean=False:
+    the loss is the (globally reduced) sum."""
+    N, C, H, W = logits.shape
+    assert logits.is_contiguous() and logits.dtype == torch.float32 and target.dtype == torch.int64 and target.is_contiguous()
+    assert weight is None or (weight.dtype == torch.float32 and weight.numel() == C and weight.is_contiguous())
+    accum = torch.zeros(2, dtype=torch.float64, device=logits.device)
+    call("seg_loss_nchw_fwd", ptr(logits), ptr(target), N, C, H, W, int(ignore_index), ptr(weight), int(gamma is not None),
+         float(gamma or 0.0), ptr(accum))
+    if reduce_fn is not None:
+        reduce_fn(accum)
+    loss = torch.empty((), dtype=torch.float32, device=logits.device)
+    call("seg_loss_finalize", ptr(accum), int(mean), ptr(loss))
+    return loss, accum
+
+
+def loss_nchw_bwd(logits, target, ignore_index, accum, weight=None, gamma=None, mean=True, gscale=None):
+    N, C, H, W = logits.shape
+    dl = torch.empty_like(logits)
+    call("seg_loss_nchw_bwd", ptr(logits), ptr(target), N, C, H, W, int(ignore_index), ptr(weight), int(gamma is not None),
+         float(gamma or 0.0), int(mean), ptr(accum), ptr(gscale), ptr(dl))
+    return dl
+
+
 def dice_nchw_fwd(logits, target, smooth=1.0):
     N, C, H, W = logits.shape
     assert logits.is_contiguous() and logits.dtype == torch.float32 and target.dtype == torch.int64 and target.is_contiguous()
@@ -528,6 +553,37 @@ def upsample_ce_bwd(logits_lo, target, align_corners, ignore_index, accum, ldx, 
     dx = torch.empty((N, Hi, Wi, ldx), dtype=torch.bfloat16, device=logits_lo.device)
     call("seg_upsample_ce_bwd", ptr(logits_lo), ptr(target), N, Hi, Wi, Ho, Wo, C, int(align_corners), int(ignore_index),
          ptr(accum), ptr(gscale), ptr(dlo), ptr(fixed), ptr(dx), ldx)
+    return dx, dlo
+
+
+def upsample_loss_fwd(logits_lo, target, align_corners, ignore_index, weight=None, gamma=None, mean=True, want_argmax=False,
+                      reduce_fn=None):
+    """upsample_ce_fwd for the class-weighted CE (gamma None) and focal (gamma >= 0) losses of loss_nchw_fwd."""
+    N, Hi, Wi, C = logits_lo.shape
+    _, Ho, Wo = target.shape
+    assert logits_lo.is_contiguous() and logits_lo.dtype == torch.float32 and target.is_contiguous()
+    assert weight is None or (weight.dtype == torch.float32 and weight.numel() == C and weight.is_contiguous())
+    accum = torch.zeros(2, dtype=torch.float64, device=logits_lo.device)
+    am = torch.empty((N, Ho, Wo), dtype=torch.int32, device=logits_lo.device) if want_argmax else None
+    call("seg_upsample_loss_fwd", ptr(logits_lo), ptr(target), N, Hi, Wi, Ho, Wo, C, int(align_corners), int(ignore_index),
+         ptr(weight), int(gamma is not None), float(gamma or 0.0), ptr(accum), ptr(am))
+    if reduce_fn is not None:
+        reduce_fn(accum)
+    loss = torch.empty((), dtype=torch.float32, device=logits_lo.device)
+    call("seg_loss_finalize", ptr(accum), int(mean), ptr(loss))
+    return loss, accum, am
+
+
+def upsample_loss_bwd(logits_lo, target, align_corners, ignore_index, accum, ldx, weight=None, gamma=None, mean=True,
+                      gscale=None):
+    N, Hi, Wi, C = logits_lo.shape
+    _, Ho, Wo = target.shape
+    dlo = torch.empty((N, Hi, Wi, C), dtype=torch.float32, device=logits_lo.device)
+    fixed = torch.empty((N, Hi, Wi, C), dtype=torch.int64, device=logits_lo.device)
+    dx = torch.empty((N, Hi, Wi, ldx), dtype=torch.bfloat16, device=logits_lo.device)
+    call("seg_upsample_loss_bwd", ptr(logits_lo), ptr(target), N, Hi, Wi, Ho, Wo, C, int(align_corners), int(ignore_index),
+         ptr(weight), int(gamma is not None), float(gamma or 0.0), int(mean), ptr(accum), ptr(gscale), ptr(dlo), ptr(fixed),
+         ptr(dx), ldx)
     return dx, dlo
 
 

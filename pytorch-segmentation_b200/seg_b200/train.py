@@ -86,11 +86,28 @@ class WeightTables:
             lib.call("seg_unpack_wgrads_batched", self.unpack_table.data_ptr(), self.unpack_n, self.unpack_total, 0.0)
 
 
+def _loss_spec(loss, ignore_index):
+    """(ignore_index, LossSpec or None) for FusedTrainStep's `loss`: None and unweighted mean CE run the unweighted kernels."""
+    from . import losses
+    if loss is None:
+        return (255 if ignore_index is None else ignore_index), None
+    if type(loss) not in (losses.CrossEntropyLoss2d, losses.FocalLoss):
+        raise NotImplementedError(
+            f"FusedTrainStep fuses seg_b200.CrossEntropyLoss2d and seg_b200.FocalLoss only, not {type(loss).__name__}; "
+            "train with it on the plugin surface instead: loss = crit(model(x), y); loss.backward(); optimizer.step()")
+    if ignore_index is not None and ignore_index != loss.ignore_index:
+        raise ValueError(f"FusedTrainStep: ignore_index={ignore_index} conflicts with the loss's ignore_index={loss.ignore_index}")
+    return loss.ignore_index, loss.spec
+
+
 class FusedTrainStep:
-    def __init__(self, model, ignore_index=255, lr=0.01, backbone_lr_scale=0.1, momentum=0.9, weight_decay=1e-4,
-                 aux_weight=0.4, world=1, cuda_graph=False, bucket_mb=0.0):
+    """loss: None (the reference configs' CrossEntropyLoss2d(ignore_index=255)), or a seg_b200.CrossEntropyLoss2d /
+    seg_b200.FocalLoss instance, applied to the main head and (x aux_weight) to the aux head; its ignore_index governs."""
+
+    def __init__(self, model, ignore_index=None, lr=0.01, backbone_lr_scale=0.1, momentum=0.9, weight_decay=1e-4,
+                 aux_weight=0.4, world=1, cuda_graph=False, bucket_mb=0.0, loss=None):
         self.model = model
-        self.ignore_index = ignore_index
+        self.ignore_index, self.loss_spec = _loss_spec(loss, ignore_index)
         self._momentum, self.wd = float(momentum), float(weight_decay)
         self.aux_weight = aux_weight
         self.world = world
@@ -266,14 +283,24 @@ class FusedTrainStep:
         # mean over the valid pixels of the GLOBAL batch, as nn.DataParallel's gathered logits give the reference
         # (trainer.py:60-66): the (loss sum, valid count) pair is all-reduced — 16 bytes — and the gradient is scaled by
         # world because the exchanged gradients are averaged over ranks below
+        # (a weighted or focal loss all-reduces its (sum, denominator) pair the same way; a 'sum' is the global sum)
         rf = (lambda acc: dist.all_reduce(acc)) if self.world > 1 else None
+        spec = self.loss_spec
         for i, (lo, ac) in enumerate(heads):
             C = lo.t.shape[-1]
-            loss, accum, _ = ops.upsample_ce_fwd(lo.t, target, ac, self.ignore_index, reduce_fn=rf)
+            if spec is None:
+                loss, accum, _ = ops.upsample_ce_fwd(lo.t, target, ac, self.ignore_index, reduce_fn=rf)
+            else:
+                cw = spec.weight_on(lo.t.device, C)
+                loss, accum, _ = ops.upsample_loss_fwd(lo.t, target, ac, self.ignore_index, cw, spec.gamma, spec.mean, reduce_fn=rf)
             w = 1.0 if i == 0 else self.aux_weight
             wg = w * self.world
             g = None if wg == 1.0 else torch.full((1,), wg, dtype=torch.float32, device=lo.t.device)
-            dx, _ = ops.upsample_ce_bwd(lo.t, target, ac, self.ignore_index, accum, (C + 7) // 8 * 8, gscale=g)
+            if spec is None:
+                dx, _ = ops.upsample_ce_bwd(lo.t, target, ac, self.ignore_index, accum, (C + 7) // 8 * 8, gscale=g)
+            else:
+                dx, _ = ops.upsample_loss_bwd(lo.t, target, ac, self.ignore_index, accum, (C + 7) // 8 * 8, cw, spec.gamma,
+                                              spec.mean, gscale=g)
             lo.grad = dx[..., :C]
             total = loss if total is None else total + w * loss
         m._finish(tape)
