@@ -297,6 +297,18 @@ int seg_upsample_loss_bwd(const float* logits_lo, const int64_t* target, int N, 
                           int align_corners, int64_t ignore_index, const float* weight, int focal, float gamma, int mean,
                           const double* accum, const float* gscale, float* dlo_f32, void* dlo_fixed, void* dx, int lddx,
                           void* stream);
+/* seg_upsample_ce_fwd / seg_upsample_loss_fwd that also count the main head's eval_metrics (trainer.py:62,84 ->
+ * utils/metrics.py:59-67) in the same launch, so neither training nor validation needs the full-resolution logits for
+ * pixel accuracy and mIoU.  counters: int64 [2 + 3*C] = correct, labeled, area_inter[C], area_pred[C], area_lab[C], the
+ * layout of seg_eval_metrics_nchw with num_class = C; ADDED to (not zeroed), so a running total needs no extra launch.
+ * The prediction is the arg-max of the interpolated fp32 logits seg_bilinear_logits_fwd produces (lowest index wins
+ * ties); a pixel is labeled when 0 <= target < C, independently of ignore_index.  Integer counters: deterministic. */
+int seg_upsample_ce_fwd_metrics(const float* logits_lo, const int64_t* target, int N, int Hi, int Wi, int Ho, int Wo, int C,
+                                int align_corners, int64_t ignore_index, double* accum, int32_t* argmax, int64_t* counters,
+                                void* stream);
+int seg_upsample_loss_fwd_metrics(const float* logits_lo, const int64_t* target, int N, int Hi, int Wi, int Ho, int Wo, int C,
+                                  int align_corners, int64_t ignore_index, const float* weight, int focal, float gamma,
+                                  double* accum, int32_t* argmax, int64_t* counters, void* stream);
 
 /* ---- misc ---- */
 /* standalone ReLU on NHWC bf16 (F.relu, deeplabv3_plus.py:210) and its backward dx = beta*dx + dy*(y>0) */

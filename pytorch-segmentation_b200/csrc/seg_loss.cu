@@ -257,16 +257,23 @@ __device__ __forceinline__ unsigned long long to_fixed(float v, double scale) {
   return (unsigned long long)__double2ll_rn((double)v * scale);
 }
 
-// one block = one 32x32 output tile; the low-res source patch (<= PATCH x PATCH pixels x C) is staged in smem
-template <bool BWD, int K>
+// one block = one 32x32 output tile; the low-res source patch (<= PATCH x PATCH pixels x C) is staged in smem.
+// MET (forward only): also add the eval_metrics counters of the tile (utils/metrics.py:42-67, as eval_metrics_kernel
+// counts them) into counters = int64 [2 + 3C]: correct, labeled, inter[C], pred[C], lab[C].  "Labeled" is 0 <= t < C,
+// whatever the loss's ignore_index; the prediction is the arg-max of the same interpolated fp32 values the loss uses
+// (first maximum wins).  The block counts into a shared-memory histogram behind the source patch and flushes it with one
+// global atomic per non-zero bin: integer sums, so the counters do not depend on the order of the blocks.
+template <bool BWD, int K, bool MET = false>
 __global__ void __launch_bounds__(256) upsample_ce_kernel(const float* __restrict__ lo, const int64_t* __restrict__ target,
                                                           int N, int Hi, int Wi, int Ho, int Wo, int C, int ac, float sh,
                                                           float sw, int64_t ignore, LossArgs la, double* accum, int32_t* argmax,
                                                           const float* __restrict__ gscale,
-                                                          unsigned long long* __restrict__ dlo_fixed, int patch, int tile) {
+                                                          unsigned long long* __restrict__ dlo_fixed, int patch, int tile,
+                                                          unsigned long long* __restrict__ counters) {
   extern __shared__ unsigned long long sm64[];
   unsigned long long* dst = BWD ? sm64 : nullptr;  // [patch*patch][C] fixed-point grad accumulators
   float* src = reinterpret_cast<float*>(BWD ? sm64 + patch * patch * C : sm64);  // [patch*patch][C]
+  unsigned int* hist = MET ? reinterpret_cast<unsigned int*>(src + patch * patch * C) : nullptr;  // [2 + 3C], as counters
   const int tiles_x = (Wo + tile - 1) / tile, tiles_y = (Ho + tile - 1) / tile;
   int t = blockIdx.x;
   const int tx = t % tiles_x;
@@ -285,8 +292,11 @@ __global__ void __launch_bounds__(256) upsample_ce_kernel(const float* __restric
     src[i] = lo[(((int64_t)n * Hi + sy0 + py) * Wi + sx0 + px) * C + c];
     if (BWD) dst[i] = 0ull;
   }
+  if (MET)
+    for (int i = threadIdx.x; i < 3 * C + 2; i += blockDim.x) hist[i] = 0u;
   __syncthreads();
   double loss = 0.0, cnt = 0.0;
+  unsigned int n_correct = 0u, n_labeled = 0u;
   float g = 0.f;
   double scale = 0.0;
   if (BWD) {
@@ -298,8 +308,9 @@ __global__ void __launch_bounds__(256) upsample_ce_kernel(const float* __restric
     if (oy >= Ho || ox >= Wo) continue;
     const int64_t tg = target[((int64_t)n * Ho + oy) * Wo + ox];
     const bool valid = tg != ignore;
+    const bool labeled = MET && tg >= 0 && tg < C;
     if (K == LOSS_FOCAL && !BWD) cnt += 1.0;
-    if (!valid && (BWD || argmax == nullptr)) continue;
+    if (!valid && (BWD || (argmax == nullptr && !labeled))) continue;
     const Lerp2 ly = src_idx(oy, sh, Hi, ac), lx = src_idx(ox, sw, Wi, ac);
     const float h1 = ly.l1, h0 = 1.f - h1, w1 = lx.l1, w0 = 1.f - w1;
     const float* pa = src + ((ly.i0 - sy0) * pw + (lx.i0 - sx0)) * C;
@@ -323,6 +334,15 @@ __global__ void __launch_bounds__(256) upsample_ce_kernel(const float* __restric
     }
     if (!BWD) {
       if (argmax) argmax[((int64_t)n * Ho + oy) * Wo + ox] = am;
+      if (MET && labeled) {
+        ++n_labeled;
+        atomicAdd(&hist[2 + C + am], 1u);          // area_pred
+        atomicAdd(&hist[2 + 2 * C + (int)tg], 1u);  // area_lab
+        if (am == (int)tg) {
+          ++n_correct;
+          atomicAdd(&hist[2 + (int)tg], 1u);  // area_inter
+        }
+      }
       if (valid) {
         const float w = K == LOSS_CE ? 1.f : class_weight(la, tg, C);
         loss += (double)pixel_loss<K>(mx + logf(se) - lt, w, la.gamma);
@@ -348,6 +368,19 @@ __global__ void __launch_bounds__(256) upsample_ce_kernel(const float* __restric
   }
   if (!BWD) {
     block_accum2(loss, cnt, accum);
+    if (MET) {
+      n_correct = __reduce_add_sync(0xffffffffu, n_correct);
+      n_labeled = __reduce_add_sync(0xffffffffu, n_labeled);
+      if ((threadIdx.x & 31) == 0) {
+        atomicAdd(&hist[0], n_correct);
+        atomicAdd(&hist[1], n_labeled);
+      }
+      __syncthreads();
+      for (int i = threadIdx.x; i < 3 * C + 2; i += blockDim.x) {
+        const unsigned int v = hist[i];
+        if (v != 0u) atomicAdd(counters + i, (unsigned long long)v);
+      }
+    }
   } else {
     __syncthreads();
     for (int i = threadIdx.x; i < ph * pw * C; i += blockDim.x) {
@@ -411,24 +444,26 @@ static int ce_nchw_bwd(const float* logits, const int64_t* target, int N, int C,
   return check_launch("ce_nchw_bwd");
 }
 
-template <int K>
+// MET: counters (int64 [2 + 3C]) += the eval_metrics counters of the batch
+template <int K, bool MET = false>
 static int upsample_ce_fwd(const float* logits_lo, const int64_t* target, int N, int Hi, int Wi, int Ho, int Wo, int C,
                            int align_corners, int64_t ignore_index, LossArgs la, double* accum, int32_t* argmax,
-                           cudaStream_t stream) {
+                           int64_t* counters, cudaStream_t stream) {
   SEG_REQUIRE(C <= MAXC, "upsample_ce: C=%d > %d", C, MAXC);
+  SEG_REQUIRE(!MET || counters != nullptr, "upsample_ce: metrics counters are NULL");
   const int patch = std::max(patch_for(Hi, Ho, align_corners, TILE), patch_for(Wi, Wo, align_corners, TILE));
-  const size_t smem = (size_t)patch * patch * C * sizeof(float);
+  const size_t smem = (size_t)patch * patch * C * sizeof(float) + (MET ? (size_t)(3 * C + 2) * sizeof(unsigned int) : 0);
   SEG_REQUIRE(smem <= 200 * 1024, "upsample_ce: patch too large (%zu B)", smem);
   static size_t set_smem = 0;
   if (smem > set_smem) {
-    cudaFuncSetAttribute(upsample_ce_kernel<false, K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaFuncSetAttribute(upsample_ce_kernel<false, K, MET>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     set_smem = smem;
   }
   const int blocks = N * ceil_div(Ho, TILE) * ceil_div(Wo, TILE);
-  upsample_ce_kernel<false, K><<<blocks, 256, smem, stream>>>(
+  upsample_ce_kernel<false, K, MET><<<blocks, 256, smem, stream>>>(
       logits_lo, target, N, Hi, Wi, Ho, Wo, C, align_corners, rscale(Hi, Ho, align_corners), rscale(Wi, Wo, align_corners),
-      ignore_index, la, accum, argmax, nullptr, nullptr, patch, TILE);
-  return check_launch("upsample_ce_fwd");
+      ignore_index, la, accum, argmax, nullptr, nullptr, patch, TILE, reinterpret_cast<unsigned long long*>(counters));
+  return check_launch(MET ? "upsample_ce_fwd_metrics" : "upsample_ce_fwd");
 }
 
 template <int K>
@@ -455,7 +490,7 @@ static int upsample_ce_bwd(const float* logits_lo, const int64_t* target, int N,
   const float sh = rscale(Hi, Ho, align_corners), sw = rscale(Wi, Wo, align_corners);
   upsample_ce_kernel<true, K><<<blocks, 256, smem, stream>>>(
       logits_lo, target, N, Hi, Wi, Ho, Wo, C, align_corners, sh, sw, ignore_index, la, const_cast<double*>(accum), nullptr,
-      gscale, fixed, patch, tile);
+      gscale, fixed, patch, tile, nullptr);
   if (check_launch("upsample_ce_bwd")) return 1;
   const int64_t n = M * C;
   ce_grad_from_fixed_kernel<K><<<(unsigned)std::min<int64_t>(ceil_div64(n, 256), (int64_t)num_sms() * 8), 256, 0, stream>>>(
@@ -530,7 +565,13 @@ int seg_loss_finalize(const double* accum, int mean, float* loss, void* stream) 
 int seg_upsample_ce_fwd(const float* logits_lo, const int64_t* target, int N, int Hi, int Wi, int Ho, int Wo, int C,
                         int align_corners, int64_t ignore_index, double* accum, int32_t* argmax, void* stream) {
   return upsample_ce_fwd<LOSS_CE>(logits_lo, target, N, Hi, Wi, Ho, Wo, C, align_corners, ignore_index, LossArgs{}, accum,
-                                  argmax, ST(stream));
+                                  argmax, nullptr, ST(stream));
+}
+int seg_upsample_ce_fwd_metrics(const float* logits_lo, const int64_t* target, int N, int Hi, int Wi, int Ho, int Wo, int C,
+                                int align_corners, int64_t ignore_index, double* accum, int32_t* argmax, int64_t* counters,
+                                void* stream) {
+  return upsample_ce_fwd<LOSS_CE, true>(logits_lo, target, N, Hi, Wi, Ho, Wo, C, align_corners, ignore_index, LossArgs{},
+                                        accum, argmax, counters, ST(stream));
 }
 int seg_upsample_loss_fwd(const float* logits_lo, const int64_t* target, int N, int Hi, int Wi, int Ho, int Wo, int C,
                           int align_corners, int64_t ignore_index, const float* weight, int focal, float gamma, double* accum,
@@ -538,7 +579,17 @@ int seg_upsample_loss_fwd(const float* logits_lo, const int64_t* target, int N, 
   LossArgs la;
   if (loss_args(weight, focal, gamma, 1, C, &la)) return 1;
   return SEG_LOSS_DISPATCH(focal, upsample_ce_fwd, logits_lo, target, N, Hi, Wi, Ho, Wo, C, align_corners, ignore_index, la, accum,
-                           argmax, ST(stream));
+                           argmax, nullptr, ST(stream));
+}
+int seg_upsample_loss_fwd_metrics(const float* logits_lo, const int64_t* target, int N, int Hi, int Wi, int Ho, int Wo, int C,
+                                  int align_corners, int64_t ignore_index, const float* weight, int focal, float gamma,
+                                  double* accum, int32_t* argmax, int64_t* counters, void* stream) {
+  LossArgs la;
+  if (loss_args(weight, focal, gamma, 1, C, &la)) return 1;
+  return focal ? upsample_ce_fwd<LOSS_FOCAL, true>(logits_lo, target, N, Hi, Wi, Ho, Wo, C, align_corners, ignore_index, la,
+                                                   accum, argmax, counters, ST(stream))
+               : upsample_ce_fwd<LOSS_WCE, true>(logits_lo, target, N, Hi, Wi, Ho, Wo, C, align_corners, ignore_index, la,
+                                                 accum, argmax, counters, ST(stream));
 }
 
 // dlo_f32: fp32 [N,Hi,Wi,C]; dlo_fixed: int64 scratch [N,Hi,Wi,C] (zeroed here); dx: bf16 [N*Hi*Wi][lddx] or NULL

@@ -99,6 +99,8 @@ _SIGS = {
     "seg_loss_finalize": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
     "seg_upsample_loss_fwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int64, c_void_p, c_int, c_float, c_void_p, c_void_p, c_void_p]),
     "seg_upsample_loss_bwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int64, c_void_p, c_int, c_float, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
+    "seg_upsample_ce_fwd_metrics": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int64, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "seg_upsample_loss_fwd_metrics": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int64, c_void_p, c_int, c_float, c_void_p, c_void_p, c_void_p, c_void_p]),
     "seg_relu_fwd": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int64, c_int, c_void_p]),
     "seg_relu_bwd": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int64, c_int, c_float, c_void_p]),
     "seg_nhwc_to_nchw_f32": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),

@@ -530,14 +530,25 @@ def eval_metrics_nchw(logits, target, num_class):
     return out
 
 
-def upsample_ce_fwd(logits_lo, target, align_corners, ignore_index, want_argmax=False, reduce_fn=None):
+def _check_counters(counters, C):
+    assert counters.dtype == torch.int64 and counters.is_contiguous() and counters.numel() == 2 + 3 * C
+
+
+def upsample_ce_fwd(logits_lo, target, align_corners, ignore_index, want_argmax=False, reduce_fn=None, counters=None):
+    """counters: None, or an int64 device vector [2 + 3C] that the same launch ADDS the batch's eval_metrics counters to
+    (the layout of eval_metrics_nchw with num_class = C)."""
     N, Hi, Wi, C = logits_lo.shape
     _, Ho, Wo = target.shape
     assert logits_lo.is_contiguous() and logits_lo.dtype == torch.float32 and target.is_contiguous()
     accum = torch.zeros(2, dtype=torch.float64, device=logits_lo.device)
     am = torch.empty((N, Ho, Wo), dtype=torch.int32, device=logits_lo.device) if want_argmax else None
-    call("seg_upsample_ce_fwd", ptr(logits_lo), ptr(target), N, Hi, Wi, Ho, Wo, C, int(align_corners), int(ignore_index),
-         ptr(accum), ptr(am))
+    if counters is None:
+        call("seg_upsample_ce_fwd", ptr(logits_lo), ptr(target), N, Hi, Wi, Ho, Wo, C, int(align_corners), int(ignore_index),
+             ptr(accum), ptr(am))
+    else:
+        _check_counters(counters, C)
+        call("seg_upsample_ce_fwd_metrics", ptr(logits_lo), ptr(target), N, Hi, Wi, Ho, Wo, C, int(align_corners),
+             int(ignore_index), ptr(accum), ptr(am), ptr(counters))
     if reduce_fn is not None:  # cross-rank sum of the fp64 (loss sum, valid-pixel count) pair: global-batch mean
         reduce_fn(accum)
     loss = torch.empty((), dtype=torch.float32, device=logits_lo.device)
@@ -557,7 +568,7 @@ def upsample_ce_bwd(logits_lo, target, align_corners, ignore_index, accum, ldx, 
 
 
 def upsample_loss_fwd(logits_lo, target, align_corners, ignore_index, weight=None, gamma=None, mean=True, want_argmax=False,
-                      reduce_fn=None):
+                      reduce_fn=None, counters=None):
     """upsample_ce_fwd for the class-weighted CE (gamma None) and focal (gamma >= 0) losses of loss_nchw_fwd."""
     N, Hi, Wi, C = logits_lo.shape
     _, Ho, Wo = target.shape
@@ -565,8 +576,13 @@ def upsample_loss_fwd(logits_lo, target, align_corners, ignore_index, weight=Non
     assert weight is None or (weight.dtype == torch.float32 and weight.numel() == C and weight.is_contiguous())
     accum = torch.zeros(2, dtype=torch.float64, device=logits_lo.device)
     am = torch.empty((N, Ho, Wo), dtype=torch.int32, device=logits_lo.device) if want_argmax else None
-    call("seg_upsample_loss_fwd", ptr(logits_lo), ptr(target), N, Hi, Wi, Ho, Wo, C, int(align_corners), int(ignore_index),
-         ptr(weight), int(gamma is not None), float(gamma or 0.0), ptr(accum), ptr(am))
+    if counters is None:
+        call("seg_upsample_loss_fwd", ptr(logits_lo), ptr(target), N, Hi, Wi, Ho, Wo, C, int(align_corners), int(ignore_index),
+             ptr(weight), int(gamma is not None), float(gamma or 0.0), ptr(accum), ptr(am))
+    else:
+        _check_counters(counters, C)
+        call("seg_upsample_loss_fwd_metrics", ptr(logits_lo), ptr(target), N, Hi, Wi, Ho, Wo, C, int(align_corners),
+             int(ignore_index), ptr(weight), int(gamma is not None), float(gamma or 0.0), ptr(accum), ptr(am), ptr(counters))
     if reduce_fn is not None:
         reduce_fn(accum)
     loss = torch.empty((), dtype=torch.float32, device=logits_lo.device)

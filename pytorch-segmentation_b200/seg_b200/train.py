@@ -1,13 +1,15 @@
 """Fused training step for the engine models: forward -> fused upsample+CE (no full-resolution logits in HBM) ->
 backward -> (NCCL gradient all-reduce) -> fused multi-tensor SGD.  Same arithmetic as one iteration of the
 reference's Trainer._train_epoch (trainer.py:55-71) with torch.optim.SGD and differential learning rates
-(base/base_trainer.py:46-57), minus the host synchronisations.
+(base/base_trainer.py:46-57), minus the host synchronisations.  Optionally also the training metrics of trainer.py:84-86
+and the validation pass of Trainer._valid_epoch (trainer.py:109-165), from the same fused loss kernel.
 """
 import numpy as np
 import torch
 import torch.distributed as dist
 
 from . import lib, ops
+from . import metrics as _metrics
 from .engine import Tape
 
 
@@ -102,10 +104,17 @@ def _loss_spec(loss, ignore_index):
 
 class FusedTrainStep:
     """loss: None (the reference configs' CrossEntropyLoss2d(ignore_index=255)), or a seg_b200.CrossEntropyLoss2d /
-    seg_b200.FocalLoss instance, applied to the main head and (x aux_weight) to the aux head; its ignore_index governs."""
+    seg_b200.FocalLoss instance, applied to the main head and (x aux_weight) to the aux head; its ignore_index governs.
+
+    metrics=True: every step() and evaluate() adds the main head's eval_metrics counters (trainer.py:62,84) into the
+    device vector `seg_counters` (int64 [2 + 3C]: correct, labeled, inter[C], pred[C], lab[C]) inside the fused loss
+    launch, so graph replays count too; `seg_metrics()` turns the running totals into Trainer._get_seg_metrics's dict and
+    `reset_metrics()` zeroes them."""
+
+    EVAL_GRAPHS_MAX = 2  # evaluate() input shapes captured at most (the batch and a smaller last batch); others run eagerly
 
     def __init__(self, model, ignore_index=None, lr=0.01, backbone_lr_scale=0.1, momentum=0.9, weight_decay=1e-4,
-                 aux_weight=0.4, world=1, cuda_graph=False, bucket_mb=0.0, loss=None):
+                 aux_weight=0.4, world=1, cuda_graph=False, bucket_mb=0.0, loss=None, metrics=False):
         self.model = model
         self.ignore_index, self.loss_spec = _loss_spec(loss, ignore_index)
         self._momentum, self.wd = float(momentum), float(weight_decay)
@@ -163,6 +172,9 @@ class FusedTrainStep:
         self.cuda_graph = cuda_graph
         self._graph = None
         self._static = None
+        self._eval_graphs = {}  # (x shape, target shape) -> (static x, static target, loss, graph) of evaluate()
+        self.num_classes = model.num_classes
+        self.seg_counters = torch.zeros(2 + 3 * self.num_classes, dtype=torch.int64, device=dev) if metrics else None
 
     @property
     def momentum(self):
@@ -192,12 +204,102 @@ class FusedTrainStep:
         return self._static[2]
 
     def release_graph(self):
-        """Drop the captured graph.  Required before torch.distributed.destroy_process_group() when world > 1: NCCL
-        keeps a communicator alive (and its destruction blocks) while a graph that captured its kernels exists."""
+        """Drop the captured graphs (the step's and evaluate()'s).  Required before
+        torch.distributed.destroy_process_group() when world > 1: NCCL keeps a communicator alive (and its destruction
+        blocks) while a graph that captured its kernels exists."""
         torch.cuda.synchronize()
         self._graph = None
         self._static = None
+        self._eval_graphs = {}
         torch.cuda.synchronize()
+
+    def reset_metrics(self):
+        """Zero the metric counters (Trainer._reset_metrics, trainer.py:173-178): one device op, no synchronisation."""
+        self._require_metrics()
+        self.seg_counters.zero_()
+
+    def seg_metrics(self):
+        """Trainer._get_seg_metrics (trainer.py:186-194) of everything counted since the last reset_metrics():
+        {"Pixel_Accuracy", "Mean_IoU", "Class_IoU"}.  One small device-to-host copy; at world > 1 the counters are summed
+        over the ranks here (one all-reduce), which gives the metrics of the batch nn.DataParallel gathers."""
+        self._require_metrics()
+        v = self.seg_counters
+        if self.world > 1:
+            v = v.clone()
+            dist.all_reduce(v)
+        return _metrics.seg_metrics(v.cpu().numpy(), self.num_classes)
+
+    def _require_metrics(self):
+        if self.seg_counters is None:
+            raise RuntimeError("FusedTrainStep counts metrics only when constructed with metrics=True")
+
+    def evaluate(self, x, target):
+        """The per-batch work of Trainer._valid_epoch (trainer.py:125-132): an eval-mode forward of the main head
+        (BatchNorm running statistics, no dropout, no SyncBN exchange), the fused upsample + loss forward with the step's
+        loss (the global-batch mean under data parallel, as in training) and, with metrics=True, the counters.  Returns
+        the loss as a device scalar; with cuda_graph=True it lives in a static buffer that the next evaluate() of the same
+        shape overwrites.  Changes no parameter, momentum, BatchNorm buffer, dropout step counter or model.training."""
+        if not self.cuda_graph:
+            return self._evaluate_impl(x, target)
+        key = (tuple(x.shape), tuple(target.shape))
+        entry = self._eval_graphs.get(key)
+        if entry is None:
+            if len(self._eval_graphs) >= self.EVAL_GRAPHS_MAX:  # every graph owns a memory pool the size of the forward's
+                return self._evaluate_impl(x, target)
+            entry = self._eval_graphs[key] = self._capture_eval(x, target)
+        xs, ys, loss, g = entry
+        xs.copy_(x, non_blocking=True)
+        ys.copy_(target, non_blocking=True)
+        g.replay()
+        return loss
+
+    def _capture_eval(self, x, target):
+        xs, ys = x.clone(), target.clone()
+        cur = torch.cuda.current_stream()
+        side = torch.cuda.Stream()
+        side.wait_stream(cur)
+        # one eager pass outside the capture (lazy one-time initialisation, allocator pools); its counts are rolled back
+        with torch.cuda.stream(side):
+            saved = None if self.seg_counters is None else self.seg_counters.clone()
+            self._evaluate_impl(xs, ys)
+            if saved is not None:
+                self.seg_counters.copy_(saved)
+        cur.wait_stream(side)
+        torch.cuda.synchronize()
+        g = torch.cuda.CUDAGraph()
+        if self.world > 1:  # every rank has finished its eager exchange before anyone starts capturing
+            dist.barrier()
+        with torch.cuda.graph(g, capture_error_mode="thread_local" if self.world > 1 else "global"):
+            loss = self._evaluate_impl(xs, ys)
+        return xs, ys, loss, g
+
+    def _evaluate_impl(self, x, target):
+        m = self.model
+        self.wt.pack()
+        tape = m._new_tape(False, False)  # eval mode: running statistics, no dropout, no step-counter increment
+        tape.packed_override = self.wt.packed_bufs
+        was = m.training
+        m.training = False  # PSPNet builds its aux head only in training mode (pspnet.py:91); only the main head is scored
+        try:
+            lo, ac = m._forward_heads(tape, x.contiguous().float())[0]
+        finally:
+            m.training = was
+        loss, _, _ = self._loss_fwd(lo.t, target, ac, self.seg_counters)
+        return loss
+
+    def _loss_fwd(self, lo_t, target, ac, counters):
+        """(loss, fp64 accum, class weights) of one head.  Mean over the valid pixels of the GLOBAL batch, as
+        nn.DataParallel's gathered logits give the reference (trainer.py:60-66): the (loss sum, denominator) pair is
+        all-reduced (16 bytes); a 'sum' is the global sum."""
+        rf = (lambda acc: dist.all_reduce(acc)) if self.world > 1 else None
+        spec = self.loss_spec
+        if spec is None:
+            loss, accum, _ = ops.upsample_ce_fwd(lo_t, target, ac, self.ignore_index, reduce_fn=rf, counters=counters)
+            return loss, accum, None
+        cw = spec.weight_on(lo_t.device, lo_t.shape[-1])
+        loss, accum, _ = ops.upsample_loss_fwd(lo_t, target, ac, self.ignore_index, cw, spec.gamma, spec.mean, reduce_fn=rf,
+                                               counters=counters)
+        return loss, accum, cw
 
     def _invalidate_param_caches(self):
         """The SGD kernel updates parameters in place without bumping autograd version counters: drop the per-parameter
@@ -213,6 +315,8 @@ class FusedTrainStep:
         # warm-up outside the capture (lazy one-time initialisation, allocator pools): two real steps whose effect on
         # the training state (parameters, momentum, BN running statistics) is rolled back afterwards
         state = [p.data for p in self.params] + [self.flat_mom] + [b for b in self.model.buffers()]
+        if self.seg_counters is not None:
+            state.append(self.seg_counters)
         with torch.cuda.stream(side):
             saved = [t.clone() for t in state]
             for _ in range(2):
@@ -280,19 +384,12 @@ class FusedTrainStep:
         tape.packed_override, tape.dw_buffers = self.wt.packed_bufs, self.wt.dw_bufs
         heads = m._forward_heads(tape, x.contiguous().float())
         total = None
-        # mean over the valid pixels of the GLOBAL batch, as nn.DataParallel's gathered logits give the reference
-        # (trainer.py:60-66): the (loss sum, valid count) pair is all-reduced — 16 bytes — and the gradient is scaled by
-        # world because the exchanged gradients are averaged over ranks below
-        # (a weighted or focal loss all-reduces its (sum, denominator) pair the same way; a 'sum' is the global sum)
-        rf = (lambda acc: dist.all_reduce(acc)) if self.world > 1 else None
         spec = self.loss_spec
         for i, (lo, ac) in enumerate(heads):
             C = lo.t.shape[-1]
-            if spec is None:
-                loss, accum, _ = ops.upsample_ce_fwd(lo.t, target, ac, self.ignore_index, reduce_fn=rf)
-            else:
-                cw = spec.weight_on(lo.t.device, C)
-                loss, accum, _ = ops.upsample_loss_fwd(lo.t, target, ac, self.ignore_index, cw, spec.gamma, spec.mean, reduce_fn=rf)
+            # the main head only is counted (trainer.py:62); the gradient is scaled by world because the exchanged
+            # gradients are averaged over ranks below
+            loss, accum, cw = self._loss_fwd(lo.t, target, ac, self.seg_counters if i == 0 else None)
             w = 1.0 if i == 0 else self.aux_weight
             wg = w * self.world
             g = None if wg == 1.0 else torch.full((1,), wg, dtype=torch.float32, device=lo.t.device)
