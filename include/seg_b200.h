@@ -226,13 +226,54 @@ int seg_bilinear_logits_bwd(const float* dy_nchw, void* dx, int lddx, int N, int
                             int align_corners, void* stream);
 
 /* ---- per-pixel loss ---- */
-/* CrossEntropyLoss2d (utils/losses.py:24-31): logits NCHW fp32, target int64 [N,H,W].
- * accum[0] += sum of -log p[target] over valid pixels, accum[1] += number of valid pixels (both fp64). */
-int seg_ce_nchw_fwd(const float* logits, const int64_t* target, int N, int C, int H, int W, int64_t ignore_index,
-                    double* accum, void* stream);
-/* dlogits = (softmax - onehot) * gscale / accum[1] for valid pixels, 0 for ignored (gscale = upstream grad) */
-int seg_ce_nchw_bwd(const float* logits, const int64_t* target, int N, int C, int H, int W, int64_t ignore_index,
-                    const double* accum, const float* gscale, float* dlogits, void* stream);
+/* Cross-entropy, class-weighted cross-entropy and focal loss, one family of entry points with the loss picked by `kind`:
+ * CrossEntropyLoss2d(weight, reduction) (utils/losses.py:24-31), FocalLoss(gamma, alpha, size_average) (:52-65) and the
+ * CE half of CE_DiceLoss(weight, reduction) (:67-77).  With nll = lse(z) - z_t at a pixel labelled t != ignore_index and
+ * w = weight (fp32 [C], finite and >= 0; NULL = all ones):
+ *   SEG_LOSS_CE     per-pixel loss nll;                             accum[1] += 1 per valid pixel
+ *   SEG_LOSS_WCE    per-pixel loss L = w_t*nll;                     accum[1] += w_t per valid pixel
+ *   SEG_LOSS_FOCAL  per-pixel loss (1-pt)^gamma * L, pt = exp(-L);  accum[1] += 1 per pixel, ignored ones included
+ * (the reference's .mean() over the unreduced loss counts ignored pixels).  accum is fp64 [2], zeroed by the caller:
+ * accum[0] += the per-pixel losses, accum[1] += the denominator; it may be summed over ranks before the finalize and the
+ * backward.  SEG_LOSS_CE takes weight = NULL and mean = 1, an error otherwise; gamma (finite, >= 0) is read by
+ * SEG_LOSS_FOCAL only.  mean = 1: loss = accum[0]/accum[1], or 0 when accum[1] == 0 (ATen gives NaN there); mean = 0
+ * ('sum', size_average=False): loss = accum[0].
+ * Backward: dL/dz_c = g * w_t (p_c - delta_ct) * F'(L), 0 for ignored pixels, with F' = 1 except for focal, where
+ * F' = u^gamma (1 + gamma r), u = -expm1(-L), r = L/expm1(L) (1 at L = 0), so 0 <= F' <= 1 + gamma and a pixel whose pt
+ * rounds to 1 gets the finite limit (0 for gamma > 0; the reference's autograd gives NaN for 0 < gamma < 1).
+ * g = gscale/accum[1] (0 when accum[1] == 0; SEG_LOSS_CE: gscale/max(accum[1], 1), divided in fp32) or gscale for a sum;
+ * gscale = the upstream gradient (fp32 scalar on the device, NULL = 1). */
+#define SEG_LOSS_CE 0
+#define SEG_LOSS_WCE 1
+#define SEG_LOSS_FOCAL 2
+/* logits NCHW fp32, target int64 [N,H,W]; dlogits NCHW fp32 */
+int seg_loss_nchw_fwd(const float* logits, const int64_t* target, int N, int C, int H, int W, int64_t ignore_index,
+                      const float* weight, int kind, float gamma, double* accum, void* stream);
+int seg_loss_nchw_bwd(const float* logits, const int64_t* target, int N, int C, int H, int W, int64_t ignore_index,
+                      const float* weight, int kind, float gamma, int mean, const double* accum, const float* gscale,
+                      float* dlogits, void* stream);
+/* loss (fp32 scalar on the device) from accum, as above */
+int seg_loss_finalize(const double* accum, int mean, float* loss, void* stream);
+/* The same losses fused with the bilinear upsample: low-res NHWC fp32 logits [N,Hi,Wi,C] (C <= 160), upsampled as
+ * deeplabv3_plus.py:361 / pspnet.py:86 do, + log-softmax + NLL, with no full-resolution logits in HBM.
+ * argmax != NULL: also the arg-max label map (int32 [N,Ho,Wo], lowest index wins ties).
+ * counters != NULL: also the main head's eval_metrics (trainer.py:62,84 -> utils/metrics.py:59-67) in the same launch, so
+ * neither training nor validation needs the full-resolution logits for pixel accuracy and mIoU.  counters: int64
+ * [2 + 3*C] = correct, labeled, area_inter[C], area_pred[C], area_lab[C], the layout of seg_eval_metrics_nchw with
+ * num_class = C; ADDED to (not zeroed), so a running total needs no extra launch.  The prediction is the arg-max of the
+ * interpolated fp32 logits seg_bilinear_logits_fwd produces (lowest index wins ties); a pixel is labeled when
+ * 0 <= target < C, independently of ignore_index.  Integer counters: deterministic.
+ * Backward: d(logits_lo) is accumulated in 64-bit fixed point in the int64 scratch dlo_fixed [N,Hi,Wi,C] (zeroed here;
+ * order-independent, hence bit-reproducible) with the scale derived from the bound |g| * max(w) * (1 + gamma) (the
+ * factors the kind has), converted to fp32 dlo_f32 [N,Hi,Wi,C], then written as bf16 NHWC with pitch lddx (channels
+ * C..lddx-1 zero) when dx != NULL. */
+int seg_upsample_loss_fwd(const float* logits_lo, const int64_t* target, int N, int Hi, int Wi, int Ho, int Wo, int C,
+                          int align_corners, int64_t ignore_index, const float* weight, int kind, float gamma, double* accum,
+                          int32_t* argmax, int64_t* counters, void* stream);
+int seg_upsample_loss_bwd(const float* logits_lo, const int64_t* target, int N, int Hi, int Wi, int Ho, int Wo, int C,
+                          int align_corners, int64_t ignore_index, const float* weight, int kind, float gamma, int mean,
+                          const double* accum, const float* gscale, float* dlo_f32, void* dlo_fixed, void* dx, int lddx,
+                          void* stream);
 /* DiceLoss (utils/losses.py:33-50): softmax over C, intersection with the one-hot target, whole-batch ratio.
  * accum (fp64 [2], zeroed by the caller) receives (sum p[target], #pixels); loss = 1 - (2I+s)/(2*#pixels+s).
  * The caller applies the reference's in-place target fix-up (losses.py:40-42) before calling. */
@@ -258,57 +299,6 @@ int seg_lovasz_softmax_nchw(const float* logits, const int64_t* target, int N, i
  * area_pred[K], area_lab[K]; union = pred + lab - inter.  Integer counters: bit-exact with the reference. */
 int seg_eval_metrics_nchw(const float* logits, const int64_t* target, int N, int C, int H, int W, int num_class,
                           int64_t* out, void* stream);
-/* fused: bilinear upsample (low-res NHWC fp32 logits) + log-softmax + NLL, no full-res logits in HBM.
- * Also emits the arg-max label map (int32 [N,Ho,Wo], lowest index wins ties) when argmax != NULL. */
-int seg_upsample_ce_fwd(const float* logits_lo, const int64_t* target, int N, int Hi, int Wi, int Ho, int Wo, int C,
-                        int align_corners, int64_t ignore_index, double* accum, int32_t* argmax, void* stream);
-/* d(logits_lo) of mean CE: accumulated in 64-bit fixed point in the int64 scratch dlo_fixed [N,Hi,Wi,C] (zeroed here;
- * order-independent, hence bit-reproducible), converted to fp32 dlo_f32 [N,Hi,Wi,C], then written as bf16 NHWC with pitch
- * lddx (channels C..lddx-1 zero) when dx != NULL; gscale = upstream grad (fp32 scalar on device) */
-int seg_upsample_ce_bwd(const float* logits_lo, const int64_t* target, int N, int Hi, int Wi, int Ho, int Wo, int C,
-                        int align_corners, int64_t ignore_index, const double* accum, const float* gscale,
-                        float* dlo_f32, void* dlo_fixed, void* dx, int lddx, void* stream);
-/* loss = accum[0]/accum[1] (fp32 scalar) */
-int seg_ce_finalize(const double* accum, float* loss, void* stream);
-
-/* Class-weighted cross-entropy and focal loss (utils/losses.py:24-31 CrossEntropyLoss2d(weight, reduction),
- * :52-65 FocalLoss(gamma, alpha, size_average), :67-77 CE_DiceLoss(weight, reduction)).  With nll = lse(z) - z_t at a
- * pixel labelled t != ignore_index and w = weight (fp32 [C], finite and >= 0; NULL = all ones):
- *   focal = 0:  per-pixel loss w_t*nll;                          accum[1] += w_t over valid pixels
- *   focal = 1:  per-pixel loss (1-pt)^gamma * L, L = w_t*nll, pt = exp(-L);  accum[1] += 1 over EVERY pixel
- * (the reference's .mean() over the unreduced loss counts ignored pixels).  accum[0] += the per-pixel losses; accum is
- * fp64 [2], zeroed by the caller.  mean = 1: loss = accum[0]/accum[1], or 0 when accum[1] == 0 (ATen gives NaN there);
- * mean = 0 ('sum', size_average=False): loss = accum[0].  gamma >= 0, finite.
- * Backward: dL/dz_c = g * w_t (p_c - delta_ct) * F'(L), F' = u^gamma (1 + gamma r), u = -expm1(-L), r = L/expm1(L)
- * (1 at L = 0), so 0 <= F' <= 1 + gamma and a pixel whose pt rounds to 1 gets the finite limit (0 for gamma > 0; the
- * reference's autograd gives NaN for 0 < gamma < 1); g = gscale/accum[1] (0 when accum[1] == 0) or gscale for a sum. */
-int seg_loss_nchw_fwd(const float* logits, const int64_t* target, int N, int C, int H, int W, int64_t ignore_index,
-                      const float* weight, int focal, float gamma, double* accum, void* stream);
-int seg_loss_nchw_bwd(const float* logits, const int64_t* target, int N, int C, int H, int W, int64_t ignore_index,
-                      const float* weight, int focal, float gamma, int mean, const double* accum, const float* gscale,
-                      float* dlogits, void* stream);
-int seg_loss_finalize(const double* accum, int mean, float* loss, void* stream);
-/* The same losses fused with the bilinear upsample, as seg_upsample_ce_fwd / seg_upsample_ce_bwd (same buffers, same
- * 64-bit fixed-point accumulation, C <= 160); the fixed-point scale is derived from |g| * max(w) * (1 + gamma). */
-int seg_upsample_loss_fwd(const float* logits_lo, const int64_t* target, int N, int Hi, int Wi, int Ho, int Wo, int C,
-                          int align_corners, int64_t ignore_index, const float* weight, int focal, float gamma, double* accum,
-                          int32_t* argmax, void* stream);
-int seg_upsample_loss_bwd(const float* logits_lo, const int64_t* target, int N, int Hi, int Wi, int Ho, int Wo, int C,
-                          int align_corners, int64_t ignore_index, const float* weight, int focal, float gamma, int mean,
-                          const double* accum, const float* gscale, float* dlo_f32, void* dlo_fixed, void* dx, int lddx,
-                          void* stream);
-/* seg_upsample_ce_fwd / seg_upsample_loss_fwd that also count the main head's eval_metrics (trainer.py:62,84 ->
- * utils/metrics.py:59-67) in the same launch, so neither training nor validation needs the full-resolution logits for
- * pixel accuracy and mIoU.  counters: int64 [2 + 3*C] = correct, labeled, area_inter[C], area_pred[C], area_lab[C], the
- * layout of seg_eval_metrics_nchw with num_class = C; ADDED to (not zeroed), so a running total needs no extra launch.
- * The prediction is the arg-max of the interpolated fp32 logits seg_bilinear_logits_fwd produces (lowest index wins
- * ties); a pixel is labeled when 0 <= target < C, independently of ignore_index.  Integer counters: deterministic. */
-int seg_upsample_ce_fwd_metrics(const float* logits_lo, const int64_t* target, int N, int Hi, int Wi, int Ho, int Wo, int C,
-                                int align_corners, int64_t ignore_index, double* accum, int32_t* argmax, int64_t* counters,
-                                void* stream);
-int seg_upsample_loss_fwd_metrics(const float* logits_lo, const int64_t* target, int N, int Hi, int Wi, int Ho, int Wo, int C,
-                                  int align_corners, int64_t ignore_index, const float* weight, int focal, float gamma,
-                                  double* accum, int32_t* argmax, int64_t* counters, void* stream);
 
 /* ---- misc ---- */
 /* standalone ReLU on NHWC bf16 (F.relu, deeplabv3_plus.py:210) and its backward dx = beta*dx + dy*(y>0) */

@@ -32,13 +32,13 @@ __device__ __forceinline__ void block_accum2(double a, double b, double* out) {
 }
 
 // Per-pixel loss variants (utils/losses.py:24-31,52-65,67-77).  With nll = lse(z) - z_t at a pixel labelled t:
-//   LOSS_CE     nll                       denominator: valid pixels      (today's unweighted mean CE, unchanged)
+//   LOSS_CE     nll                       denominator: valid pixels      (unweighted mean CE)
 //   LOSS_WCE    L = w_t * nll             denominator: sum of valid w_t  (nn.CrossEntropyLoss(weight); w = 1 without one)
 //   LOSS_FOCAL  (1 - pt)^gamma * L, pt = exp(-L)   denominator: every pixel, ignored ones included (FocalLoss's .mean())
 // accum[1] holds the denominator; the 'sum' reductions ignore it.  dL/dz_c = w_t (p_c - delta_ct) F'(L) with the focal
 // factor F'(L) = u^gamma (1 + gamma r), u = -expm1(-L), r = L / expm1(L) (r = 1 at L = 0): u and r lie in [0, 1], so
 // 0 <= F' <= 1 + gamma, and no 0 * inf is formed where pt rounds to 1 (F' -> 0 there for gamma > 0).
-enum LossKind { LOSS_CE = 0, LOSS_WCE = 1, LOSS_FOCAL = 2 };
+enum LossKind { LOSS_CE = SEG_LOSS_CE, LOSS_WCE = SEG_LOSS_WCE, LOSS_FOCAL = SEG_LOSS_FOCAL };
 struct LossArgs {
   const float* weight;  // fp32 [C] (finite, >= 0) or NULL = all ones; unused by LOSS_CE
   float gamma;          // LOSS_FOCAL only
@@ -192,10 +192,8 @@ __global__ void dice_finalize_kernel(const double* accum, float smooth, float* l
     *loss = (float)(1.0 - (2.0 * accum[0] + smooth) / (accum[1] + accum[1] + smooth));
 }
 
-__global__ void ce_finalize_kernel(const double* accum, float* loss) {
-  if (threadIdx.x == 0 && blockIdx.x == 0) *loss = (float)(accum[0] / fmax(accum[1], 1.0));
-}
-// weighted / focal: a mean with a zero denominator is 0 (see loss_grad_g); a sum is accum[0]
+// a mean with a zero denominator is 0 (see loss_grad_g); a sum is accum[0]
+// LOSS_CE (mean): accum[1] is an integer count and accum[0] is +0.0 when it is 0, so this equals accum[0] / fmax(accum[1], 1)
 __global__ void loss_finalize_kernel(const double* accum, int mean, float* loss) {
   if (threadIdx.x == 0 && blockIdx.x == 0) *loss = (float)(!mean ? accum[0] : accum[1] > 0.0 ? accum[0] / accum[1] : 0.0);
 }
@@ -444,26 +442,27 @@ static int ce_nchw_bwd(const float* logits, const int64_t* target, int N, int C,
   return check_launch("ce_nchw_bwd");
 }
 
-// MET: counters (int64 [2 + 3C]) += the eval_metrics counters of the batch
-template <int K, bool MET = false>
+// counters != NULL: counters (int64 [2 + 3C]) += the eval_metrics counters of the batch (the MET instantiation)
+template <int K>
 static int upsample_ce_fwd(const float* logits_lo, const int64_t* target, int N, int Hi, int Wi, int Ho, int Wo, int C,
                            int align_corners, int64_t ignore_index, LossArgs la, double* accum, int32_t* argmax,
                            int64_t* counters, cudaStream_t stream) {
   SEG_REQUIRE(C <= MAXC, "upsample_ce: C=%d > %d", C, MAXC);
-  SEG_REQUIRE(!MET || counters != nullptr, "upsample_ce: metrics counters are NULL");
+  const bool met = counters != nullptr;
+  const auto kernel = met ? upsample_ce_kernel<false, K, true> : upsample_ce_kernel<false, K, false>;
   const int patch = std::max(patch_for(Hi, Ho, align_corners, TILE), patch_for(Wi, Wo, align_corners, TILE));
-  const size_t smem = (size_t)patch * patch * C * sizeof(float) + (MET ? (size_t)(3 * C + 2) * sizeof(unsigned int) : 0);
+  const size_t smem = (size_t)patch * patch * C * sizeof(float) + (met ? (size_t)(3 * C + 2) * sizeof(unsigned int) : 0);
   SEG_REQUIRE(smem <= 200 * 1024, "upsample_ce: patch too large (%zu B)", smem);
-  static size_t set_smem = 0;
-  if (smem > set_smem) {
-    cudaFuncSetAttribute(upsample_ce_kernel<false, K, MET>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    set_smem = smem;
+  static size_t set_smem[2] = {0, 0};  // per instantiation
+  if (smem > set_smem[met]) {
+    cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    set_smem[met] = smem;
   }
   const int blocks = N * ceil_div(Ho, TILE) * ceil_div(Wo, TILE);
-  upsample_ce_kernel<false, K, MET><<<blocks, 256, smem, stream>>>(
+  kernel<<<blocks, 256, smem, stream>>>(
       logits_lo, target, N, Hi, Wi, Ho, Wo, C, align_corners, rscale(Hi, Ho, align_corners), rscale(Wi, Wo, align_corners),
       ignore_index, la, accum, argmax, nullptr, nullptr, patch, TILE, reinterpret_cast<unsigned long long*>(counters));
-  return check_launch(MET ? "upsample_ce_fwd_metrics" : "upsample_ce_fwd");
+  return check_launch(met ? "upsample_ce_fwd_metrics" : "upsample_ce_fwd");
 }
 
 template <int K>
@@ -504,38 +503,36 @@ static int upsample_ce_bwd(const float* logits_lo, const int64_t* target, int N,
   return 0;
 }
 
-// the weighted / focal entry points: focal selects LOSS_FOCAL (weight optional), otherwise LOSS_WCE (NULL weight = ones)
-static int loss_args(const float* weight, int focal, float gamma, int mean, int C, LossArgs* la) {
+// kind: LOSS_CE (weight NULL, a mean), LOSS_WCE (NULL weight = ones) or LOSS_FOCAL (weight optional)
+static int loss_args(const float* weight, int kind, float gamma, int mean, int C, LossArgs* la) {
   SEG_REQUIRE(C > 0, "loss: C=%d", C);
-  SEG_REQUIRE(!focal || (gamma >= 0.f && isfinite(gamma)), "loss: focal gamma must be finite and >= 0 (got %g)", (double)gamma);
+  SEG_REQUIRE(kind == LOSS_CE || kind == LOSS_WCE || kind == LOSS_FOCAL, "loss: unknown kind %d", kind);
+  SEG_REQUIRE(kind != LOSS_CE || (weight == nullptr && mean), "loss: SEG_LOSS_CE takes no class weight and is a mean");
+  SEG_REQUIRE(kind != LOSS_FOCAL || (gamma >= 0.f && isfinite(gamma)), "loss: focal gamma must be finite and >= 0 (got %g)",
+              (double)gamma);
   *la = LossArgs{weight, gamma, mean ? 1 : 0};
   return 0;
 }
-#define SEG_LOSS_DISPATCH(focal, fn, ...) ((focal) ? fn<LOSS_FOCAL>(__VA_ARGS__) : fn<LOSS_WCE>(__VA_ARGS__))
+#define SEG_LOSS_DISPATCH(kind, fn, ...)                   \
+  ((kind) == LOSS_CE    ? fn<LOSS_CE>(__VA_ARGS__)         \
+   : (kind) == LOSS_WCE ? fn<LOSS_WCE>(__VA_ARGS__)        \
+                        : fn<LOSS_FOCAL>(__VA_ARGS__))
 }  // namespace seg
 
 extern "C" {
 
-int seg_ce_nchw_fwd(const float* logits, const int64_t* target, int N, int C, int H, int W, int64_t ignore_index,
-                    double* accum, void* stream) {
-  return ce_nchw_fwd<LOSS_CE>(logits, target, N, C, H, W, ignore_index, LossArgs{}, accum, ST(stream));
-}
-int seg_ce_nchw_bwd(const float* logits, const int64_t* target, int N, int C, int H, int W, int64_t ignore_index,
-                    const double* accum, const float* gscale, float* dlogits, void* stream) {
-  return ce_nchw_bwd<LOSS_CE>(logits, target, N, C, H, W, ignore_index, LossArgs{}, accum, gscale, dlogits, ST(stream));
-}
 int seg_loss_nchw_fwd(const float* logits, const int64_t* target, int N, int C, int H, int W, int64_t ignore_index,
-                      const float* weight, int focal, float gamma, double* accum, void* stream) {
+                      const float* weight, int kind, float gamma, double* accum, void* stream) {
   LossArgs la;
-  if (loss_args(weight, focal, gamma, 1, C, &la)) return 1;
-  return SEG_LOSS_DISPATCH(focal, ce_nchw_fwd, logits, target, N, C, H, W, ignore_index, la, accum, ST(stream));
+  if (loss_args(weight, kind, gamma, 1, C, &la)) return 1;
+  return SEG_LOSS_DISPATCH(kind, ce_nchw_fwd, logits, target, N, C, H, W, ignore_index, la, accum, ST(stream));
 }
 int seg_loss_nchw_bwd(const float* logits, const int64_t* target, int N, int C, int H, int W, int64_t ignore_index,
-                      const float* weight, int focal, float gamma, int mean, const double* accum, const float* gscale,
+                      const float* weight, int kind, float gamma, int mean, const double* accum, const float* gscale,
                       float* dlogits, void* stream) {
   LossArgs la;
-  if (loss_args(weight, focal, gamma, mean, C, &la)) return 1;
-  return SEG_LOSS_DISPATCH(focal, ce_nchw_bwd, logits, target, N, C, H, W, ignore_index, la, accum, gscale, dlogits, ST(stream));
+  if (loss_args(weight, kind, gamma, mean, C, &la)) return 1;
+  return SEG_LOSS_DISPATCH(kind, ce_nchw_bwd, logits, target, N, C, H, W, ignore_index, la, accum, gscale, dlogits, ST(stream));
 }
 int seg_dice_nchw_fwd(const float* logits, const int64_t* target, int N, int C, int H, int W, float smooth, double* accum,
                       float* loss, void* stream) {
@@ -553,59 +550,27 @@ int seg_dice_nchw_bwd(const float* logits, const int64_t* target, int N, int C, 
   dice_nchw_bwd_kernel<<<blocks, 256, 0, ST(stream)>>>(logits, target, N, C, H, W, accum, smooth, gscale, dlogits, beta);
   return check_launch("dice_nchw_bwd");
 }
-int seg_ce_finalize(const double* accum, float* loss, void* stream) {
-  ce_finalize_kernel<<<1, 32, 0, ST(stream)>>>(accum, loss);
-  return check_launch("ce_finalize");
-}
 int seg_loss_finalize(const double* accum, int mean, float* loss, void* stream) {
   loss_finalize_kernel<<<1, 32, 0, ST(stream)>>>(accum, mean, loss);
   return check_launch("loss_finalize");
 }
 
-int seg_upsample_ce_fwd(const float* logits_lo, const int64_t* target, int N, int Hi, int Wi, int Ho, int Wo, int C,
-                        int align_corners, int64_t ignore_index, double* accum, int32_t* argmax, void* stream) {
-  return upsample_ce_fwd<LOSS_CE>(logits_lo, target, N, Hi, Wi, Ho, Wo, C, align_corners, ignore_index, LossArgs{}, accum,
-                                  argmax, nullptr, ST(stream));
-}
-int seg_upsample_ce_fwd_metrics(const float* logits_lo, const int64_t* target, int N, int Hi, int Wi, int Ho, int Wo, int C,
-                                int align_corners, int64_t ignore_index, double* accum, int32_t* argmax, int64_t* counters,
-                                void* stream) {
-  return upsample_ce_fwd<LOSS_CE, true>(logits_lo, target, N, Hi, Wi, Ho, Wo, C, align_corners, ignore_index, LossArgs{},
-                                        accum, argmax, counters, ST(stream));
-}
 int seg_upsample_loss_fwd(const float* logits_lo, const int64_t* target, int N, int Hi, int Wi, int Ho, int Wo, int C,
-                          int align_corners, int64_t ignore_index, const float* weight, int focal, float gamma, double* accum,
-                          int32_t* argmax, void* stream) {
+                          int align_corners, int64_t ignore_index, const float* weight, int kind, float gamma, double* accum,
+                          int32_t* argmax, int64_t* counters, void* stream) {
   LossArgs la;
-  if (loss_args(weight, focal, gamma, 1, C, &la)) return 1;
-  return SEG_LOSS_DISPATCH(focal, upsample_ce_fwd, logits_lo, target, N, Hi, Wi, Ho, Wo, C, align_corners, ignore_index, la, accum,
-                           argmax, nullptr, ST(stream));
+  if (loss_args(weight, kind, gamma, 1, C, &la)) return 1;
+  return SEG_LOSS_DISPATCH(kind, upsample_ce_fwd, logits_lo, target, N, Hi, Wi, Ho, Wo, C, align_corners, ignore_index, la, accum,
+                           argmax, counters, ST(stream));
 }
-int seg_upsample_loss_fwd_metrics(const float* logits_lo, const int64_t* target, int N, int Hi, int Wi, int Ho, int Wo, int C,
-                                  int align_corners, int64_t ignore_index, const float* weight, int focal, float gamma,
-                                  double* accum, int32_t* argmax, int64_t* counters, void* stream) {
-  LossArgs la;
-  if (loss_args(weight, focal, gamma, 1, C, &la)) return 1;
-  return focal ? upsample_ce_fwd<LOSS_FOCAL, true>(logits_lo, target, N, Hi, Wi, Ho, Wo, C, align_corners, ignore_index, la,
-                                                   accum, argmax, counters, ST(stream))
-               : upsample_ce_fwd<LOSS_WCE, true>(logits_lo, target, N, Hi, Wi, Ho, Wo, C, align_corners, ignore_index, la,
-                                                 accum, argmax, counters, ST(stream));
-}
-
 // dlo_f32: fp32 [N,Hi,Wi,C]; dlo_fixed: int64 scratch [N,Hi,Wi,C] (zeroed here); dx: bf16 [N*Hi*Wi][lddx] or NULL
-int seg_upsample_ce_bwd(const float* logits_lo, const int64_t* target, int N, int Hi, int Wi, int Ho, int Wo, int C,
-                        int align_corners, int64_t ignore_index, const double* accum, const float* gscale,
-                        float* dlo_f32, void* dlo_fixed, void* dx, int lddx, void* stream) {
-  return upsample_ce_bwd<LOSS_CE>(logits_lo, target, N, Hi, Wi, Ho, Wo, C, align_corners, ignore_index, LossArgs{}, accum,
-                                  gscale, dlo_f32, dlo_fixed, dx, lddx, ST(stream));
-}
 int seg_upsample_loss_bwd(const float* logits_lo, const int64_t* target, int N, int Hi, int Wi, int Ho, int Wo, int C,
-                          int align_corners, int64_t ignore_index, const float* weight, int focal, float gamma, int mean,
+                          int align_corners, int64_t ignore_index, const float* weight, int kind, float gamma, int mean,
                           const double* accum, const float* gscale, float* dlo_f32, void* dlo_fixed, void* dx, int lddx,
                           void* stream) {
   LossArgs la;
-  if (loss_args(weight, focal, gamma, mean, C, &la)) return 1;
-  return SEG_LOSS_DISPATCH(focal, upsample_ce_bwd, logits_lo, target, N, Hi, Wi, Ho, Wo, C, align_corners, ignore_index, la, accum,
+  if (loss_args(weight, kind, gamma, mean, C, &la)) return 1;
+  return SEG_LOSS_DISPATCH(kind, upsample_ce_bwd, logits_lo, target, N, Hi, Wi, Ho, Wo, C, align_corners, ignore_index, la, accum,
                            gscale, dlo_f32, dlo_fixed, dx, lddx, ST(stream));
 }
 

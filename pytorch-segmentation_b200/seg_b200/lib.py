@@ -15,6 +15,7 @@ LIB_PATH = os.path.join(os.path.dirname(_HERE), "libseg_b200.so")
 
 DT_BF16, DT_F32 = 0, 1
 IMPL_AUTO, IMPL_SIMT, IMPL_TC = 0, 1, 2
+LOSS_CE, LOSS_WCE, LOSS_FOCAL = 0, 1, 2  # SEG_LOSS_* (the `kind` of the seg_loss_* / seg_upsample_loss_* entry points)
 
 
 class SyncDesc(Structure):
@@ -83,24 +84,17 @@ _SIGS = {
     "seg_bilinear_bwd": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "seg_bilinear_logits_fwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "seg_bilinear_logits_bwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
-    "seg_ce_nchw_fwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int64, c_void_p, c_void_p]),
-    "seg_ce_nchw_bwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int64, c_void_p, c_void_p, c_void_p, c_void_p]),
     "seg_dice_nchw_fwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p]),
     "seg_dice_nchw_bwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_float, c_void_p, c_void_p, c_float, c_void_p]),
     "seg_lovasz_count": (c_int, [c_void_p, c_int64, c_int, c_int64, c_void_p, c_void_p]),
     "seg_lovasz_workspace_bytes": (c_int64, [c_int64, c_int, c_int]),
     "seg_lovasz_softmax_nchw": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int64, c_void_p, c_int64, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "seg_eval_metrics_nchw": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
-    "seg_ce_finalize": (c_int, [c_void_p, c_void_p, c_void_p]),
-    "seg_upsample_ce_fwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int64, c_void_p, c_void_p, c_void_p]),
-    "seg_upsample_ce_bwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
     "seg_loss_nchw_fwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int64, c_void_p, c_int, c_float, c_void_p, c_void_p]),
     "seg_loss_nchw_bwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int64, c_void_p, c_int, c_float, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "seg_loss_finalize": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
-    "seg_upsample_loss_fwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int64, c_void_p, c_int, c_float, c_void_p, c_void_p, c_void_p]),
+    "seg_upsample_loss_fwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int64, c_void_p, c_int, c_float, c_void_p, c_void_p, c_void_p, c_void_p]),
     "seg_upsample_loss_bwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int64, c_void_p, c_int, c_float, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
-    "seg_upsample_ce_fwd_metrics": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int64, c_void_p, c_void_p, c_void_p, c_void_p]),
-    "seg_upsample_loss_fwd_metrics": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int64, c_void_p, c_int, c_float, c_void_p, c_void_p, c_void_p, c_void_p]),
     "seg_relu_fwd": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int64, c_int, c_void_p]),
     "seg_relu_bwd": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int64, c_int, c_float, c_void_p]),
     "seg_nhwc_to_nchw_f32": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),

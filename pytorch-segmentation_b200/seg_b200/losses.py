@@ -7,7 +7,8 @@
     LovaszSoftmax(classes='present', per_image=False, ignore_index=255)   — utils/losses.py:79-89
 
 forward(output fp32 [B,C,H,W], target int64 [B,H,W]) -> 0-dim tensor with autograd, computed by the sm_90a kernels
-(`seg_ce_nchw_fwd/bwd`, `seg_loss_nchw_fwd/bwd` for class weights, 'sum' and focal); `.item()` works as the trainer expects (trainer.py:72,81).  CUDA tensors only.
+(`seg_loss_nchw_fwd/bwd` for cross-entropy, class-weighted CE and focal, `seg_dice_nchw_*`, `seg_lovasz_*`); `.item()` works
+as the trainer expects (trainer.py:72,81).  CUDA tensors only.
 """
 import torch
 import torch.nn as nn
@@ -21,8 +22,9 @@ def _dp_world():
 
 
 class LossSpec:
-    """A class-weighted cross-entropy (gamma None) or focal loss (gamma >= 0): the class weights (float64 CPU tensor or
-    None = all ones), gamma, and whether the loss is a mean (else a sum).  Shared by the plugin path and FusedTrainStep."""
+    """A cross-entropy (gamma None) or focal loss (gamma >= 0): the class weights (float64 CPU tensor or None = all ones),
+    gamma, and whether the loss is a mean (else a sum); ops._loss_kind picks the kernels.  Shared by the plugin path and
+    FusedTrainStep."""
 
     def __init__(self, weight, gamma, mean):
         self.weight, self.gamma, self.mean = weight, gamma, mean
@@ -66,8 +68,8 @@ class _CEFn(torch.autograd.Function):
     that is (sum over ranks of the loss sums) / (sum over ranks of the valid-pixel counts): the (sum, count) pair is
     all-reduced — 16 bytes — so every rank reports the global loss and its gradient carries the global normalisation
     (times world: the engine's gradient exchange averages over ranks).  `global_mean=False` keeps per-rank means.
-    spec (LossSpec): a class-weighted or focal loss instead; its (sum, denominator) pair is all-reduced the same way, and a
-    'sum' is the global sum."""
+    spec (LossSpec, None = unweighted mean CE): a class-weighted or focal loss instead; its (sum, denominator) pair is
+    all-reduced the same way, and a 'sum' is the global sum."""
 
     @staticmethod
     def forward(ctx, logits, target, ignore_index, global_mean=True, spec=None):
@@ -78,11 +80,9 @@ class _CEFn(torch.autograd.Function):
         if world > 1:
             def reduce_fn(accum):
                 torch.distributed.all_reduce(accum)
-        if spec is None:
-            loss, accum = ops.ce_nchw_fwd(logits, target, ignore_index, reduce_fn=reduce_fn)
-        else:
-            loss, accum = ops.loss_nchw_fwd(logits, target, ignore_index, spec.weight_on(logits.device, logits.shape[1]),
-                                            spec.gamma, spec.mean, reduce_fn=reduce_fn)
+        spec = LossSpec(None, None, True) if spec is None else spec
+        loss, accum = ops.loss_nchw_fwd(logits, target, ignore_index, spec.weight_on(logits.device, logits.shape[1]),
+                                        spec.gamma, spec.mean, reduce_fn=reduce_fn)
         ctx.save_for_backward(logits, target, accum)
         ctx.ignore_index, ctx.world, ctx.spec = ignore_index, world, spec
         return loss
@@ -94,11 +94,8 @@ class _CEFn(torch.autograd.Function):
         if ctx.world > 1:
             g = g * float(ctx.world)
         spec = ctx.spec
-        if spec is None:
-            dl = ops.ce_nchw_bwd(logits, target, ctx.ignore_index, accum, gscale=g)
-        else:
-            dl = ops.loss_nchw_bwd(logits, target, ctx.ignore_index, accum, spec.weight_on(logits.device, logits.shape[1]),
-                                   spec.gamma, spec.mean, gscale=g)
+        dl = ops.loss_nchw_bwd(logits, target, ctx.ignore_index, accum, spec.weight_on(logits.device, logits.shape[1]),
+                               spec.gamma, spec.mean, gscale=g)
         return (dl,) + (None,) * (len(ctx.needs_input_grad) - 1)
 
 
@@ -112,8 +109,7 @@ class CrossEntropyLoss2d(nn.Module):
         w = _class_weight(weight)
         self.ignore_index = ignore_index
         self.reduction = reduction
-        # unweighted mean CE runs the dedicated kernels (spec None)
-        self.spec = None if (w is None and mean) else LossSpec(w, None, mean)
+        self.spec = LossSpec(w, None, mean)
 
     def forward(self, output, target):
         if not output.is_cuda:

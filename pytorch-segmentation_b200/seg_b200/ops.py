@@ -438,35 +438,23 @@ def bilinear_logits_bwd(dy_nchw, Hi, Wi, align_corners, ldx):
 
 
 # ---------------------------------------------------------------- loss
-def ce_nchw_fwd(logits, target, ignore_index, reduce_fn=None):
-    """reduce_fn(accum): optional in-place cross-rank sum of the fp64 (loss sum, valid-pixel count) pair before the mean."""
-    N, C, H, W = logits.shape
-    assert logits.is_contiguous() and logits.dtype == torch.float32 and target.dtype == torch.int64 and target.is_contiguous()
-    accum = torch.zeros(2, dtype=torch.float64, device=logits.device)
-    call("seg_ce_nchw_fwd", ptr(logits), ptr(target), N, C, H, W, int(ignore_index), ptr(accum))
-    if reduce_fn is not None:
-        reduce_fn(accum)
-    loss = torch.empty((), dtype=torch.float32, device=logits.device)
-    call("seg_ce_finalize", ptr(accum), ptr(loss))
-    return loss, accum
-
-
-def ce_nchw_bwd(logits, target, ignore_index, accum, gscale=None):
-    N, C, H, W = logits.shape
-    dl = torch.empty_like(logits)
-    call("seg_ce_nchw_bwd", ptr(logits), ptr(target), N, C, H, W, int(ignore_index), ptr(accum), ptr(gscale), ptr(dl))
-    return dl
+def _loss_kind(weight, gamma, mean):
+    """SEG_LOSS_* of a per-pixel loss: focal when gamma is given; else unweighted cross-entropy for a mean without class
+    weights; else class-weighted cross-entropy (weight None = all ones)."""
+    if gamma is not None:
+        return lib.LOSS_FOCAL
+    return lib.LOSS_CE if weight is None and mean else lib.LOSS_WCE
 
 
 def loss_nchw_fwd(logits, target, ignore_index, weight=None, gamma=None, mean=True, reduce_fn=None):
-    """Class-weighted CE (gamma None) or focal loss (gamma >= 0), weight: fp32 [C] device tensor or None (all ones).
-    Returns (loss, accum); accum = fp64 (per-pixel loss sum, denominator), reduce_fn(accum) as in ce_nchw_fwd.  mean=False:
-    the loss is the (globally reduced) sum."""
+    """Cross-entropy, class-weighted CE or focal loss (gamma >= 0) on NCHW fp32 logits; weight: fp32 [C] device tensor or
+    None.  Returns (loss, accum); accum = fp64 (per-pixel loss sum, denominator).  reduce_fn(accum): optional in-place
+    cross-rank sum of accum before the loss is formed.  mean=False: the loss is the (globally reduced) sum."""
     N, C, H, W = logits.shape
     assert logits.is_contiguous() and logits.dtype == torch.float32 and target.dtype == torch.int64 and target.is_contiguous()
     assert weight is None or (weight.dtype == torch.float32 and weight.numel() == C and weight.is_contiguous())
     accum = torch.zeros(2, dtype=torch.float64, device=logits.device)
-    call("seg_loss_nchw_fwd", ptr(logits), ptr(target), N, C, H, W, int(ignore_index), ptr(weight), int(gamma is not None),
+    call("seg_loss_nchw_fwd", ptr(logits), ptr(target), N, C, H, W, int(ignore_index), ptr(weight), _loss_kind(weight, gamma, mean),
          float(gamma or 0.0), ptr(accum))
     if reduce_fn is not None:
         reduce_fn(accum)
@@ -478,7 +466,7 @@ def loss_nchw_fwd(logits, target, ignore_index, weight=None, gamma=None, mean=Tr
 def loss_nchw_bwd(logits, target, ignore_index, accum, weight=None, gamma=None, mean=True, gscale=None):
     N, C, H, W = logits.shape
     dl = torch.empty_like(logits)
-    call("seg_loss_nchw_bwd", ptr(logits), ptr(target), N, C, H, W, int(ignore_index), ptr(weight), int(gamma is not None),
+    call("seg_loss_nchw_bwd", ptr(logits), ptr(target), N, C, H, W, int(ignore_index), ptr(weight), _loss_kind(weight, gamma, mean),
          float(gamma or 0.0), int(mean), ptr(accum), ptr(gscale), ptr(dl))
     return dl
 
@@ -534,55 +522,21 @@ def _check_counters(counters, C):
     assert counters.dtype == torch.int64 and counters.is_contiguous() and counters.numel() == 2 + 3 * C
 
 
-def upsample_ce_fwd(logits_lo, target, align_corners, ignore_index, want_argmax=False, reduce_fn=None, counters=None):
-    """counters: None, or an int64 device vector [2 + 3C] that the same launch ADDS the batch's eval_metrics counters to
-    (the layout of eval_metrics_nchw with num_class = C)."""
-    N, Hi, Wi, C = logits_lo.shape
-    _, Ho, Wo = target.shape
-    assert logits_lo.is_contiguous() and logits_lo.dtype == torch.float32 and target.is_contiguous()
-    accum = torch.zeros(2, dtype=torch.float64, device=logits_lo.device)
-    am = torch.empty((N, Ho, Wo), dtype=torch.int32, device=logits_lo.device) if want_argmax else None
-    if counters is None:
-        call("seg_upsample_ce_fwd", ptr(logits_lo), ptr(target), N, Hi, Wi, Ho, Wo, C, int(align_corners), int(ignore_index),
-             ptr(accum), ptr(am))
-    else:
-        _check_counters(counters, C)
-        call("seg_upsample_ce_fwd_metrics", ptr(logits_lo), ptr(target), N, Hi, Wi, Ho, Wo, C, int(align_corners),
-             int(ignore_index), ptr(accum), ptr(am), ptr(counters))
-    if reduce_fn is not None:  # cross-rank sum of the fp64 (loss sum, valid-pixel count) pair: global-batch mean
-        reduce_fn(accum)
-    loss = torch.empty((), dtype=torch.float32, device=logits_lo.device)
-    call("seg_ce_finalize", ptr(accum), ptr(loss))
-    return loss, accum, am
-
-
-def upsample_ce_bwd(logits_lo, target, align_corners, ignore_index, accum, ldx, gscale=None):
-    N, Hi, Wi, C = logits_lo.shape
-    _, Ho, Wo = target.shape
-    dlo = torch.empty((N, Hi, Wi, C), dtype=torch.float32, device=logits_lo.device)
-    fixed = torch.empty((N, Hi, Wi, C), dtype=torch.int64, device=logits_lo.device)
-    dx = torch.empty((N, Hi, Wi, ldx), dtype=torch.bfloat16, device=logits_lo.device)
-    call("seg_upsample_ce_bwd", ptr(logits_lo), ptr(target), N, Hi, Wi, Ho, Wo, C, int(align_corners), int(ignore_index),
-         ptr(accum), ptr(gscale), ptr(dlo), ptr(fixed), ptr(dx), ldx)
-    return dx, dlo
-
-
 def upsample_loss_fwd(logits_lo, target, align_corners, ignore_index, weight=None, gamma=None, mean=True, want_argmax=False,
                       reduce_fn=None, counters=None):
-    """upsample_ce_fwd for the class-weighted CE (gamma None) and focal (gamma >= 0) losses of loss_nchw_fwd."""
+    """loss_nchw_fwd fused with the bilinear upsample of the low-res NHWC fp32 logits; returns (loss, accum, argmax map or
+    None).  counters: None, or an int64 device vector [2 + 3C] that the same launch ADDS the batch's eval_metrics counters
+    to (the layout of eval_metrics_nchw with num_class = C)."""
     N, Hi, Wi, C = logits_lo.shape
     _, Ho, Wo = target.shape
     assert logits_lo.is_contiguous() and logits_lo.dtype == torch.float32 and target.is_contiguous()
     assert weight is None or (weight.dtype == torch.float32 and weight.numel() == C and weight.is_contiguous())
+    if counters is not None:
+        _check_counters(counters, C)
     accum = torch.zeros(2, dtype=torch.float64, device=logits_lo.device)
     am = torch.empty((N, Ho, Wo), dtype=torch.int32, device=logits_lo.device) if want_argmax else None
-    if counters is None:
-        call("seg_upsample_loss_fwd", ptr(logits_lo), ptr(target), N, Hi, Wi, Ho, Wo, C, int(align_corners), int(ignore_index),
-             ptr(weight), int(gamma is not None), float(gamma or 0.0), ptr(accum), ptr(am))
-    else:
-        _check_counters(counters, C)
-        call("seg_upsample_loss_fwd_metrics", ptr(logits_lo), ptr(target), N, Hi, Wi, Ho, Wo, C, int(align_corners),
-             int(ignore_index), ptr(weight), int(gamma is not None), float(gamma or 0.0), ptr(accum), ptr(am), ptr(counters))
+    call("seg_upsample_loss_fwd", ptr(logits_lo), ptr(target), N, Hi, Wi, Ho, Wo, C, int(align_corners), int(ignore_index),
+         ptr(weight), _loss_kind(weight, gamma, mean), float(gamma or 0.0), ptr(accum), ptr(am), ptr(counters))
     if reduce_fn is not None:
         reduce_fn(accum)
     loss = torch.empty((), dtype=torch.float32, device=logits_lo.device)
@@ -598,8 +552,8 @@ def upsample_loss_bwd(logits_lo, target, align_corners, ignore_index, accum, ldx
     fixed = torch.empty((N, Hi, Wi, C), dtype=torch.int64, device=logits_lo.device)
     dx = torch.empty((N, Hi, Wi, ldx), dtype=torch.bfloat16, device=logits_lo.device)
     call("seg_upsample_loss_bwd", ptr(logits_lo), ptr(target), N, Hi, Wi, Ho, Wo, C, int(align_corners), int(ignore_index),
-         ptr(weight), int(gamma is not None), float(gamma or 0.0), int(mean), ptr(accum), ptr(gscale), ptr(dlo), ptr(fixed),
-         ptr(dx), ldx)
+         ptr(weight), _loss_kind(weight, gamma, mean), float(gamma or 0.0), int(mean), ptr(accum), ptr(gscale), ptr(dlo),
+         ptr(fixed), ptr(dx), ldx)
     return dx, dlo
 
 

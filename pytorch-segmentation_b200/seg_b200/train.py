@@ -89,10 +89,10 @@ class WeightTables:
 
 
 def _loss_spec(loss, ignore_index):
-    """(ignore_index, LossSpec or None) for FusedTrainStep's `loss`: None and unweighted mean CE run the unweighted kernels."""
+    """(ignore_index, LossSpec) for FusedTrainStep's `loss`; None is the unweighted mean cross-entropy."""
     from . import losses
     if loss is None:
-        return (255 if ignore_index is None else ignore_index), None
+        return (255 if ignore_index is None else ignore_index), losses.LossSpec(None, None, True)
     if type(loss) not in (losses.CrossEntropyLoss2d, losses.FocalLoss):
         raise NotImplementedError(
             f"FusedTrainStep fuses seg_b200.CrossEntropyLoss2d and seg_b200.FocalLoss only, not {type(loss).__name__}; "
@@ -293,9 +293,6 @@ class FusedTrainStep:
         all-reduced (16 bytes); a 'sum' is the global sum."""
         rf = (lambda acc: dist.all_reduce(acc)) if self.world > 1 else None
         spec = self.loss_spec
-        if spec is None:
-            loss, accum, _ = ops.upsample_ce_fwd(lo_t, target, ac, self.ignore_index, reduce_fn=rf, counters=counters)
-            return loss, accum, None
         cw = spec.weight_on(lo_t.device, lo_t.shape[-1])
         loss, accum, _ = ops.upsample_loss_fwd(lo_t, target, ac, self.ignore_index, cw, spec.gamma, spec.mean, reduce_fn=rf,
                                                counters=counters)
@@ -393,11 +390,8 @@ class FusedTrainStep:
             w = 1.0 if i == 0 else self.aux_weight
             wg = w * self.world
             g = None if wg == 1.0 else torch.full((1,), wg, dtype=torch.float32, device=lo.t.device)
-            if spec is None:
-                dx, _ = ops.upsample_ce_bwd(lo.t, target, ac, self.ignore_index, accum, (C + 7) // 8 * 8, gscale=g)
-            else:
-                dx, _ = ops.upsample_loss_bwd(lo.t, target, ac, self.ignore_index, accum, (C + 7) // 8 * 8, cw, spec.gamma,
-                                              spec.mean, gscale=g)
+            dx, _ = ops.upsample_loss_bwd(lo.t, target, ac, self.ignore_index, accum, (C + 7) // 8 * 8, cw, spec.gamma, spec.mean,
+                                          gscale=g)
             lo.grad = dx[..., :C]
             total = loss if total is None else total + w * loss
         m._finish(tape)

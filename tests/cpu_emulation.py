@@ -320,7 +320,13 @@ def bilinear_logits_bwd(dy, Hi, Wi, align_corners, ldx):
     return out
 
 
-def ce_nchw_fwd(logits, target, ignore_index, reduce_fn=None):
+def _unweighted_mean_ce_only(weight, gamma, mean):
+    if weight is not None or gamma is not None or not mean:
+        raise NotImplementedError("the emulation restates the unweighted mean cross-entropy only")
+
+
+def loss_nchw_fwd(logits, target, ignore_index, weight=None, gamma=None, mean=True, reduce_fn=None):
+    _unweighted_mean_ce_only(weight, gamma, mean)
     valid = target != ignore_index
     loss_sum = F.cross_entropy(logits, target, ignore_index=ignore_index, reduction="sum")
     accum = torch.tensor([loss_sum.item(), float(valid.sum())], dtype=torch.float64)
@@ -329,8 +335,9 @@ def ce_nchw_fwd(logits, target, ignore_index, reduce_fn=None):
     return (accum[0] / accum[1].clamp(min=1)).float(), accum
 
 
-def ce_nchw_bwd(logits, target, ignore_index, accum, gscale=None):
+def loss_nchw_bwd(logits, target, ignore_index, accum, weight=None, gamma=None, mean=True, gscale=None):
     """d(loss sum)/d(logits) / accum.count  (the count may be the cross-rank total)"""
+    _unweighted_mean_ce_only(weight, gamma, mean)
     with torch.enable_grad():
         l = logits.detach().clone().requires_grad_(True)
         F.cross_entropy(l, target, ignore_index=ignore_index, reduction="sum").backward()

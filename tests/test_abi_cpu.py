@@ -28,8 +28,8 @@ def cdll():
 def test_header_declares_entry_points():
     syms = declared_symbols()
     assert len(syms) >= 30
-    for must in ("seg_conv2d_fwd", "seg_conv2d_dgrad", "seg_conv2d_wgrad", "seg_bn_finalize", "seg_upsample_ce_fwd",
-                 "seg_last_error"):
+    for must in ("seg_conv2d_fwd", "seg_conv2d_dgrad", "seg_conv2d_wgrad", "seg_bn_finalize", "seg_upsample_loss_fwd",
+                 "seg_loss_nchw_fwd", "seg_last_error"):
         assert must in syms
 
 

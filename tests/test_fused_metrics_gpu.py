@@ -1,4 +1,4 @@
-"""Pixel accuracy / mIoU counters from the fused upsample + loss forward (seg_upsample_*_fwd_metrics), the training
+"""Pixel accuracy / mIoU counters from the fused upsample + loss forward (seg_upsample_loss_fwd with counters), the training
 metrics of FusedTrainStep(metrics=True) and its validation pass FusedTrainStep.evaluate, on the H100.
 
 The reference for the counters is the plugin path bit for bit: seg_eval_metrics_nchw over the full-resolution logits
@@ -31,19 +31,17 @@ def log(gpu_out_dir, msg):
 
 
 def kind_args(kind, C):
-    """(weight, gamma) of the upsample_loss_fwd call for `kind`; None for the unweighted CE entry point."""
+    """(weight, gamma) of the upsample_loss_fwd call for `kind`."""
     if kind == "ce":
-        return None
+        return None, None
     g = torch.Generator().manual_seed(C)
     w = (torch.rand(C, generator=g) * 2 + 0.1).to(DEV)
     return (w, None) if kind == "wce" else (w, 2.0)
 
 
 def fused_fwd(lo, t, ac, ign, kind, counters=None, want_argmax=False):
-    a = kind_args(kind, lo.shape[-1])
-    if a is None:
-        return ops.upsample_ce_fwd(lo, t, ac, ign, want_argmax=want_argmax, counters=counters)
-    return ops.upsample_loss_fwd(lo, t, ac, ign, a[0], a[1], want_argmax=want_argmax, counters=counters)
+    w, gamma = kind_args(kind, lo.shape[-1])
+    return ops.upsample_loss_fwd(lo, t, ac, ign, w, gamma, want_argmax=want_argmax, counters=counters)
 
 
 def plugin_counters(lo, t, ac, C):

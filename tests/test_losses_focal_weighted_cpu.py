@@ -157,16 +157,57 @@ def test_constructors_reject_bad_arguments():
     assert ce.spec is not None and not ce.spec.mean and ce.spec.gamma is None
     with pytest.raises(ValueError):
         ce.spec.weight_on("cpu", 4)
-    assert losses.CrossEntropyLoss2d().spec is None  # unweighted mean CE keeps the dedicated kernels
+    assert _is_plain_ce(losses.CrossEntropyLoss2d().spec)  # unweighted mean CE keeps the dedicated kernels
     f = losses.FocalLoss()
     assert f.spec.gamma == 2.0 and f.spec.mean and f.spec.weight is None and f.ignore_index == 255
+
+
+def _is_plain_ce(spec):
+    """spec is the unweighted mean cross-entropy, and the ops layer runs it on the SEG_LOSS_CE kernels."""
+    from seg_b200 import lib, ops
+    return (spec.weight is None and spec.mean and spec.gamma is None
+            and ops._loss_kind(spec.weight, spec.gamma, spec.mean) == lib.LOSS_CE)
+
+
+def test_specs_select_the_loss_kernels():
+    from seg_b200 import lib, losses, ops
+    header = open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "include", "seg_b200.h")).read()
+    for name in ("CE", "WCE", "FOCAL"):
+        assert f"#define SEG_LOSS_{name} {getattr(lib, 'LOSS_' + name)}\n" in header, name
+    kind = lambda crit: ops._loss_kind(crit.spec.weight, crit.spec.gamma, crit.spec.mean)  # noqa: E731
+    assert kind(losses.CrossEntropyLoss2d()) == lib.LOSS_CE
+    assert kind(losses.CrossEntropyLoss2d(reduction="sum")) == lib.LOSS_WCE
+    assert kind(losses.CrossEntropyLoss2d(weight=[1.0, 2.0])) == lib.LOSS_WCE
+    assert kind(losses.FocalLoss()) == lib.LOSS_FOCAL
+    assert kind(losses.FocalLoss(gamma=0, alpha=[1.0, 2.0], size_average=False)) == lib.LOSS_FOCAL
+
+
+def test_loss_entry_points_reject_bad_kinds():
+    """The C ABI checks `kind` on the host before anything reaches the device (so no GPU is needed here): an unknown kind,
+    SEG_LOSS_CE with a class weight or as a sum, and a negative focal gamma are errors."""
+    from seg_b200 import lib
+    so = lib.load()
+    w = 256  # never dereferenced: the checks reject the call first
+    nchw = (None, None, 1, 4, 1, 1, 255)
+    up = (None, None, 1, 2, 2, 4, 4, 4, 0, 255)
+    calls = [("unknown kind", so.seg_loss_nchw_fwd, nchw + (None, 3, 0.0, None, None)),
+             ("unknown kind", so.seg_upsample_loss_fwd, up + (None, -1, 0.0, None, None, None, None)),
+             ("SEG_LOSS_CE", so.seg_loss_nchw_fwd, nchw + (w, lib.LOSS_CE, 0.0, None, None)),
+             ("SEG_LOSS_CE", so.seg_loss_nchw_bwd, nchw + (None, lib.LOSS_CE, 0.0, 0, None, None, None, None)),
+             ("SEG_LOSS_CE", so.seg_upsample_loss_bwd, up + (w, lib.LOSS_CE, 0.0, 1, None, None, None, None, None, 8, None)),
+             ("gamma", so.seg_upsample_loss_fwd, up + (None, lib.LOSS_FOCAL, -1.0, None, None, None, None))]
+    for what, fn, args in calls:
+        assert fn(*args) != 0, what
+        assert what in lib.last_error(), (what, lib.last_error())
 
 
 def test_fused_train_step_loss_argument_checks():
     from seg_b200 import losses
     from seg_b200.train import _loss_spec
-    assert _loss_spec(None, None) == (255, None)
-    assert _loss_spec(None, 7) == (7, None)
+    ii, spec = _loss_spec(None, None)
+    assert ii == 255 and _is_plain_ce(spec)
+    ii, spec = _loss_spec(None, 7)
+    assert ii == 7 and _is_plain_ce(spec)
     ii, spec = _loss_spec(losses.FocalLoss(ignore_index=-1), None)
     assert ii == -1 and spec.gamma == 2.0
     assert _loss_spec(losses.CrossEntropyLoss2d(ignore_index=3), 3)[0] == 3

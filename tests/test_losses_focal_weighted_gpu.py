@@ -1,4 +1,4 @@
-"""Class-weighted cross-entropy and focal loss on the H100 (seg_loss_nchw_*, seg_upsample_loss_*, seg_b200.FocalLoss,
+"""Cross-entropy, class-weighted cross-entropy and focal loss on the H100 (seg_loss_nchw_*, seg_upsample_loss_*, seg_b200.FocalLoss,
 CrossEntropyLoss2d(weight, reduction), FusedTrainStep(loss=...)) against the float64 oracle on the same inputs
 (oracle/losses_weighted.py: weighted_loss_and_grad, which tests/test_losses_focal_weighted_cpu.py checks against the reference)."""
 import os
@@ -17,7 +17,7 @@ pytestmark = pytest.mark.gpu
 
 if torch.cuda.is_available():
     import seg_b200
-    from seg_b200 import losses, ops
+    from seg_b200 import lib, losses, ops
     from seg_b200.train import FusedTrainStep
 
 DEV = "cuda"
@@ -72,6 +72,21 @@ def engine_nchw(z, t, ign, w, gamma, mean):
     return loss, dl
 
 
+def raw_wce_nchw(z, t, ign):
+    """SEG_LOSS_WCE without class weights, as a mean, through the C ABI: ops runs SEG_LOSS_CE for that combination, so
+    this keeps the unit-weight path of the weighted kernels compared with the oracle."""
+    zd, td = z.contiguous().to(DEV), t.to(DEV)
+    N, C, H, W = zd.shape
+    accum = torch.zeros(2, dtype=torch.float64, device=DEV)
+    loss = torch.empty((), dtype=torch.float32, device=DEV)
+    dl = torch.empty_like(zd)
+    lib.call("seg_loss_nchw_fwd", zd.data_ptr(), td.data_ptr(), N, C, H, W, ign, None, lib.LOSS_WCE, 0.0, accum.data_ptr())
+    lib.call("seg_loss_finalize", accum.data_ptr(), 1, loss.data_ptr())
+    lib.call("seg_loss_nchw_bwd", zd.data_ptr(), td.data_ptr(), N, C, H, W, ign, None, lib.LOSS_WCE, 0.0, 1, accum.data_ptr(),
+             None, dl.data_ptr())
+    return loss, dl
+
+
 NCHW_CASES = [(C, ign, gm, use_w, mean, "none") for C, ign in CLASSES for gm in GAMMAS for use_w in (False, True)
               for mean in (True, False)]
 NCHW_CASES += [(19, 255, gm, use_w, mean, sp) for sp in ("img_ignored", "all_ignored", "zero_weight", "saturated")
@@ -82,19 +97,22 @@ NCHW_CASES += [(19, 255, gm, use_w, mean, sp) for sp in ("img_ignored", "all_ign
 def test_nchw_matches_oracle(C, ign, gamma, use_w, mean, special, gpu_out_dir):
     z, t, w = nchw_inputs(C, ign, special)
     w = w if use_w else None
-    loss, dl = engine_nchw(z, t, ign, w, gamma, mean)
     ref_l, ref_g = olw.weighted_loss_and_grad(z, t, ign, None if w is None else w.double(), gamma, mean)
-    tag = f"nchw C={C} gamma={gamma} w={use_w} mean={mean} {special}"
-    assert torch.isfinite(dl).all(), tag
-    if float(ref_l) == 0.0 and float(ref_g.abs().max()) == 0.0:  # nothing valid / only zero-weight classes
-        assert float(loss) == 0.0 and float(dl.abs().max()) == 0.0, tag
-        log(gpu_out_dir, f"{tag}: loss 0, gradient 0")
-        return
-    el, eg = abs(float(loss) - float(ref_l)) / abs(float(ref_l)), rel(dl, ref_g)
-    log(gpu_out_dir, f"{tag}: loss rel {el:.2e}, grad {eg:.2e}")
-    assert el <= 1e-5 and eg <= 1e-4, tag
-    if special == "saturated" and gamma is not None and gamma > 0:  # the finite limit, where the reference gives NaN
-        assert float(dl.cpu()[:, :, 5:9, :].abs().max()) == 0.0, tag
+    runs = [("", engine_nchw(z, t, ign, w, gamma, mean))]
+    if w is None and gamma is None and mean:
+        runs.append((" SEG_LOSS_WCE", raw_wce_nchw(z, t, ign)))
+    for suffix, (loss, dl) in runs:
+        tag = f"nchw C={C} gamma={gamma} w={use_w} mean={mean} {special}{suffix}"
+        assert torch.isfinite(dl).all(), tag
+        if float(ref_l) == 0.0 and float(ref_g.abs().max()) == 0.0:  # nothing valid / only zero-weight classes
+            assert float(loss) == 0.0 and float(dl.abs().max()) == 0.0, tag
+            log(gpu_out_dir, f"{tag}: loss 0, gradient 0")
+            continue
+        el, eg = abs(float(loss) - float(ref_l)) / abs(float(ref_l)), rel(dl, ref_g)
+        log(gpu_out_dir, f"{tag}: loss rel {el:.2e}, grad {eg:.2e}")
+        assert el <= 1e-5 and eg <= 1e-4, tag
+        if special == "saturated" and gamma is not None and gamma > 0:  # the finite limit, where the reference gives NaN
+            assert float(dl.cpu()[:, :, 5:9, :].abs().max()) == 0.0, tag
 
 
 @pytest.mark.parametrize("C,ign", CLASSES)

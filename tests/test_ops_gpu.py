@@ -365,9 +365,9 @@ def test_cross_entropy(C, ignore, gpu_out_dir):
     loss = F.cross_entropy(logits, target, ignore_index=ignore)
     loss.backward()
     ld, td = logits.detach().to(DEV), target.to(DEV)
-    l, accum = ops.ce_nchw_fwd(ld, td, ignore)
+    l, accum = ops.loss_nchw_fwd(ld, td, ignore)
     check(f"ce_fwd C={C}", l, loss, 1e-5, gpu_out_dir)
-    dl = ops.ce_nchw_bwd(ld, td, ignore, accum)
+    dl = ops.loss_nchw_bwd(ld, td, ignore, accum)
     check(f"ce_bwd C={C}", dl, logits.grad, 1e-4, gpu_out_dir)
 
 
@@ -383,13 +383,13 @@ def test_fused_upsample_ce(C, ignore, ac, gpu_out_dir):
     loss = F.cross_entropy(full, target, ignore_index=ignore)
     loss.backward()
     lod = lo.detach().permute(0, 2, 3, 1).contiguous().to(DEV)
-    l, accum, am = ops.upsample_ce_fwd(lod, target.to(DEV), ac, ignore, want_argmax=True)
+    l, accum, am = ops.upsample_loss_fwd(lod, target.to(DEV), ac, ignore, want_argmax=True)
     check(f"fused_ce_fwd C={C} ac={ac}", l, loss, 1e-5, gpu_out_dir)
     ref_am = full.detach().argmax(1)
     mism = (am.cpu().long() != ref_am).float().mean().item()
     assert mism < 1e-4, f"argmax mismatch fraction {mism}"
     ldx = (C + 7) // 8 * 8
-    dx, dlo = ops.upsample_ce_bwd(lod, target.to(DEV), ac, ignore, accum, ldx)
+    dx, dlo = ops.upsample_loss_bwd(lod, target.to(DEV), ac, ignore, accum, ldx)
     check(f"fused_ce_bwd C={C} ac={ac}", dlo.permute(0, 3, 1, 2), lo.grad, 1e-4, gpu_out_dir)
     check(f"fused_ce_bwd_bf16 C={C} ac={ac}", dx[..., :C].permute(0, 3, 1, 2), lo.grad, 1e-2, gpu_out_dir)
 

@@ -1,8 +1,8 @@
 """Times the per-pixel losses on the GPU with CUDA events: unweighted CE, class-weighted CE and focal loss (gamma 2, with
 class weights), forward + backward, on both paths:
-  * fused: bilinear upsample + loss from the low-resolution NHWC fp32 logits (seg_upsample_ce_* / seg_upsample_loss_*),
-    as FusedTrainStep runs it;
-  * nchw: the loss on full-resolution NCHW fp32 logits (seg_ce_nchw_* / seg_loss_nchw_*), as the plugin surface runs it.
+  * fused: bilinear upsample + loss from the low-resolution NHWC fp32 logits (seg_upsample_loss_*), as FusedTrainStep
+    runs it;
+  * nchw: the loss on full-resolution NCHW fp32 logits (seg_loss_nchw_*), as the plugin surface runs it.
 Shapes: C3 (19 classes, 129x129 -> 513x513, batch 16) and C5 (150 classes, 128x128 -> 512x512, batch 8).
 
     python tools/loss_timing.py [--iters 50] [--rounds 5] [--out FILE]
@@ -72,25 +72,16 @@ def main():
         w = torch.rand(C, device="cuda", generator=g) + 0.5
         ldx = (C + 7) // 8 * 8
         full = torch.randn(N, C, Ho, Ho, device="cuda", generator=g) * 3
-        variants = {"ce": None, "weighted_ce": (w, None), "focal_g2_weighted": (w, 2.0)}
+        variants = {"ce": (None, None), "weighted_ce": (w, None), "focal_g2_weighted": (w, 2.0)}
         fns = {}
         for vname, v in variants.items():
-            if v is None:
-                def fused():
-                    _, acc, _ = ops.upsample_ce_fwd(lo, target, ac, ign)
-                    ops.upsample_ce_bwd(lo, target, ac, ign, acc, ldx)
+            def fused(v=v):
+                _, acc, _ = ops.upsample_loss_fwd(lo, target, ac, ign, v[0], v[1])
+                ops.upsample_loss_bwd(lo, target, ac, ign, acc, ldx, v[0], v[1])
 
-                def nchw():
-                    _, acc = ops.ce_nchw_fwd(full, target, ign)
-                    ops.ce_nchw_bwd(full, target, ign, acc)
-            else:
-                def fused(v=v):
-                    _, acc, _ = ops.upsample_loss_fwd(lo, target, ac, ign, v[0], v[1])
-                    ops.upsample_loss_bwd(lo, target, ac, ign, acc, ldx, v[0], v[1])
-
-                def nchw(v=v):
-                    _, acc = ops.loss_nchw_fwd(full, target, ign, v[0], v[1])
-                    ops.loss_nchw_bwd(full, target, ign, acc, v[0], v[1])
+            def nchw(v=v):
+                _, acc = ops.loss_nchw_fwd(full, target, ign, v[0], v[1])
+                ops.loss_nchw_bwd(full, target, ign, acc, v[0], v[1])
             fns[("fused", vname)], fns[("nchw", vname)] = fused, nchw
         times = {k: [] for k in fns}
         for _ in range(a.rounds):
