@@ -47,15 +47,14 @@ typedef struct seg_conv_desc {
 } seg_conv_desc;
 
 /* SyncBN exchange handle (seg_comm_*): device array of every rank's symmetric-buffer pointer + this rank.  Passed to the
- * kernels that produce / consume BatchNorm statistics so the cross-GPU exchange (utils/sync_batchnorm/batchnorm.py:105-126:
- * ReduceAddCoalesced + Broadcast + thread pipes) rides inside them: no launch of its own (csrc/seg_sync.cuh). */
+ * kernels that produce BatchNorm statistics so the cross-GPU exchange (utils/sync_batchnorm/batchnorm.py:105-126:
+ * ReduceAddCoalesced + Broadcast + thread pipes) rides inside them, with no launch of its own (csrc/seg_sync.cuh): the
+ * producer's last block performs the whole exchange and leaves the WORLD's totals in its output (stats / sums), so the
+ * consumers (seg_bn_apply_train, seg_bn_bwd_apply) take no handle.  32 bytes. */
 typedef struct seg_sync_desc {
   void* const* peers;        /* DEVICE array of `world` base pointers; peers[rank] is this rank's buffer */
   int32_t rank, world, n_max;
   int64_t timeout_clocks;    /* spin-wait bound in GPU clocks (<= 0: unbounded) */
-  int32_t mode;              /* 0: producers push, the CONSUMER kernels (seg_bn_apply_train / seg_bn_bwd_apply with the same handle)
-                              *    wait for the world and add; 1: the producer's last block performs the whole exchange and leaves
-                              *    the world's totals in its output (stats / sums): call the consumers with sync = NULL */
 } seg_sync_desc;
 
 const char* seg_last_error(void);
@@ -73,9 +72,9 @@ void seg_launch_count_reset(void);
  * half of nn.BatchNorm2d, produced by the conv epilogue.  Every CTA adds its (fixed-order) fp32 column sums with one fp64
  * atomic per channel: a sum of fp32 values in fp64 is exact while their exponents span < 2^17, so the order of the atomics
  * cannot change the result — the statistics are bit-reproducible (fp32 atomics would not be).
- * sync (optional, with stats): SyncBN — the last CTA to finish also pushes the totals (as fp32) to every peer's symmetric
- * buffer and raises the flags (csrc/seg_sync.cuh); sync_ticket = one zeroed uint32.  The consumer is
- * seg_bn_apply_train(..., sync, ...).  stats requires beta == 0 (an error otherwise, on both implementations).
+ * sync (optional, with stats): SyncBN — the last CTA to finish also exchanges the totals (as fp64) with every peer and
+ * leaves the WORLD's totals in stats (csrc/seg_sync.cuh); sync_ticket = one zeroed uint32.  The consumer is
+ * seg_bn_apply_train with the world's count.  stats requires beta == 0 (an error otherwise, on both implementations).
  * beta != 0 with a bf16 y: the wgmma epilogue rounds the convolution (+bias) to bf16 before it adds beta*y, so the result
  * is rounded twice; the SIMT kernel adds in fp32 and rounds once. */
 int seg_conv2d_fwd(const seg_conv_desc* d, const void* x, const void* w_packed, void* y, int y_dtype,
@@ -150,16 +149,14 @@ int seg_bn_eval_scale_shift(int C, const float* gamma, const float* beta, const 
 int seg_bn_apply(const void* x, int ldx, const float* scale_shift, const void* res, int ldr, void* out, int ldo,
                  int64_t M, int C, int relu, float drop_p, uint64_t seed, const uint64_t* step_ctr, int drop_hw,
                  void* stream);
-/* stats: fp64 [2C] from seg_conv2d_fwd / seg_dwconv3x3_fwd / seg_bn_stats.
- * sync != NULL (SyncBN, the producer was called with the same handle): `stats` is ignored, the kernel waits for the
- * world's flags and adds every rank's sums itself; `count` is then the WORLD's element count; sync_done = one zeroed uint32.
+/* stats: fp64 [2C] from seg_conv2d_fwd / seg_dwconv3x3_fwd / seg_bn_stats over `count` elements (under SyncBN the world's
+ * totals and the WORLD's element count).
  * seg_bn_finalize + seg_bn_apply in ONE launch (training mode): coefficients are derived from the batch sums inside the
  * kernel; save[2C] = (mean, 1/std) for the backward pass and the running statistics are written by one block row. */
 int seg_bn_apply_train(const void* x, int ldx, const double* stats, double count, const float* gamma, const float* beta,
                        float eps, float momentum, int clamp_eps, float* running_mean, float* running_var, float* save,
                        const void* res, int ldr, void* out, int ldo, int64_t M, int C, int relu, float drop_p,
-                       uint64_t seed, const uint64_t* step_ctr, int drop_hw, const seg_sync_desc* sync,
-                       void* sync_done, void* stream);
+                       uint64_t seed, const uint64_t* step_ctr, int drop_hw, void* stream);
 /* device-side step counter (*ctr += inc): mixed into dropout seeds and SyncBN epochs so a captured CUDA graph of the
  * train step stays correct on every replay */
 int seg_counter_add(uint64_t* ctr, uint64_t inc, void* stream);
@@ -167,8 +164,8 @@ int seg_counter_add(uint64_t* ctr, uint64_t inc, void* stream);
  * launch: every block adds its partial sums to one of seg_bn_bwd_reduce_slots() copies of `acc` (fp64 [slots][2C], ZERO at
  * launch; exact, order-independent accumulation; the copies spread the atomics); the
  * last block (ticket: one zeroed uint32) rounds them into sums[] and, if given, dbeta (=|+=) sums[0:C] and dgamma (=|+=)
- * sums[C:2C] — the parameter gradients from the LOCAL sums.  sync: SyncBN — that block also pushes the sums to every peer;
- * the consumer is seg_bn_bwd_apply(..., sync, sync_done, ...).
+ * sums[C:2C] — the parameter gradients from the LOCAL sums.  sync: SyncBN — that block then exchanges the sums with every
+ * peer and leaves the WORLD's in sums[]; the consumer is seg_bn_bwd_apply with the world's count.
  * out == NULL with relu (both backward passes): the ReLU mask is recomputed from x with the forward's own coefficients
  * (sc = gamma/std, sh = fma(-mean, sc, beta)) instead of being read from the stored activation — valid for
  * conv -> BN(batch statistics) -> ReLU with no residual and no dropout; needs gamma and beta. */
@@ -178,18 +175,18 @@ int seg_bn_bwd_reduce(const void* dout, int lddo, const void* out, int ldo, cons
                       void* ticket, float* dgamma, float* dbeta, int accumulate, const float* gamma, const float* beta,
                       const seg_sync_desc* sync, void* stream);
 /* backward, pass 2: dx = gamma*istd*(dz - sums0/count - xhat*sums1/count); dres = beta_res*dres + dz (optional).
- * `sums` are the sums over `count` elements; sync != NULL: `sums` is ignored, the kernel waits for the world's flags and adds
- * every rank's sums itself (count = the world's); sync_done = one zeroed uint32. */
+ * `sums` are the sums over `count` elements (under SyncBN the world's, from seg_bn_bwd_reduce). */
 int seg_bn_bwd_apply(const void* dout, int lddo, const void* out, int ldo, const void* x, int ldx,
                      const float* save_mean_istd, const float* gamma, const float* sums, double count, int64_t M,
                      int C, int relu, float drop_p, void* dx, int lddx, void* dres, int lddres, float beta_res,
-                     const float* beta, const seg_sync_desc* sync, void* sync_done, void* stream);
+                     const float* beta, void* stream);
 /* BatchNorm backward in ONE cooperative launch = seg_bn_bwd_reduce + (SyncBN exchange) + seg_bn_bwd_apply: partial sums per
  * block -> grid barrier -> the cross-block sum spread over all blocks in fixed order (bit-reproducible) -> grid barrier ->
- * dx / dres.  sums[2C] receives the LOCAL totals; dgamma / dbeta (optional) the parameter gradients from them.  count_total =
- * rows summed over the world.  zero_sums != 0: frozen BatchNorm (BaseModel.freeze_bn): dx = gamma*istd*dz.  sync != NULL:
- * the totals are exchanged with the SyncBN peers inside the kernel.  Workspace from seg_bn_bwd_fused_workspace: rows
- * (uninitialised floats) and tickets (uint32, ZERO at launch).  The grid is sized to be co-resident. */
+ * dx / dres.  dgamma / dbeta (optional) receive the parameter gradients from the LOCAL totals.  count_total = rows summed
+ * over the world.  zero_sums != 0: frozen BatchNorm (BaseModel.freeze_bn): dx = gamma*istd*dz.  sync != NULL: one block
+ * exchanges the totals with the SyncBN peers inside the kernel.  sums[2C] receives the totals dx is computed from (the WORLD's
+ * under SyncBN).  Workspace from seg_bn_bwd_fused_workspace: rows (uninitialised floats) and tickets (uint32, ZERO at launch).
+ * The grid is sized to be co-resident. */
 int seg_bn_bwd_fused_workspace(int64_t M, int C, int64_t* rows_floats, int64_t* tickets);
 int seg_bn_bwd_fused(const void* dout, int lddo, const void* out, int ldo, const void* x, int ldx,
                      const float* save_mean_istd, const float* gamma, const float* beta, double count_total, int64_t M,
@@ -388,16 +385,18 @@ int seg_argmax_nchw_f32(const float* scores, int N, int C, int H, int W, int64_t
  *      sync_batchnorm/batchnorm.py:117,120 and the thread pipes of sync_batchnorm/comm.py) ----
  * Each rank owns a symmetric buffer of seg_comm_buffer_bytes(world, n_max) bytes (seg_comm_alloc, zeroed), exports it
  * with seg_comm_ipc_get, opens its peers' with seg_comm_ipc_open, and passes the world's pointers (indexed by rank;
- * its own pointer at [rank]) as a DEVICE array.  seg_syncbn_exchange(vals[n]) leaves the rank-ordered sum over all
- * ranks in vals on every rank (bit-identical everywhere).  All ranks must issue the same sequence of exchanges; the
- * sequence number lives in the symmetric buffer on the device, so the call can be captured in a CUDA graph. */
+ * its own pointer at [rank]) as a DEVICE array in a seg_sync_desc.  seg_syncbn_exchange(sync, vals[n]) leaves the
+ * rank-ordered sum over all ranks in vals on every rank (bit-identical everywhere): one block running the same exchange as
+ * the statistics producers (csrc/seg_sync.cuh), n <= n_max, world <= 64, spin wait bounded by sync->timeout_clocks.  All
+ * ranks must issue the same sequence of exchanges, in-kernel and stand-alone alike; the sequence number lives in the
+ * symmetric buffer on the device, so the call can be captured in a CUDA graph. */
 size_t seg_comm_buffer_bytes(int world, int n_max);
 int seg_comm_alloc(size_t bytes, void** ptr);
 int seg_comm_free(void* ptr);
 int seg_comm_ipc_get(void* ptr, void* handle64);
 int seg_comm_ipc_open(const void* handle64, void** ptr);
 int seg_comm_ipc_close(void* ptr);
-int seg_syncbn_exchange(void* const* peer_bufs, int rank, int world, float* local_vals, int n, int n_max, void* stream);
+int seg_syncbn_exchange(const seg_sync_desc* sync, float* vals, int n, void* stream);
 
 #ifdef __cplusplus
 }

@@ -2,7 +2,6 @@
 // (wgmma path where the shape allows it, CUDA-core implicit GEMM otherwise).  No CPU fallback anywhere.
 #include <stdarg.h>
 #include "seg_common.cuh"
-#include "seg_sync.cuh"
 
 namespace seg {
 
@@ -19,7 +18,7 @@ void set_error(const char* fmt, ...) {
 namespace tc {
 bool supported(const seg_conv_desc* d);
 int conv_fwd(const seg_conv_desc* d, const void* x, const void* w, void* y, int y_dtype, const float* bias, float beta,
-             double* stats, unsigned* stat_ticket, const SyncDesc* sync, cudaStream_t stream);
+             double* stats, unsigned* stat_ticket, const seg_sync_desc* sync, cudaStream_t stream);
 int conv_dgrad(const seg_conv_desc* d, const void* dy, const void* w, void* dx, float beta, cudaStream_t stream);
 int conv_wgrad(const seg_conv_desc* d, const void* dy, const void* x, float* dw, float* ws, cudaStream_t stream);
 int64_t wgrad_workspace_floats(const seg_conv_desc* d);
@@ -82,13 +81,8 @@ int seg_conv2d_fwd(const seg_conv_desc* d, const void* x, const void* w_packed, 
   SEG_REQUIRE(!stats || beta == 0.f, "seg_conv2d_fwd: BatchNorm statistics need beta = 0 (got beta = %g)", (double)beta);
   const bool tc_ok = tc::supported(d) && tma_base_ok(x) && tma_base_ok(w_packed);
   unsigned* tk = reinterpret_cast<unsigned*>(sync_ticket);
-  if (impl == SEG_IMPL_TC || (impl == SEG_IMPL_AUTO && tc_ok)) {
-    SyncDesc sd{nullptr, 0, 0, 0, 0, 0};
-    if (sync) {
-      sd.peers = sync->peers; sd.rank = sync->rank; sd.world = sync->world; sd.n_max = sync->n_max; sd.timeout_clocks = sync->timeout_clocks; sd.mode = sync->mode;
-    }
-    return tc::conv_fwd(d, x, w_packed, y, y_dtype, bias, beta, stats, tk, sync ? &sd : nullptr, ST(stream));
-  }
+  if (impl == SEG_IMPL_TC || (impl == SEG_IMPL_AUTO && tc_ok))
+    return tc::conv_fwd(d, x, w_packed, y, y_dtype, bias, beta, stats, tk, sync, ST(stream));
   return simt::conv_fwd(d, x, w_packed, y, y_dtype, bias, beta, stats, tk, sync, ST(stream));
 }
 

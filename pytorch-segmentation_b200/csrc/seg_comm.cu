@@ -1,82 +1,24 @@
-// seg_comm.cu — one-shot SyncBN statistics exchange over NVLink peer memory.
+// seg_comm.cu — symmetric buffers of the SyncBN statistics exchange and its stand-alone form.
 //
 // Replaces the reference's per-layer master-reduce + broadcast (utils/sync_batchnorm/batchnorm.py:105-126:
 // ReduceAddCoalesced.apply at :117, Broadcast.apply at :120, thread pipes in comm.py) — two collectives and a Python
-// queue round trip per BN layer — by ONE kernel per layer: every rank stores its <=16 KB vector (sum, sum of squares)
-// straight into a slot of every peer's symmetric buffer (P2P stores through NVSwitch), raises a flag with release
-// semantics, waits for the world's flags, and sums the world's vectors locally in rank order (so every rank gets
-// bit-identical totals and no broadcast is needed).  Every rank keeps a DEVICE-side sequence number in its own buffer
-// (all ranks issue the same exchanges in the same order, so the numbers agree): it is the flag value, and its parity
-// picks one of two slots.  A rank can run at most one exchange ahead of the slowest peer, so a slot is never
-// overwritten while still being read — and, the number living on the device, a captured CUDA graph replays correctly.
+// queue round trip per BN layer.  The protocol (push into every peer's slot, release flags, acquire wait, rank-ordered sum,
+// device-side sequence number) and the buffer layout live in seg_sync.cuh; the engine's kernels run it in their last block.
+// seg_syncbn_exchange is the same exchange as a one-block launch, for callers outside the engine.
 //
 // Symmetric buffer layout (per rank, allocated by seg_comm_alloc, exported with CUDA IPC):
 //   float    data [2][world][n_max]
 //   uint32_t flags[2][world]         (at byte offset 2*world*n_max*4, 128-byte aligned)
 //   uint32_t seq                     (next 128-byte line; number of exchanges this rank has completed)
 #include "seg_common.cuh"
+#include "seg_sync.cuh"
 
 namespace seg {
 
-__device__ __forceinline__ void st_release_sys(uint32_t* p, uint32_t v) {
-  asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
-__device__ __forceinline__ uint32_t ld_acquire_sys(const uint32_t* p) {
-  uint32_t v;
-  asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
+static_assert(sizeof(seg_sync_desc) == 32, "seg_sync_desc: pointer, three int32, padding, int64 (lib.SyncDesc mirrors it)");
 
-__host__ __device__ inline size_t flags_offset(int world, int n_max) {
-  size_t b = (size_t)2 * world * n_max * sizeof(float);
-  return (b + 127) & ~(size_t)127;
-}
-
-__host__ __device__ inline size_t seq_offset(int world, int n_max) {
-  size_t b = flags_offset(world, n_max) + (size_t)2 * world * sizeof(uint32_t);
-  return (b + 127) & ~(size_t)127;
-}
-
-__global__ void __launch_bounds__(1024) syncbn_exchange_kernel(void* const* __restrict__ peers, int rank, int world,
-                                                               float* __restrict__ vals, int n, int n_max) {
-  uint32_t* seq = reinterpret_cast<uint32_t*>(reinterpret_cast<char*>(peers[rank]) + seq_offset(world, n_max));
-  uint32_t epoch = *seq + 1u;  // written only by thread 0 at the very end of the previous exchange on this stream
-  if (epoch == 0u) epoch = 2u;  // flags start at 0: skip it on wrap-around, keeping the parity alternation
-  const int slot = epoch & 1;
-  const size_t foff = flags_offset(world, n_max);
-  // 1. scatter my vector into slot[rank] of every peer (including myself)
-  for (int i = threadIdx.x; i < n; i += blockDim.x) {
-    const float v = vals[i];
-    for (int p = 0; p < world; ++p) {
-      float* dst = reinterpret_cast<float*>(peers[p]) + ((size_t)slot * world + rank) * n_max + i;
-      *dst = v;
-    }
-  }
-  __threadfence_system();
-  __syncthreads();
-  // 2. publish, 3. wait for the world
-  if (threadIdx.x < world) {
-    const int p = threadIdx.x;
-    uint32_t* pf = reinterpret_cast<uint32_t*>(reinterpret_cast<char*>(peers[p]) + foff) + slot * world + rank;
-    st_release_sys(pf, epoch);
-    const uint32_t* mine = reinterpret_cast<const uint32_t*>(reinterpret_cast<const char*>(peers[rank]) + foff) + slot * world + p;
-    const long long t0 = clock64();
-    while (ld_acquire_sys(mine) != epoch) {
-      if (clock64() - t0 > 20000000000ll) {  // ~10 s: a peer died; trap instead of hanging the box
-        printf("seg_b200: syncbn exchange timeout (rank %d waiting for rank %d, epoch %u)\n", rank, p, epoch);
-        __trap();
-      }
-    }
-  }
-  __syncthreads();
-  // 4. reduce in rank order (bit-identical on every rank)
-  const float* my = reinterpret_cast<const float*>(peers[rank]) + (size_t)slot * world * n_max;
-  for (int i = threadIdx.x; i < n; i += blockDim.x) {
-    float s = 0.f;
-    for (int p = 0; p < world; ++p) s += __ldcv(my + (size_t)p * n_max + i);
-    vals[i] = s;
-  }
-  if (threadIdx.x == 0) *seq = epoch;  // every thread read *seq before the first __syncthreads above
+__global__ void __launch_bounds__(1024) syncbn_exchange_kernel(const SyncDesc s, float* __restrict__ vals, int n) {
+  sync_exchange_block_f(s, vals, n, (int)threadIdx.x, (int)blockDim.x, [] { __syncthreads(); });
 }
 
 }  // namespace seg
@@ -85,7 +27,7 @@ using namespace seg;
 
 extern "C" {
 
-size_t seg_comm_buffer_bytes(int world, int n_max) { return seq_offset(world, n_max) + 128; }
+size_t seg_comm_buffer_bytes(int world, int n_max) { return sync_seq_offset(world, n_max) + 128; }
 
 int seg_comm_alloc(size_t bytes, void** ptr) {
   cudaError_t e = cudaMalloc(ptr, bytes);
@@ -118,12 +60,18 @@ int seg_comm_ipc_close(void* ptr) {
   return 0;
 }
 
-int seg_syncbn_exchange(void* const* peer_bufs, int rank, int world, float* local_vals, int n, int n_max, void* stream) {
-  SEG_REQUIRE(world >= 1 && world <= 64 && rank >= 0 && rank < world, "bad rank/world %d/%d", rank, world);
-  SEG_REQUIRE(n > 0 && n <= n_max, "syncbn exchange: n=%d exceeds n_max=%d", n, n_max);
+int seg_syncbn_exchange(const seg_sync_desc* sync, float* vals, int n, void* stream) {
+  // the handle is read on the host: a device address (such as the peer-pointer array itself) is refused, not dereferenced
+  cudaPointerAttributes attr;
+  const bool host_handle = sync != nullptr && cudaPointerGetAttributes(&attr, sync) == cudaSuccess && attr.type != cudaMemoryTypeDevice;
+  if (!host_handle) cudaGetLastError();  // a failed query must not surface at the next launch check
+  SEG_REQUIRE(host_handle, "syncbn exchange: `sync` must point to a seg_sync_desc in host memory");
+  SEG_REQUIRE(sync->world >= 1 && sync->world <= 64 && sync->rank >= 0 && sync->rank < sync->world, "bad rank/world %d/%d",
+              sync->rank, sync->world);
+  SEG_REQUIRE(n > 0 && n <= sync->n_max, "syncbn exchange: n=%d exceeds n_max=%d", n, sync->n_max);
+  // >= 64 threads: thread p < world raises this rank's flag on peer p and waits for peer p's
   const int threads = n >= 1024 ? 1024 : ((n + 31) / 32 * 32 < 64 ? 64 : (n + 31) / 32 * 32);
-  syncbn_exchange_kernel<<<1, threads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(peer_bufs, rank, world, local_vals, n,
-                                                                                     n_max);
+  syncbn_exchange_kernel<<<1, threads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(*sync, vals, n);
   return check_launch("syncbn_exchange");
 }
 

@@ -265,12 +265,9 @@ int seg_dwconv3x3_fwd(const seg_conv_desc* d, const void* x, const float* w9, vo
   if (dw_check(d)) return 1;
   SEG_REQUIRE(!sync || (stats && sync_ticket && 4 * d->C <= sync->n_max), "dwconv fwd: SyncBN needs stats, a zeroed ticket and 4*C <= n_max");
   const int64_t M = (int64_t)d->N * d->P * d->Q;
-  SyncDesc sd{nullptr, 0, 0, 0, 0, 0};
-  if (sync) {
-    sd.peers = sync->peers; sd.rank = sync->rank; sd.world = sync->world; sd.n_max = sync->n_max; sd.timeout_clocks = sync->timeout_clocks; sd.mode = sync->mode;
-  }
   dwconv_fwd_kernel<<<dw_grid(M, d->C), 256, 0, ST(stream)>>>(CBF(x), d->ldx, w9, BF(y), d->ldy, d->N, d->H, d->W, d->C, d->P, d->Q,
-                                                              d->stride, d->pad, d->dil, stats, sd, reinterpret_cast<unsigned*>(sync_ticket));
+                                                              d->stride, d->pad, d->dil, stats, sync ? *sync : SyncDesc{},
+                                                              reinterpret_cast<unsigned*>(sync_ticket));
   return check_launch("dwconv_fwd");
 }
 

@@ -295,24 +295,15 @@ struct BnTrain {
   float *running_mean, *running_var, *save;
 };
 
-template <bool SYNC>
 __global__ void __launch_bounds__(256, 4) bn_apply_kernel(const __nv_bfloat16* __restrict__ x, int ldx,
                                                        const float* __restrict__ ss, const __nv_bfloat16* __restrict__ res,
                                                        int ldr, __nv_bfloat16* __restrict__ out, int ldo, int64_t M, int C,
                                                        int relu, float drop_p, uint64_t seed,
-                                                       const uint64_t* __restrict__ step_ctr, int drop_hw, const BnTrain tr,
-                                                       const SyncDesc sync, unsigned* sync_done) {
+                                                       const uint64_t* __restrict__ step_ctr, int drop_hw, const BnTrain tr) {
   pdl_wait();
   const RowMap rm = row_map(C);
   if (step_ctr) seed += (*step_ctr) * 0x9E3779B97F4A7C15ull;  // device-side step counter keeps CUDA-graph replays fresh
   const float keep_scale = drop_p > 0.f ? 1.f / (1.f - drop_p) : 1.f;
-  // SyncBN (seg_sync.cuh): the producing conv pushed every rank's sums into this rank's symmetric buffer; wait for the
-  // world's flags, then add the world's sums in rank order
-  uint32_t epoch = 0u;
-  if constexpr (SYNC) {
-    epoch = sync_epoch(sync);
-    sync_wait_world(sync, epoch);
-  }
   float sc[8], sh[8];
   if (rm.active) {
     if (tr.stats) {
@@ -323,10 +314,11 @@ __global__ void __launch_bounds__(256, 4) bn_apply_kernel(const __nv_bfloat16* _
       const double inv_count = 1.0 / tr.count;  // one division; the per-channel math below is multiply-add + fp32 rsqrt
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
-        // fp64 totals, one channel at a time (no register arrays of doubles): local accumulators, or the world's (SyncBN)
+        // fp64 totals, one channel at a time (no register arrays of doubles); under SyncBN the producer's exchange has
+        // already turned them into the world's
         const int cj = rm.g * 8 + j;
-        const double s1 = SYNC ? sync_total_d(sync, epoch, cj) : __ldg(tr.stats + cj);
-        const double s2 = SYNC ? sync_total_d(sync, epoch, C + cj) : __ldg(tr.stats + C + cj);
+        const double s1 = __ldg(tr.stats + cj);
+        const double s2 = __ldg(tr.stats + C + cj);
         const double mean = s1 * inv_count;
         double var = fma(s2, inv_count, -mean * mean);
         if (var < 0) var = 0;
@@ -392,12 +384,10 @@ __global__ void __launch_bounds__(256, 4) bn_apply_kernel(const __nv_bfloat16* _
     }
   }
   pdl_trigger();
-  if constexpr (SYNC) sync_consumer_done(sync, epoch, sync_done, gridDim.x * gridDim.y);
 }
 
 __device__ __noinline__ void bn_bwd_reduce_finalize(const double* acc, float* final_sums, float* dgamma, float* dbeta, int accumulate,
                                                     int C, const SyncDesc sync) {
-  const uint32_t epoch = (sync.world > 0 && sync.mode == 0) ? sync_epoch(sync) : 0u;
   for (int c = threadIdx.x; c < 2 * C; c += blockDim.x) {
     double t = 0.0;  // the copies' totals are exact sums; so is their sum
 #pragma unroll
@@ -407,16 +397,11 @@ __device__ __noinline__ void bn_bwd_reduce_finalize(const double* acc, float* fi
     float* pg = c < C ? dbeta : dgamma;
     const int ch = c < C ? c : c - C;
     if (pg) pg[ch] = accumulate ? pg[ch] + v : v;
-    if (sync.world > 0 && sync.mode == 0) sync_push_value(sync, epoch, c, v);
   }
-  if (sync.world > 0) {
-    if (sync.mode == 1) {  // whole exchange here: final_sums becomes the world's sums (bn_bwd_apply then needs no SyncBN logic)
-      __threadfence();
-      __syncthreads();
-      sync_exchange_block_f(sync, final_sums, 2 * C, (int)threadIdx.x, (int)blockDim.x, [] { __syncthreads(); });
-    } else {
-      sync_publish(sync, epoch, (int)threadIdx.x, [] { __syncthreads(); });
-    }
+  if (sync.world > 0) {  // whole exchange here: final_sums becomes the world's sums (bn_bwd_apply then needs no SyncBN logic)
+    __threadfence();
+    __syncthreads();
+    sync_exchange_block_f(sync, final_sums, 2 * C, (int)threadIdx.x, (int)blockDim.x, [] { __syncthreads(); });
   }
 }
 
@@ -478,20 +463,15 @@ __global__ void __launch_bounds__(256, 4)
 }
 
 // dx = A*dz + B*x + Cc with A = gamma*istd, B = -gamma*istd^2*s1/count, Cc = -gamma*istd*s0/count + gamma*istd^2*mean*s1/count
-template <bool REMASK, bool SYNC>
+template <bool REMASK>
 __global__ void __launch_bounds__(256, 4)
     bn_bwd_apply_kernel(const __nv_bfloat16* __restrict__ dout, int lddo, const __nv_bfloat16* __restrict__ out, int ldo,
                         const __nv_bfloat16* __restrict__ x, int ldx, const float* __restrict__ save,
                         const float* __restrict__ gamma, const float* __restrict__ sums, float inv_count, int64_t M, int C,
                         int relu, float drop_p, __nv_bfloat16* __restrict__ dx, int lddx, __nv_bfloat16* dres, int lddres,
-                        float beta_res, const float* __restrict__ beta, const SyncDesc sync, unsigned* sync_done) {
+                        float beta_res, const float* __restrict__ beta) {
   pdl_wait();
   const RowMap rm = row_map(C);
-  uint32_t epoch = 0u;
-  if constexpr (SYNC) {  // SyncBN: bn_bwd_reduce pushed every rank's sums; wait for the world, add in rank order
-    epoch = sync_epoch(sync);
-    sync_wait_world(sync, epoch);
-  }
   const float keep_scale = drop_p > 0.f ? 1.f / (1.f - drop_p) : 1.f;
   const int co = rm.g * 8;
   float cA[8], cB[8], cC[8], sh[REMASK ? 8 : 1];
@@ -500,13 +480,8 @@ __global__ void __launch_bounds__(256, 4)
     ld8(save + co, mean);
     ld8(save + C + co, istd);
     ld8(gamma + co, gm);
-    if constexpr (SYNC) {
-      sync_total8(sync, epoch, co, s0);
-      sync_total8(sync, epoch, C + co, s1);
-    } else {
-      ld8(sums + co, s0);
-      ld8(sums + C + co, s1);
-    }
+    ld8(sums + co, s0);
+    ld8(sums + C + co, s1);
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       const float a = gm[j] * istd[j];
@@ -556,7 +531,6 @@ __global__ void __launch_bounds__(256, 4)
     *reinterpret_cast<bf16x8*>(dx + row * lddx + co) = pack8(o8);
   }
   pdl_trigger();
-  if constexpr (SYNC) sync_consumer_done(sync, epoch, sync_done, gridDim.x * gridDim.y);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -566,9 +540,8 @@ __global__ void __launch_bounds__(256, 4)
 //   barrier   all blocks are co-resident (the host sizes the grid from the occupancy of THIS kernel), so a grid-wide
 //             barrier is an atomic counter + spin
 //   phase 1b  the cross-block sum is spread over ALL blocks: block b adds its few columns over every row, in row order ->
-//             bit-reproducible totals with no atomics at all;
-//             the same threads write dgamma / dbeta and, under SyncBN, push the totals to every peer (seg_sync.cuh)
-//   barrier   (+ SyncBN: block 0 raises this rank's flags, every block waits for the world's)
+//             bit-reproducible totals with no atomics at all; the same threads write dgamma / dbeta
+//   barrier   (+ SyncBN: block 0 exchanges the totals with the peers (seg_sync.cuh), leaving the world's; barrier)
 //   phase 2   dx = A*dz + B*x + Cc (and the residual branch's gradient); the second read of dz / x hits L2 for the small maps
 // Same arithmetic as the two-launch path.
 __device__ __forceinline__ unsigned ld_acquire_gpu(const unsigned* p) {
@@ -601,8 +574,8 @@ struct BnBwdFused {
   int C, relu;
   float drop_p, inv_count;  // inv_count = 1 / (rows summed over the WORLD)
   float* rows;              // [gridDim.y][gridDim.x][2][W] partial sums (W = channels of a slab)
-  float* totals;            // [2C] LOCAL totals (always written)
-  unsigned* ctr;            // [0] grid-barrier counter, [1] SyncBN consumer ticket; zero at launch
+  float* totals;            // [2C] totals (always written): the LOCAL ones, the world's after a SyncBN exchange
+  unsigned* ctr;            // grid-barrier counter, zero at launch
   float *dgamma, *dbeta;
   int accumulate, zero_sums;  // zero_sums: frozen BatchNorm (eval statistics): dx = gamma*istd*dz
   __nv_bfloat16 *dx, *dres;
@@ -686,7 +659,6 @@ __global__ void __launch_bounds__(256, 3) bn_bwd_fused_kernel(const BnBwdFused p
   }
   grid_barrier(p.ctr, nblocks);
   // ------------------------------------------------ phase 1b: distributed fixed-order fold of this slab's 2W columns
-  const uint32_t epoch = p.sync.world > 0 ? sync_epoch(p.sync) : 0u;
   {
     const int nb = gridDim.x;
     const int ncol = 2 * W;
@@ -713,29 +685,21 @@ __global__ void __launch_bounds__(256, 3) bn_bwd_fused_kernel(const BnBwdFused p
           p.totals[(size_t)a * C + ch] = tot;
           float* pg = a == 0 ? p.dbeta : p.dgamma;
           if (pg) pg[ch] = p.accumulate ? pg[ch] + tot : tot;
-          if (p.sync.world > 0 && p.sync.mode == 0) sync_push_value(p.sync, epoch, a * C + ch, tot);
         }
       }
     }
     if (p.sync.world > 0) __threadfence_system();
   }
   grid_barrier(p.ctr, 2u * nblocks);
-  // ------------------------------------------------ SyncBN: publish, wait for the world, totals from every rank
+  // ------------------------------------------------ SyncBN: ONE block exchanges the finished local totals with the world and
+  // leaves the world's in p.totals
   float s0[8], s1[8];
-  if (p.sync.world > 0 && p.sync.mode == 1) {
-    // mode 1: ONE block exchanges the finished local totals with the world and leaves the world's in p.totals
+  if (p.sync.world > 0) {
     if (blockIdx.x == 0 && blockIdx.y == 0)
       sync_exchange_block_f(p.sync, p.totals, 2 * C, (int)threadIdx.x, 256, [] { __syncthreads(); });
     grid_barrier(p.ctr, 3u * nblocks);
   }
-  if (p.sync.world > 0 && p.sync.mode == 0) {
-    if (blockIdx.x == 0 && blockIdx.y == 0) sync_publish(p.sync, epoch, (int)threadIdx.x, [] { __syncthreads(); });
-    sync_wait_world(p.sync, epoch);
-    if (rm.active) {
-      sync_total8(p.sync, epoch, co, s0);
-      sync_total8(p.sync, epoch, C + co, s1);
-    }
-  } else if (rm.active) {
+  if (rm.active) {
     *reinterpret_cast<float4*>(s0) = __ldcg(reinterpret_cast<const float4*>(p.totals + co));
     *reinterpret_cast<float4*>(s0 + 4) = __ldcg(reinterpret_cast<const float4*>(p.totals + co + 4));
     *reinterpret_cast<float4*>(s1) = __ldcg(reinterpret_cast<const float4*>(p.totals + C + co));
@@ -784,7 +748,6 @@ __global__ void __launch_bounds__(256, 3) bn_bwd_fused_kernel(const BnBwdFused p
       *reinterpret_cast<bf16x8*>(p.dx + row * p.lddx + co) = pack8(o8);
     }
   }
-  if (p.sync.world > 0 && p.sync.mode == 0) sync_consumer_done(p.sync, epoch, p.ctr + 1, nblocks);
 }
 
 __global__ void bn_param_grad_kernel(const float* __restrict__ sums, int C, float* dgamma, float* dbeta, int accumulate) {
@@ -1379,14 +1342,7 @@ static dim3 colreduce_grid(int64_t M, int C) {
   return dim3((unsigned)gx, (unsigned)gy, 1);
 }
 
-static SyncDesc to_sync(const seg_sync_desc* sync) {
-  SyncDesc sd{nullptr, 0, 0, 0, 0, 0};
-  if (sync) {
-    sd.peers = sync->peers; sd.rank = sync->rank; sd.world = sync->world; sd.n_max = sync->n_max; sd.timeout_clocks = sync->timeout_clocks;
-    sd.mode = sync->mode;
-  }
-  return sd;
-}
+static SyncDesc to_sync(const seg_sync_desc* sync) { return sync ? *sync : SyncDesc{}; }
 }  // extern "C"
 namespace seg {
 // also used by the CUDA-core conv path (seg_conv_simt.cu) for its BatchNorm statistics
@@ -1419,23 +1375,19 @@ int seg_bn_apply(const void* x, int ldx, const float* ss, const void* res, int l
   SEG_REQUIRE(C % 8 == 0 && ldx % 8 == 0 && ldo % 8 == 0 && (!res || ldr % 8 == 0), "bn_apply: alignment");
   BnTrain tr;
   memset(&tr, 0, sizeof(tr));
-  launch_pdl(bn_apply_kernel<false>, rowmap_grid(M, C), dim3(256), 0, ST(stream), CBF(x), ldx, ss, CBF(res), ldr, BF(out), ldo, M, C, relu,
-             drop_p, seed, step_ctr, drop_hw, tr, SyncDesc{nullptr, 0, 0, 0, 0, 0}, (unsigned*)nullptr);
+  launch_pdl(bn_apply_kernel, rowmap_grid(M, C), dim3(256), 0, ST(stream), CBF(x), ldx, ss, CBF(res), ldr, BF(out), ldo, M, C, relu,
+             drop_p, seed, step_ctr, drop_hw, tr);
   return check_launch("bn_apply");
 }
 int seg_bn_apply_train(const void* x, int ldx, const double* stats, double count, const float* gamma, const float* beta,
                        float eps, float momentum, int clamp_eps, float* running_mean, float* running_var, float* save,
                        const void* res, int ldr, void* out, int ldo, int64_t M, int C, int relu, float drop_p,
-                       uint64_t seed, const uint64_t* step_ctr, int drop_hw, const seg_sync_desc* sync, void* sync_done,
-                       void* stream) {
+                       uint64_t seed, const uint64_t* step_ctr, int drop_hw, void* stream) {
   SEG_REQUIRE(C % 8 == 0 && ldx % 8 == 0 && ldo % 8 == 0 && (!res || ldr % 8 == 0), "bn_apply_train: alignment");
   SEG_REQUIRE(stats && gamma && beta && save && count > 0, "bn_apply_train: stats, gamma, beta, save required");
-  SEG_REQUIRE(!sync || (sync_done != nullptr && 4 * C <= sync->n_max), "bn_apply_train: SyncBN needs a zeroed ticket and 4*C <= n_max (fp64 totals)");
-  const SyncDesc sd = to_sync(sync);
   BnTrain tr = {stats, count, gamma, beta, eps, momentum, clamp_eps, running_mean, running_var, save};
-  launch_pdl(sync ? bn_apply_kernel<true> : bn_apply_kernel<false>, rowmap_grid(M, C), dim3(256), 0, ST(stream), CBF(x), ldx,
-             (const float*)nullptr, CBF(res), ldr, BF(out), ldo, M, C, relu, drop_p, seed, step_ctr, drop_hw, tr, sd,
-             reinterpret_cast<unsigned*>(sync_done));
+  launch_pdl(bn_apply_kernel, rowmap_grid(M, C), dim3(256), 0, ST(stream), CBF(x), ldx, (const float*)nullptr, CBF(res), ldr, BF(out),
+             ldo, M, C, relu, drop_p, seed, step_ctr, drop_hw, tr);
   return check_launch("bn_apply_train");
 }
 // reductions end with a block fold + 2C atomics per block: fewer, fatter blocks (>= 32 rows per thread)
@@ -1458,17 +1410,12 @@ int seg_bn_bwd_reduce(const void* dout, int lddo, const void* out, int ldo, cons
 }
 int seg_bn_bwd_apply(const void* dout, int lddo, const void* out, int ldo, const void* x, int ldx, const float* save,
                      const float* gamma, const float* sums, double count, int64_t M, int C, int relu, float drop_p,
-                     void* dx, int lddx, void* dres, int lddres, float beta_res, const float* beta, const seg_sync_desc* sync,
-                     void* sync_done, void* stream) {
+                     void* dx, int lddx, void* dres, int lddres, float beta_res, const float* beta, void* stream) {
   SEG_REQUIRE(C % 8 == 0 && lddo % 8 == 0 && ldx % 8 == 0 && lddx % 8 == 0, "bn_bwd_apply: alignment");
   SEG_REQUIRE(!(relu && !out) || (beta && drop_p == 0.f), "bn_bwd_apply: out == NULL (mask recomputed from x) needs beta and no dropout");
-  SEG_REQUIRE(!sync || (sync_done && 2 * C <= sync->n_max), "bn_bwd_apply: SyncBN needs a zeroed ticket and 2*C <= n_max");
-  auto kfn = sync ? ((relu && !out) ? bn_bwd_apply_kernel<true, true> : bn_bwd_apply_kernel<false, true>)
-                  : ((relu && !out) ? bn_bwd_apply_kernel<true, false> : bn_bwd_apply_kernel<false, false>);
-  launch_pdl(kfn, rowmap_grid(M, C), dim3(256), 0, ST(stream),
+  launch_pdl((relu && !out) ? bn_bwd_apply_kernel<true> : bn_bwd_apply_kernel<false>, rowmap_grid(M, C), dim3(256), 0, ST(stream),
              CBF(dout), lddo, CBF(out), ldo, CBF(x), ldx, save,
-             gamma, sums, (float)(1.0 / count), M, C, relu, drop_p, BF(dx), lddx, BF(dres), lddres, beta_res, beta, to_sync(sync),
-             reinterpret_cast<unsigned*>(sync_done));
+             gamma, sums, (float)(1.0 / count), M, C, relu, drop_p, BF(dx), lddx, BF(dres), lddres, beta_res, beta);
   return check_launch("bn_bwd_apply");
 }
 }  // extern "C"
@@ -1496,7 +1443,7 @@ int seg_bn_bwd_fused_workspace(int64_t M, int C, int64_t* rows_floats, int64_t* 
   const dim3 g = fused_grid(M, C, bps);
   const int G = C / 8, GB = G < 256 ? G : 256;
   *rows_floats = (int64_t)g.y * g.x * 2 * GB * 8;
-  *tickets = 2;
+  *tickets = 1;
   return 0;
 }
 int seg_bn_bwd_fused(const void* dout, int lddo, const void* out, int ldo, const void* x, int ldx, const float* save,
@@ -1519,7 +1466,7 @@ int seg_bn_bwd_fused(const void* dout, int lddo, const void* out, int ldo, const
   p.dx = BF(dx); p.dres = BF(dres); p.lddx = lddx; p.lddres = lddres; p.beta_res = beta_res;
   if (sync) {
     SEG_REQUIRE(2 * C <= sync->n_max, "bn_bwd_fused: 2*C = %d sums exceed the SyncBN buffer (%d floats)", 2 * C, sync->n_max);
-    p.sync = to_sync(sync);
+    p.sync = *sync;
   }
   // multi-GPU: leave one block slot per SM free — a concurrently running NCCL kernel (bucketed gradient all-reduce on the side
   // stream) must not keep part of this grid from becoming resident, or every block would sit at the barrier until it finishes

@@ -1,38 +1,34 @@
-// seg_sync.cuh — SyncBN statistics exchange folded INTO the kernels that produce and consume the statistics.
+// seg_sync.cuh — SyncBN statistics exchange folded INTO the kernels that produce the statistics.
 //
 // A stand-alone exchange kernel per BatchNorm layer and direction (226 launches per DeepLab-R101 step) would be a world-wide
 // flag barrier sitting alone between a conv epilogue and bn_apply, paid once per exchange.  Here the exchange has no launch
-// of its own:
+// of its own.  A producer is a kernel that ends with per-channel totals: the conv epilogues / the depthwise conv / bn_stats
+// (fp64 atomics into the layer's accumulators), bn_bwd_reduce and the cooperative BN backward.  ONE block of it — the last to
+// finish (one ticket per launch), or block 0 after a grid barrier — runs the whole exchange with its cooperating threads:
+//   push     store the finished totals into slot[rank] of EVERY peer's symmetric buffer (P2P stores through NVSwitch);
+//   publish  raise this rank's flag on every peer (st.release.sys);
+//   wait     poll the world's flags in the LOCAL buffer (ld.acquire.sys);
+//   total    add the world's vectors in rank order (-> bit-identical totals on every rank, no broadcast), in place;
+//   advance  store the sequence number.
+// The producer's ordinary output then holds the WORLD's totals, so the consumers (bn_apply, bn_bwd_apply) are the single-GPU
+// kernels.  seg_comm.cu's stand-alone exchange (seg_syncbn_exchange, for callers outside the engine) is one block running
+// sync_exchange_block_f.
 //
-//   producer  = a kernel that ends with per-channel totals: the conv epilogues / the depthwise conv / bn_stats (fp64 atomics
-//               into the layer's accumulators) and bn_bwd_reduce / the cooperative BN backward.  The LAST block to finish
-//               (one ticket per launch) reads the finished totals and stores them into slot[rank] of EVERY peer's symmetric
-//               buffer (P2P stores through NVSwitch), then raises this rank's flag on every peer (st.release.sys).  The NVLink
-//               latency overlaps the kernel's tail and the next launch.
-//   consumer  = the prologue of bn_apply / bn_bwd_apply: every block waits for the world's flags (ld.acquire.sys), then each
-//               thread adds, in rank order (-> bit-identical totals on every rank, no broadcast), the world's sums for its own
-//               channels from the LOCAL symmetric buffer.  The last consumer block to finish advances the sequence number.
-//
-// Protocol state is the same as seg_comm.cu's stand-alone exchange kernel (kept for tests and callers outside the engine): per
-// rank a symmetric buffer
+// Protocol state, per rank a symmetric buffer
 //     float data[2][world][n_max] | uint32 flags[2][world] | uint32 seq
 // `seq` = number of exchanges this rank has COMPLETED, kept on the device (all ranks issue the same exchanges in the same
 // order) so a captured CUDA graph replays correctly; epoch = seq + 1 is the flag value and its parity picks the slot.  A rank
-// can run at most one exchange ahead of the slowest peer (its consumer needs every peer's flag of the current epoch, and a
-// peer raises it only after ITS consumer of the previous epoch has finished), so a slot is never overwritten while read.
+// can run at most one exchange ahead of the slowest peer (it waits for every peer's flag of the current epoch, and a peer
+// raises it only after it has read the totals of the previous epoch), so a slot is never overwritten while read.
 #pragma once
 #include <stdint.h>
 #include <stdio.h>
+#include "../../include/seg_b200.h"
 
 namespace seg {
 
-struct SyncDesc {  // mirror of seg_sync_desc (include/seg_b200.h)
-  void* const* peers;        // device array of `world` symmetric-buffer base pointers (peers[rank] = mine)
-  int rank, world, n_max;
-  long long timeout_clocks;  // spin-wait bound (<= 0: 2^62)
-  int mode;                  // 0: the CONSUMER kernel waits for the world and sums (every block polls the flags);
-                             // 1: the PRODUCER's last block does the whole exchange and leaves the world totals in the local buffer
-};
+// the kernels take the C handle by value; timeout_clocks <= 0 bounds the spin wait at 2^62 clocks
+using SyncDesc = seg_sync_desc;
 
 __host__ __device__ inline size_t sync_flags_offset(int world, int n_max) {
   size_t b = (size_t)2 * world * n_max * sizeof(float);
@@ -57,7 +53,7 @@ __device__ __forceinline__ uint32_t sync_ld_relaxed_sys(const uint32_t* p) {
   return v;
 }
 
-// epoch of the exchange in flight on this stream (seq is advanced by the last consumer block of the previous one)
+// epoch of the exchange in flight on this stream (seq is advanced at the end of the previous one)
 __device__ __forceinline__ uint32_t sync_epoch(const SyncDesc& s) {
   const uint32_t* seq = reinterpret_cast<const uint32_t*>(reinterpret_cast<const char*>(s.peers[s.rank]) + sync_seq_offset(s.world, s.n_max));
   uint32_t e = sync_ld_relaxed_sys(seq) + 1u;
@@ -65,7 +61,7 @@ __device__ __forceinline__ uint32_t sync_epoch(const SyncDesc& s) {
   return e;
 }
 
-// producer, per value: store element `idx` of this rank's vector into slot[rank] of every peer (myself included)
+// push, per value: store element `idx` of this rank's vector into slot[rank] of every peer (myself included)
 __device__ __forceinline__ void sync_push_value(const SyncDesc& s, uint32_t epoch, int idx, float v) {
   const size_t off = ((size_t)(epoch & 1u) * s.world + s.rank) * s.n_max + idx;
   for (int p = 0; p < s.world; ++p) reinterpret_cast<float*>(s.peers[p])[off] = v;
@@ -84,8 +80,7 @@ __device__ __forceinline__ double sync_total_d(const SyncDesc& s, uint32_t epoch
   return t;
 }
 
-// producer, once per layer, by the `nthr` cooperating threads of the block that completed the layer's LAST lane (every
-// pushing block executed __threadfence_system() before taking the lane ticket): raise this rank's flag on every peer
+// publish, by the `nthr` cooperating threads of the exchanging block after their pushes: raise this rank's flag on every peer
 template <class Sync>
 __device__ __forceinline__ void sync_publish(const SyncDesc& s, uint32_t epoch, int tid, Sync sync) {
   __threadfence_system();
@@ -97,50 +92,14 @@ __device__ __forceinline__ void sync_publish(const SyncDesc& s, uint32_t epoch, 
   }
 }
 
-// producer epilogue for kernels that accumulate their per-channel totals with fp64 atomics into `acc` (n doubles): every
-// contributing block calls this with its `nthr` cooperating threads after issuing its atomics; the LAST of `nblocks` blocks to
-// arrive (ticket) reads the finished totals and pushes them (as fp64) to every peer, then raises the flags.
-template <bool kPrint, class Sync>
-__device__ __forceinline__ void sync_exchange_block_d(const SyncDesc& s, double* acc, int n, int tid, int nthr, Sync sync);
-// kPrint = false: time out with a bare trap — no printf call, which would make ptxas serialise a caller's wgmma pipeline
-template <bool kPrint = true, class Sync>
-__device__ __forceinline__ void sync_push_when_last(const SyncDesc& s, const double* acc, int n, unsigned* ticket, unsigned nblocks,
-                                                    int tid, int nthr, Sync sync, volatile int* sm_flag) {
-  __threadfence();
-  sync();
-  if (tid == 0) *sm_flag = (atomicAdd(ticket, 1u) == nblocks - 1u);
-  sync();
-  if (!*sm_flag) return;
-  __threadfence();
-  if (s.mode == 1) {  // the whole exchange here: acc becomes the world's totals, the consumer needs no SyncBN logic
-    sync_exchange_block_d<kPrint>(s, const_cast<double*>(acc), n, tid, nthr, sync);
-    return;
-  }
-  const uint32_t epoch = sync_epoch(s);
-  for (int i = tid; i < n; i += nthr) sync_push_value_d(s, epoch, i, __ldcg(acc + i));
-  sync_publish(s, epoch, tid, sync);
-}
-
-// consumer: world total of element idx, added in rank order (bit-identical on every rank)
+// total: world total of element idx, added in rank order (bit-identical on every rank)
 __device__ __forceinline__ float sync_total(const SyncDesc& s, uint32_t epoch, int idx) {
   const float* my = reinterpret_cast<const float*>(s.peers[s.rank]) + (size_t)(epoch & 1u) * s.world * s.n_max + idx;
   float t = 0.f;
   for (int p = 0; p < s.world; ++p) t += __ldcv(my + (size_t)p * s.n_max);
   return t;
 }
-__device__ __forceinline__ void sync_total8(const SyncDesc& s, uint32_t epoch, int idx, float* out8) {
-  const float* my = reinterpret_cast<const float*>(s.peers[s.rank]) + (size_t)(epoch & 1u) * s.world * s.n_max + idx;
-#pragma unroll
-  for (int j = 0; j < 8; ++j) out8[j] = 0.f;
-  for (int p = 0; p < s.world; ++p) {
-    const float4 a = __ldcv(reinterpret_cast<const float4*>(my + (size_t)p * s.n_max));
-    const float4 b = __ldcv(reinterpret_cast<const float4*>(my + (size_t)p * s.n_max + 4));
-    out8[0] += a.x; out8[1] += a.y; out8[2] += a.z; out8[3] += a.w;
-    out8[4] += b.x; out8[5] += b.y; out8[6] += b.z; out8[7] += b.w;
-  }
-}
 
-// ---- mode 1: the whole exchange inside the producer's last block -----------------------------------------------------------------
 // wait for the world's flags with the `nthr` cooperating threads of ONE block (tid 0..nthr-1, `sync()` their barrier)
 template <bool kPrint = true, class Sync>
 __device__ __forceinline__ void sync_wait_world_block(const SyncDesc& s, uint32_t epoch, int tid, Sync sync) {
@@ -176,7 +135,7 @@ __device__ __forceinline__ void sync_exchange_block_d(const SyncDesc& s, double*
   sync();
   if (tid == 0) sync_advance(s, epoch);
 }
-// fp32 variant (BatchNorm backward sums)
+// fp32 variant (BatchNorm backward sums, seg_syncbn_exchange)
 template <class Sync>
 __device__ __forceinline__ void sync_exchange_block_f(const SyncDesc& s, float* vals, int n, int tid, int nthr, Sync sync) {
   const uint32_t epoch = sync_epoch(s);
@@ -189,36 +148,20 @@ __device__ __forceinline__ void sync_exchange_block_f(const SyncDesc& s, float* 
   if (tid == 0) sync_advance(s, epoch);
 }
 
-// consumer: all threads of the block call this; returns after every rank's flag shows `epoch`
-__device__ __forceinline__ void sync_wait_world(const SyncDesc& s, uint32_t epoch) {
-  if ((int)threadIdx.x < s.world) {
-    const uint32_t* mine = reinterpret_cast<const uint32_t*>(reinterpret_cast<const char*>(s.peers[s.rank]) + sync_flags_offset(s.world, s.n_max)) +
-                           (size_t)(epoch & 1u) * s.world + threadIdx.x;
-    const long long limit = s.timeout_clocks > 0 ? s.timeout_clocks : (1ll << 62);
-    const long long t0 = clock64();
-    while (sync_ld_acquire_sys(mine) != epoch) {
-      if (clock64() - t0 > limit) {
-        printf("seg_b200: SyncBN exchange timeout (rank %d waiting for rank %d, epoch %u; raise SEG_SYNC_TIMEOUT_S)\n", s.rank,
-               (int)threadIdx.x, epoch);
-        __trap();
-      }
-    }
-  }
-  __syncthreads();
-}
-
-// consumer, at the very end of the kernel (every thread of every block calls it): the last block to get here advances seq.
-// `done` = a zeroed uint32 owned by this launch.
-__device__ __forceinline__ void sync_consumer_done(const SyncDesc& s, uint32_t epoch, unsigned* done, unsigned nblocks) {
-  __syncthreads();  // every thread of this block has read its totals
-  if (threadIdx.x == 0) {
-    __threadfence();
-    if (atomicAdd(done, 1u) == nblocks - 1u) {
-      uint32_t* seq = reinterpret_cast<uint32_t*>(reinterpret_cast<char*>(s.peers[s.rank]) + sync_seq_offset(s.world, s.n_max));
-      *seq = epoch;
-      __threadfence();
-    }
-  }
+// producer epilogue for kernels that accumulate their per-channel totals with fp64 atomics into `acc` (n doubles): every
+// contributing block calls this with its `nthr` cooperating threads after issuing its atomics; the LAST of `nblocks` blocks to
+// arrive (ticket) turns the finished totals into the world's (sync_exchange_block_d).
+// kPrint = false: time out with a bare trap — no printf call, which would make ptxas serialise a caller's wgmma pipeline
+template <bool kPrint = true, class Sync>
+__device__ __forceinline__ void sync_push_when_last(const SyncDesc& s, double* acc, int n, unsigned* ticket, unsigned nblocks,
+                                                    int tid, int nthr, Sync sync, volatile int* sm_flag) {
+  __threadfence();
+  sync();
+  if (tid == 0) *sm_flag = (atomicAdd(ticket, 1u) == nblocks - 1u);
+  sync();
+  if (!*sm_flag) return;
+  __threadfence();
+  sync_exchange_block_d<kPrint>(s, acc, n, tid, nthr, sync);
 }
 
 }  // namespace seg

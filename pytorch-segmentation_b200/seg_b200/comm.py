@@ -4,8 +4,10 @@ NVLink peer buffers of the SyncBN statistics exchange.
 Replaces the reference's single-process nn.DataParallel + threaded SyncBN (base/base_trainer.py:33-38,
 utils/sync_batchnorm/batchnorm.py:105-126, comm.py): batch-dim sharding stays, the per-step parameter broadcast and logit gather
 disappear, and the two small collectives per BN layer ride inside the kernels that produce the statistics (csrc/seg_sync.cuh;
-`SyncBNGroup.desc` is the descriptor those kernels take).  The stand-alone exchange kernel (`allreduce_`, `seg_syncbn_exchange`)
-shares the buffers and the device-side sequence number, for callers outside the engine and for tests.
+`SyncBNGroup.desc` is the descriptor those kernels take): the producer's last block performs the whole exchange and leaves the
+world's totals in its output, so the kernels that consume them are the single-GPU ones.  The stand-alone exchange
+(`allreduce_`, `seg_syncbn_exchange`) is one block running the same protocol code with the same descriptor, for callers outside
+the engine.
 """
 import ctypes
 
@@ -22,16 +24,8 @@ def _sync_timeout_clocks():
     return int(float(os.environ.get("SEG_SYNC_TIMEOUT_S", "120")) * 2e9)
 
 
-def _sync_mode():
-    """1 (default): the producer kernel's last block performs the whole exchange (push, flags, wait, rank-ordered sum) and
-    leaves the world's totals in its output — ONE block polls the flags.  0: producers push, every block of the consumer kernel
-    (bn_apply / bn_bwd_apply) waits for the world and adds.  SEG_SYNC_MODE overrides (A/B measurements)."""
-    import os
-    return int(os.environ.get("SEG_SYNC_MODE", "1"))
-
-
 def _make_desc(peers, rank, world, n_max):
-    return lib.SyncDesc(peers.data_ptr(), rank, world, n_max, _sync_timeout_clocks(), _sync_mode())
+    return lib.SyncDesc(peers.data_ptr(), rank, world, n_max, _sync_timeout_clocks())
 
 
 class SyncBNGroup:
@@ -67,13 +61,12 @@ class SyncBNGroup:
             ptrs.append(p.value)
         self.peers = torch.tensor(ptrs, dtype=torch.int64, device="cuda")
         self.desc = _make_desc(self.peers, self.rank, self.world, n_max)
-        self.mode = self.desc.mode
         self.fused = True  # the kernels that produce / consume the statistics carry the exchange (csrc/seg_sync.cuh)
         dist.barrier(group=group)
 
     def allreduce_(self, vec):
         assert vec.dtype == torch.float32 and vec.is_contiguous() and vec.numel() <= self.n_max
-        lib.call("seg_syncbn_exchange", self.peers.data_ptr(), self.rank, self.world, vec.data_ptr(), vec.numel(), self.n_max)
+        lib.call("seg_syncbn_exchange", ctypes.addressof(self.desc), vec.data_ptr(), vec.numel())
         return vec
 
     def close(self):
@@ -97,13 +90,12 @@ class LocalLoopbackGroup:
         self._mine = mine
         self.peers = torch.tensor([mine.value], dtype=torch.int64, device="cuda")
         self.desc = _make_desc(self.peers, 0, 1, n_max)
-        self.mode = self.desc.mode
         self.fused = True
         self.force = False  # True: the engine runs the whole SyncBN protocol (push, flags, wait, sequence number) against
                             # this one-rank buffer — the single-GPU test of the fused exchange
 
     def allreduce_(self, vec):
-        lib.call("seg_syncbn_exchange", self.peers.data_ptr(), 0, 1, vec.data_ptr(), vec.numel(), self.n_max)
+        lib.call("seg_syncbn_exchange", ctypes.addressof(self.desc), vec.data_ptr(), vec.numel())
         return vec
 
 

@@ -324,13 +324,10 @@ class Tape:
                 if sync0 is not None:
                     self._pushed.add(stats.data_ptr())
             count = count_local
-            in_kernel = None
             if self.sync_active():
-                if stats.data_ptr() in self._pushed:
-                    if getattr(self.sync, "mode", 0) == 0:
-                        in_kernel = self.sync  # bn_apply waits for the world's flags and adds every rank's sums itself
-                    # mode 1: the producer's last block already did the exchange; `stats` holds the world's totals
-                else:  # exchange object without the in-kernel protocol (the gloo stand-in of the CPU tests): sums over ranks
+                # a producer called with sync= has already exchanged: `stats` holds the world's totals
+                if stats.data_ptr() not in self._pushed:
+                    # exchange object without the in-kernel protocol (the gloo stand-in of the CPU tests): sums over ranks
                     self.sync.allreduce_(stats)
                 count = count_local * self.sync.world
             # finalize (coefficients, saved mean / 1/std, running statistics) happens inside the apply kernel
@@ -339,8 +336,7 @@ class Tape:
                                          1 if (self.clamp_eps and self.sync is not None and self.sync.world > 1) else 0,
                                          bn.running_mean, bn.running_var, res=res.t if res is not None else None, out=out,
                                          relu=relu, drop_p=drop_p, seed=seed, step_ctr=self.step_ctr if drop_p > 0.0 else None,
-                                         drop_hw=drop_hw, sync=in_kernel,
-                                         sync_done=self.zalloc(1, y.t.device) if in_kernel is not None else None)
+                                         drop_hw=drop_hw)
             self.bn_modules.append(bn)
         else:
             ss, save = ops.bn_eval_scale_shift(bn.weight.detach(), bn.bias.detach(), bn.running_mean, bn.running_var, bn.eps,
@@ -385,20 +381,19 @@ class Tape:
                 elif count_local * C * 2 <= FUSED_BWD_MAX_BYTES:
                     # small maps (the operands stay in L2 between the phases): reduce -> grid barrier -> fixed-order cross-block
                     # sum (-> SyncBN exchange) -> apply in ONE cooperative launch.  Frozen BN (freeze_bn): dx = gamma*inv_std*dz,
-                    # the sums only feed the parameter gradients
+                    # the sums only feed the parameter gradients.  Its one ticket (seg_bn_bwd_fused_workspace) is the
+                    # grid-barrier counter
                     ops.bn_bwd_fused(da, a_mask, y.t, save, bn.weight.detach(), count, relu=relu, drop_p=drop_p, dgamma=dg, dbeta=db,
                                      accumulate=acc_pg, dx=dy, dres=dres, beta_res=beta_res, beta=bn.bias.detach(),
-                                     zero_sums=not use_batch_stats, tickets=self.zalloc(2, a.device), sync=sync)
+                                     zero_sums=not use_batch_stats, tickets=self.zalloc(1, a.device), sync=sync)
                 else:
                     # large maps stream from HBM in both passes anyway: two launches at full occupancy; under SyncBN the
-                    # reduction's last block pushes the sums and the apply pass waits for the world's
+                    # reduction's last block exchanges the sums, so the apply pass gets the world's
                     sums = ops.bn_bwd_reduce(da, a, y.t, save, relu=relu, drop_p=drop_p, dgamma=dg, dbeta=db, accumulate=acc_pg,
                                              acc=self.zalloc64(ops.bn_bwd_reduce_acc_words(C), a.device), sync=sync)
                     gsums = sums if use_batch_stats else torch.zeros_like(sums)
-                    csync = sync if (sync is not None and getattr(sync, "mode", 0) == 0) else None  # mode 1: sums are the world's
                     ops.bn_bwd_apply(da, a_mask, y.t, save, bn.weight.detach(), gsums, count, relu=relu, drop_p=drop_p, dx=dy,
-                                     dres=dres, beta_res=beta_res, beta=bn.bias.detach(), sync=csync,
-                                     sync_done=self.zalloc(1, a.device) if csync is not None else None)
+                                     dres=dres, beta_res=beta_res, beta=bn.bias.detach())
                 y.grad = dy
                 aa.grad = None
             self._push_back(bwd, (bn.weight, bn.bias))

@@ -21,8 +21,7 @@ LOSS_CE, LOSS_WCE, LOSS_FOCAL = 0, 1, 2  # SEG_LOSS_* (the `kind` of the seg_los
 class SyncDesc(Structure):
     """Mirror of ``seg_sync_desc`` (include/seg_b200.h)."""
 
-    _fields_ = [("peers", c_void_p), ("rank", c_int32), ("world", c_int32), ("n_max", c_int32), ("timeout_clocks", c_int64),
-                ("mode", c_int32)]
+    _fields_ = [("peers", c_void_p), ("rank", c_int32), ("world", c_int32), ("n_max", c_int32), ("timeout_clocks", c_int64)]
 
 
 class ConvDesc(Structure):
@@ -70,11 +69,11 @@ _SIGS = {
     "seg_counter_add": (c_int, [c_void_p, c_uint64, c_void_p]),
     "seg_bn_bwd_reduce_slots": (c_int, []),
     "seg_bn_bwd_reduce": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int64, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
-    "seg_bn_apply_train": (c_int, [c_void_p, c_int, c_void_p, c_double, c_void_p, c_void_p, c_float, c_float, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int64, c_int, c_int, c_float, c_uint64, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
+    "seg_bn_apply_train": (c_int, [c_void_p, c_int, c_void_p, c_double, c_void_p, c_void_p, c_float, c_float, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int64, c_int, c_int, c_float, c_uint64, c_void_p, c_int, c_void_p]),
     "seg_bn_bwd_fused_workspace": (c_int, [c_int64, c_int, POINTER(c_int64), POINTER(c_int64)]),
     "seg_bn_bwd_fused": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_double, c_int64, c_int, c_int, c_float,
                                  c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_float, c_int, c_void_p, c_void_p]),
-    "seg_bn_bwd_apply": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_double, c_int64, c_int, c_int, c_float, c_void_p, c_int, c_void_p, c_int, c_float, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "seg_bn_bwd_apply": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_double, c_int64, c_int, c_int, c_float, c_void_p, c_int, c_void_p, c_int, c_float, c_void_p, c_void_p]),
     "seg_bn_param_grad": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p]),
     "seg_maxpool3x3s2_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "seg_maxpool3x3s2_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
@@ -105,7 +104,7 @@ _SIGS = {
     "seg_comm_ipc_get": (c_int, [c_void_p, c_void_p]),
     "seg_comm_ipc_open": (c_int, [c_void_p, POINTER(c_void_p)]),
     "seg_comm_ipc_close": (c_int, [c_void_p]),
-    "seg_syncbn_exchange": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_void_p]),
+    "seg_syncbn_exchange": (c_int, [c_void_p, c_void_p, c_int, c_void_p]),
     "seg_sgd_step": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_float, c_float, c_int, c_float, c_void_p]),
     "seg_aug_entry_bytes": (c_int, []),
     "seg_augment_batch_u8": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, POINTER(c_float), POINTER(c_float), c_void_p, c_void_p, c_void_p]),

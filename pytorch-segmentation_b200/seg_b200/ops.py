@@ -104,7 +104,7 @@ def new_stats(C, device):
 
 
 def _sync_args(sync, ticket, device):
-    """(desc pointer, ticket pointer, ticket tensor kept alive) for a SyncBN producer / consumer call."""
+    """(desc pointer, ticket pointer, ticket tensor kept alive) for a SyncBN producer call."""
     if sync is None:
         return None, None, None
     if ticket is None:
@@ -280,8 +280,8 @@ def bn_bwd_reduce(dout, out, x, save, relu=True, drop_p=0.0, dgamma=None, dbeta=
                   gamma=None, beta=None, sync=None):
     """Returns sums fp32 [2C] = (sum dz, sum dz*xhat); optionally writes the parameter gradients from them.  One launch: fp64
     atomics into `acc` (exact, bit-reproducible), the last block rounds / writes.  acc: zeroed fp64 [bn_bwd_reduce_acc_words(C)]
-    (accumulator copies + ticket) from the caller's arena, allocated here if None.  sync: SyncBN — the last block pushes the sums to the peers (the
-    consumer is bn_bwd_apply(sync=...)).
+    (accumulator copies + ticket) from the caller's arena, allocated here if None.  sync: SyncBN — the last block exchanges the sums with the
+    peers and the returned sums are the world's.
     out=None (with relu, gamma, beta): the ReLU mask is recomputed from x instead of read from the stored activation."""
     C = x.shape[-1]
     M = rows(x)
@@ -298,34 +298,28 @@ def bn_bwd_reduce(dout, out, x, save, relu=True, drop_p=0.0, dgamma=None, dbeta=
 
 
 def bn_apply_train(x, stats, count, gamma, beta, eps, momentum, clamp_eps, running_mean, running_var, res=None, out=None,
-                   relu=True, drop_p=0.0, seed=0, step_ctr=None, drop_hw=0, sync=None, sync_done=None):
+                   relu=True, drop_p=0.0, seed=0, step_ctr=None, drop_hw=0):
     """Training-mode BN (+residual, ReLU, dropout) straight from the batch sums.  Returns (out, save[2C]).
-    sync (comm.SyncBNGroup, with the producing conv2d_fwd(sync=...)): the kernel waits for the world's flags and adds every
-    rank's sums itself; `count` is the world's; sync_done: one zeroed word (allocated here if None)."""
+    Under SyncBN the producer called with sync= has left the world's sums in `stats`; `count` is then the world's."""
     C = x.shape[-1]
     if out is None:
         out = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
     save = torch.empty(2 * C, dtype=torch.float32, device=x.device)
     assert stats.dtype == torch.float64
-    if sync is not None and sync_done is None:
-        sync_done = torch.zeros(1, dtype=torch.float32, device=x.device)
     call("seg_bn_apply_train", ptr(x), ld(x), ptr(stats), float(count), ptr(gamma), ptr(beta), float(eps), float(momentum),
          int(clamp_eps), ptr(running_mean), ptr(running_var), ptr(save), ptr(res), ld(res) if res is not None else 0,
          ptr(out), ld(out), rows(x), C, int(relu), float(drop_p), int(seed), ptr(step_ctr), int(drop_hw),
-         ctypes.addressof(sync.desc) if sync is not None else None, ptr(sync_done) if sync is not None else None,
          meta=_meta_rows(rows(x), C, 3 if res is not None else 2, res is not None))
     return out, save
 
 
-def bn_bwd_apply(dout, out, x, save, gamma, sums, count, relu=True, drop_p=0.0, dx=None, dres=None, beta_res=0.0, beta=None,
-                 sync=None, sync_done=None):
+def bn_bwd_apply(dout, out, x, save, gamma, sums, count, relu=True, drop_p=0.0, dx=None, dres=None, beta_res=0.0, beta=None):
     C = x.shape[-1]
     if dx is None:
         dx = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
-    sp, tp, _keep = _sync_args(sync, sync_done, x.device)
     call("seg_bn_bwd_apply", ptr(dout), ld(dout), ptr(out), ld(out) if out is not None else 0, ptr(x), ld(x), ptr(save),
          ptr(gamma), ptr(sums), float(count), rows(x), C, int(relu), float(drop_p), ptr(dx), ld(dx), ptr(dres),
-         ld(dres) if dres is not None else 0, float(beta_res), ptr(beta), sp, tp,
+         ld(dres) if dres is not None else 0, float(beta_res), ptr(beta),
          meta=_meta_rows(rows(x), C, (3 if (relu and out is not None) else 2) + 1 + (0 if dres is None else (2 if beta_res != 0.0 else 1)), dres is not None))
     return dx
 
@@ -344,7 +338,8 @@ def bn_bwd_fused_workspace(M, C):
 def bn_bwd_fused(dout, out, x, save, gamma, count_total, relu=True, drop_p=0.0, dgamma=None, dbeta=None, accumulate=False,
                  dx=None, dres=None, beta_res=0.0, beta=None, zero_sums=False, tickets=None, sync=None):
     """BatchNorm backward in ONE cooperative launch (reduce -> grid barrier -> fixed-order cross-block sum [-> SyncBN exchange]
-    -> apply).  Returns (dx, local sums [2C]).  out=None: ReLU mask recomputed from x (needs beta).  tickets: 2 zeroed words."""
+    -> apply).  Returns (dx, sums [2C]: the world's under sync).  out=None: ReLU mask recomputed from x (needs beta).  tickets:
+    bn_bwd_fused_workspace(M, C)[1] zeroed words."""
     C = x.shape[-1]
     M = rows(x)
     if dx is None:

@@ -195,7 +195,7 @@ def bn_apply(x, ss, res=None, out=None, relu=True, drop_p=0.0, seed=0, step_ctr=
 
 
 def bn_apply_train(x, stats, count, gamma, beta, eps, momentum, clamp_eps, running_mean, running_var, res=None, out=None,
-                   relu=True, drop_p=0.0, seed=0, step_ctr=None, drop_hw=0, sync=None, sync_done=None):
+                   relu=True, drop_p=0.0, seed=0, step_ctr=None, drop_hw=0):
     ss, save = bn_finalize(stats, count, gamma, beta, eps, momentum, clamp_eps, running_mean, running_var)
     return bn_apply(x, ss, res=res, out=out, relu=relu, drop_p=drop_p, seed=seed, step_ctr=step_ctr), save
 
@@ -226,8 +226,7 @@ def bn_bwd_reduce(dout, out, x, save, relu=True, drop_p=0.0, dgamma=None, dbeta=
     return sums
 
 
-def bn_bwd_apply(dout, out, x, save, gamma, sums, count, relu=True, drop_p=0.0, dx=None, dres=None, beta_res=0.0, beta=None,
-                 sync=None, sync_done=None):
+def bn_bwd_apply(dout, out, x, save, gamma, sums, count, relu=True, drop_p=0.0, dx=None, dres=None, beta_res=0.0, beta=None):
     C = x.shape[-1]
     dz = _dz(dout, out, relu, drop_p, x, save, gamma, beta)
     xhat = (x.float() - save[:C]) * save[C:]

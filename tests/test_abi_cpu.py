@@ -50,6 +50,7 @@ def test_python_binding_matches_header(cdll):
 def test_conv_desc_layout_matches_header():
     from seg_b200 import lib
     assert ctypes.sizeof(lib.ConvDesc) == 14 * 4
+    assert ctypes.sizeof(lib.SyncDesc) == 32  # pointer, three int32, padding, int64: static_assert'ed in csrc/seg_comm.cu
     d = lib.make_conv_desc(2, 33, 33, 2048, 256, 3, 3, 1, 18, 18)
     assert (d.P, d.Q) == (33, 33)
     d = lib.make_conv_desc(1, 513, 513, 3, 64, 7, 7, 2, 3, 1)

@@ -2,16 +2,15 @@
 a one-GPU box cannot exercise and whose mistakes show up as rare corruption, not as a failing unit test.
 
 The model transcribes the protocol onto W abstract ranks.  Each rank owns a symmetric buffer `data[2][W] | flags[2][W] | seq`
-and runs, for every exchange of the step (all ranks issue the same exchanges in the same order):
+and runs, for every exchange of the step (all ranks issue the same exchanges in the same order), in ONE block
+(seg_sync.cuh::sync_exchange_block_*, which the producers' last block and the stand-alone seg_syncbn_exchange both run):
     epoch = seq + 1;  slot = epoch & 1
     push   : store my vector into data[slot][me] of EVERY peer        (one store per peer = one schedulable event)
     publish: store `epoch` into flags[slot][me] of EVERY peer          (after the pushes: fence + release store)
     wait   : spin until flags[slot][p] == epoch for every p in MY buffer
     total  : read data[slot][p] for every p from MY buffer, add in rank order
     advance: seq = epoch
-mode 1 = all five inside the producer kernel's last block (seg_sync.cuh::sync_exchange_block_*); mode 0 = push + publish in the
-producer kernel, wait + total by several consumer blocks, the last of which advances (sync_push_when_last / sync_wait_world /
-sync_consumer_done).  Between exchanges a rank does an arbitrary amount of unrelated work, so ranks drift apart.
+Between exchanges a rank does an arbitrary amount of unrelated work, so ranks drift apart.
 
 Events are interleaved by a seeded random scheduler (sequentially consistent: the memory-ordering side — who fences, release /
 acquire at system scope — is argued in the header, the LOGIC is what is checked here).  On every schedule:
@@ -46,7 +45,7 @@ def epoch_of(seq):
     return 2 if e == 0 else e  # flags start at 0: skip it on wrap-around, keeping the parity alternation (sync_epoch)
 
 
-def rank_program(me, ranks, n_exchanges, payload, mode, consumers, rng, bug):
+def rank_program(me, ranks, n_exchanges, payload, rng, bug):
     """Generator: one yield per externally visible memory event, so the scheduler can interleave ranks between any two."""
     W = len(ranks)
     mine = ranks[me]
@@ -74,50 +73,40 @@ def rank_program(me, ranks, n_exchanges, payload, mode, consumers, rng, bug):
         if bug != "flag_before_data":
             yield from raise_flags()
 
-        # ---- wait + total (+ advance): mode 1 = this block; mode 0 = `consumers` blocks of the next kernel, in any order
-        blocks = 1 if mode == 1 else consumers
-        left = blocks
-        pending = list(range(blocks))
-        rng.shuffle(pending)
-        results = []
-        for b in pending:
-            if bug == "advance_early" and b == pending[0]:
-                mine.seq = epoch  # before anyone has read
-            spins = 0
-            for p in range(W):
-                while True:
-                    f = mine.flags[slot][p]
-                    ok = (f >= epoch) if bug == "ge_compare" else (f == epoch)
-                    if ok:
-                        break
-                    spins += 1
-                    if spins > 200000:
-                        raise Violation(f"rank {me} starved waiting for rank {p} at exchange {x} (flag {f}, epoch {epoch})")
-                    yield "spin"
-            mine.reading = slot
-            tot = 0.0
-            for p in range(W):
-                yield "read"
-                v = mine.data[slot][p]
-                if v is None or v[0] != x or v[1] != p:
-                    raise Violation(f"rank {me} read {v} from slot {slot} while summing exchange {x}, rank {p}")
-                tot += v[2]
-            results.append(tot)
-            left -= 1
-            if left == 0:
-                mine.reading = None
-                if bug != "advance_early":
-                    mine.seq = epoch
-                yield "advance"
-        assert all(r == results[0] for r in results)
-        mine.totals.append(results[0])
+        # ---- wait + total + advance, by the same block
+        if bug == "advance_early":
+            mine.seq = epoch  # before anyone has read
+        spins = 0
+        for p in range(W):
+            while True:
+                f = mine.flags[slot][p]
+                ok = (f >= epoch) if bug == "ge_compare" else (f == epoch)
+                if ok:
+                    break
+                spins += 1
+                if spins > 200000:
+                    raise Violation(f"rank {me} starved waiting for rank {p} at exchange {x} (flag {f}, epoch {epoch})")
+                yield "spin"
+        mine.reading = slot
+        tot = 0.0
+        for p in range(W):
+            yield "read"
+            v = mine.data[slot][p]
+            if v is None or v[0] != x or v[1] != p:
+                raise Violation(f"rank {me} read {v} from slot {slot} while summing exchange {x}, rank {p}")
+            tot += v[2]
+        mine.reading = None
+        if bug != "advance_early":
+            mine.seq = epoch
+        yield "advance"
+        mine.totals.append(tot)
         mine.done = x + 1
         lead = mine.done - min(r.done for r in ranks)
         if lead > 1 and bug is None:
             raise Violation(f"rank {me} is {lead} exchanges ahead of the slowest peer")
 
 
-def run(world, n_exchanges, mode, seed, bug=None, consumers=3, seq0=0):
+def run(world, n_exchanges, seed, bug=None, seq0=0):
     rng = random.Random(seed)
     ranks = [Rank(world) for _ in range(world)]
     for r in ranks:
@@ -126,7 +115,7 @@ def run(world, n_exchanges, mode, seed, bug=None, consumers=3, seq0=0):
     def payload(x, rank):
         return float((x * 131 + rank * 17) % 1009) + 0.25 * rank
 
-    progs = [rank_program(i, ranks, n_exchanges, payload, mode, consumers, random.Random(seed * 977 + i), bug) for i in range(world)]
+    progs = [rank_program(i, ranks, n_exchanges, payload, random.Random(seed * 977 + i), bug) for i in range(world)]
     alive = list(range(world))
     # a biased scheduler: now and then one rank is held back for a long stretch (a slow data loader, a checkpoint write)
     held, hold_left = None, 0
@@ -153,19 +142,20 @@ def run(world, n_exchanges, mode, seed, bug=None, consumers=3, seq0=0):
     return ranks
 
 
-@pytest.mark.parametrize("mode", [1, 0])
+# seq0: a fresh buffer, and a sequence number whose epoch wraps past 2^32 at the 12th of the 24 exchanges
+@pytest.mark.parametrize("seq0", [0, 0xFFFFFFF4], ids=["fresh", "wrap"])
 @pytest.mark.parametrize("world", [1, 2, 3, 8])
-def test_exchange_protocol_is_safe_under_random_interleavings(world, mode):
+def test_exchange_protocol_is_safe_under_random_interleavings(world, seq0):
     for seed in range(40 if world < 8 else 12):
-        run(world, 24, mode, seed)
+        run(world, 24, seed, seq0=seq0)
 
 
 def test_epoch_wraparound_keeps_parity_and_skips_zero():
     # seq close to 2^32: epochs ... fffffffe, ffffffff, (0 skipped ->) 2, 3 ...; the flag value 0 (initial state) is never used
     assert epoch_of(0xFFFFFFFE) == 0xFFFFFFFF and epoch_of(0xFFFFFFFF) == 2 and epoch_of(2) == 3
     for seed in range(10):
-        run(2, 6, 1, seed, seq0=0xFFFFFFFC)
-        run(3, 6, 0, seed, seq0=0xFFFFFFFD)
+        run(2, 6, seed, seq0=0xFFFFFFFC)
+        run(3, 6, seed, seq0=0xFFFFFFFD)
 
 
 @pytest.mark.parametrize("bug", ["one_slot", "flag_before_data", "ge_compare"])
@@ -173,16 +163,16 @@ def test_seeded_protocol_mistakes_are_caught(bug):
     caught = 0
     for seed in range(60):
         try:
-            run(3, 24, 1, seed, bug=bug, seq0=0xFFFFFFF0 if bug == "ge_compare" else 0)
+            run(3, 24, seed, bug=bug, seq0=0xFFFFFFF0 if bug == "ge_compare" else 0)
         except (Violation, AssertionError):
             caught += 1
     assert caught > 0, f"the model did not notice the seeded mistake '{bug}'"
 
 
 def test_slot_safety_rests_on_the_flag_dependency_not_on_advance_order():
-    """Advancing seq BEFORE the totals are read (mode 1, one block) does not break the two-slot scheme: the next-but-one
+    """Advancing seq BEFORE the totals are read does not break the two-slot scheme: the next-but-one
     exchange — the first that reuses the slot — still needs every peer's flag of the next one, which a peer raises only after
     it has finished reading.  The model documents that it is this dependency, not the advance-after-read order, that protects
     the slot (so the single `__threadfence(); sync(); advance` tail of sync_exchange_block_* is not load-bearing for safety)."""
     for seed in range(20):
-        run(3, 16, 1, seed, bug="advance_early")
+        run(3, 16, seed, bug="advance_early")

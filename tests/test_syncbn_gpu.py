@@ -1,6 +1,8 @@
-"""SyncBN one-shot exchange kernel (seg_syncbn_exchange): single-GPU loopback, two simulated ranks on one GPU (two
-streams, two symmetric buffers), and — when the box has >= 2 GPUs — a real 2-process run over CUDA IPC / NVLink peer
-memory checked against the single-process concatenated batch (the property of sync_batchnorm/batchnorm.py:160-167)."""
+"""SyncBN exchange: the stand-alone seg_syncbn_exchange (one block running the protocol code of csrc/seg_sync.cuh that the
+statistics producers run in their last block) on a single-GPU loopback and on two simulated ranks on one GPU (two streams,
+two symmetric buffers); the in-kernel exchange on a one-rank loopback; and — when the box has >= 2 GPUs — a real 2-process
+run over CUDA IPC / NVLink peer memory checked against the single-process concatenated batch (the property of
+sync_batchnorm/batchnorm.py:160-167)."""
 import ctypes
 import os
 import sys
@@ -32,21 +34,26 @@ def test_loopback_world1():
         assert torch.equal(v, ref)
 
 
-def test_two_simulated_ranks_on_one_gpu():
+def test_two_simulated_ranks_exchange_through_the_sync_handle():
+    """seg_syncbn_exchange with one seg_sync_desc per rank: the exchange code of the statistics producers, on two streams."""
     L = lib.load()
     n_max = 4096
     bufs = [_alloc(2, n_max), _alloc(2, n_max)]
     peers = torch.tensor([b.value for b in bufs], dtype=torch.int64, device="cuda")
+    descs = [comm._make_desc(peers, r, 2, n_max) for r in (0, 1)]
     streams = [torch.cuda.Stream(), torch.cuda.Stream()]
     torch.cuda.synchronize()
+    # the handle is read on the host: a device address in its place is refused before anything is launched
+    probe = torch.zeros(64, device="cuda")
+    assert L.seg_syncbn_exchange(peers.data_ptr(), probe.data_ptr(), 64, None) != 0
+    assert "host memory" in lib.last_error()
     for epoch, n in enumerate((128, 2048, 4096, 64), start=1):
         vals = [torch.randn(n, device="cuda"), torch.randn(n, device="cuda")]
         expect = vals[0] + vals[1]
         torch.cuda.synchronize()
         for r in (0, 1):
             with torch.cuda.stream(streams[r]):
-                rc = L.seg_syncbn_exchange(peers.data_ptr(), r, 2, vals[r].data_ptr(), n, n_max,
-                                           streams[r].cuda_stream)
+                rc = L.seg_syncbn_exchange(ctypes.byref(descs[r]), vals[r].data_ptr(), n, streams[r].cuda_stream)
                 assert rc == 0, lib.last_error()
         torch.cuda.synchronize()
         assert torch.equal(vals[0], vals[1]), "ranks must end with bit-identical sums"
@@ -56,8 +63,8 @@ def test_two_simulated_ranks_on_one_gpu():
 
 
 def test_fused_exchange_protocol_on_a_one_rank_loopback():
-    """The SyncBN exchange now rides inside the conv epilogue (push + flags), bn_apply (wait + rank-ordered sum) and the
-    cooperative BN backward (both): run the WHOLE protocol — symmetric-buffer stores, release flags, acquire waits, device-side
+    """The SyncBN exchange rides inside the kernels that produce the statistics (conv epilogue, BN backward reduction, the
+    cooperative BN backward), whose last block runs it from push to advance: run the WHOLE protocol — symmetric-buffer stores, release flags, acquire waits, device-side
     sequence number, slot alternation — against a one-rank buffer.  With one rank the sums are unchanged, so three training
     steps must be bit-identical to the same steps without an exchange, eagerly and replayed from a CUDA graph."""
     import seg_b200
