@@ -222,6 +222,20 @@ int seg_bilinear_logits_fwd(const float* x, float* y_nchw, int N, int Hi, int Wi
 int seg_bilinear_logits_bwd(const float* dy_nchw, void* dx, int lddx, int N, int Hi, int Wi, int Ho, int Wo, int C,
                             int align_corners, void* stream);
 
+/* ---- pixel shuffle, nn.PixelShuffle(r) (duc_hdc.py:22,30) ---- */
+/* NHWC bf16 x [N,H,W,r*r*C] (pitch ldx) -> NHWC bf16 y [N,Ho,Wo,C] (pitch ldy; a channel slice is allowed), cropped to
+ * Ho <= r*H, Wo <= r*W: y[n,oy,ox,c] = x[n, oy/r, ox/r, c*r*r + (oy%r)*r + ox%r].  Replaces the DUC block's shuffle and the
+ * decoder's crop x[:, :, :Hl, :Wl] (duc_hdc.py:30,206), writing straight into the decoder's concat buffer.  Exact. */
+int seg_pixel_shuffle_fwd(const void* x, int ldx, void* y, int ldy, int N, int H, int W, int C, int r, int Ho, int Wo,
+                          void* stream);
+/* dx = beta*dx + shuffle^T(dy) over all r*r*C channels of dx; source positions the crop dropped get zero */
+int seg_pixel_shuffle_bwd(const void* dy, int lddy, void* dx, int lddx, int N, int H, int W, int C, int r, int Ho, int Wo,
+                          float beta, void* stream);
+/* final logits of DeepLab_DUC_HDC (duc_hdc.py:233): NHWC bf16 [N,h,w,r*r*C] (pitch ldx) -> NCHW fp32 [N,C,r*h,r*w] */
+int seg_pixel_shuffle_logits_fwd(const void* x, int ldx, float* y_nchw, int N, int h, int w, int C, int r, void* stream);
+/* NCHW fp32 grad -> NHWC bf16 grad [N,h,w,lddx] (channels r*r*C .. lddx-1 zero) */
+int seg_pixel_shuffle_logits_bwd(const float* dy_nchw, void* dx, int lddx, int N, int h, int w, int C, int r, void* stream);
+
 /* ---- per-pixel loss ---- */
 /* Cross-entropy, class-weighted cross-entropy and focal loss, one family of entry points with the loss picked by `kind`:
  * CrossEntropyLoss2d(weight, reduction) (utils/losses.py:24-31), FocalLoss(gamma, alpha, size_average) (:52-65) and the
@@ -271,6 +285,18 @@ int seg_upsample_loss_bwd(const float* logits_lo, const int64_t* target, int N, 
                           int align_corners, int64_t ignore_index, const float* weight, int kind, float gamma, int mean,
                           const double* accum, const float* gscale, float* dlo_f32, void* dlo_fixed, void* dx, int lddx,
                           void* stream);
+/* The same losses fused with the pixel shuffle of DeepLab_DUC_HDC's output (duc_hdc.py:233 + trainer.py:60): the logits
+ * are the nn.PixelShuffle(r) view of the low-res NHWC bf16 map [N,h,w,r*r*C] (pitch ldlo, C <= 160), read in place, and
+ * target is int64 [N, r*h, r*w].  kind, weight, gamma, mean, accum, gscale and counters as for seg_upsample_loss_*; the
+ * prediction is the arg-max of the values seg_pixel_shuffle_logits_fwd produces (lowest index wins ties).
+ * Backward: every low-res element belongs to exactly one pixel, so dx (bf16 [N,h,w,lddx], channels r*r*C .. lddx-1 zero) is
+ * written directly, once per element: deterministic, no scratch. */
+int seg_shuffle_loss_fwd(const void* logits_lo, int ldlo, const int64_t* target, int N, int h, int w, int C, int r,
+                         int64_t ignore_index, const float* weight, int kind, float gamma, double* accum, int64_t* counters,
+                         void* stream);
+int seg_shuffle_loss_bwd(const void* logits_lo, int ldlo, const int64_t* target, int N, int h, int w, int C, int r,
+                         int64_t ignore_index, const float* weight, int kind, float gamma, int mean, const double* accum,
+                         const float* gscale, void* dx, int lddx, void* stream);
 /* DiceLoss (utils/losses.py:33-50): softmax over C, intersection with the one-hot target, whole-batch ratio.
  * accum (fp64 [2], zeroed by the caller) receives (sum p[target], #pixels); loss = 1 - (2I+s)/(2*#pixels+s).
  * The caller applies the reference's in-place target fix-up (losses.py:40-42) before calling. */

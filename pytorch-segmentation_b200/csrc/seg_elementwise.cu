@@ -1160,6 +1160,86 @@ __global__ void __launch_bounds__(128) bilinear_logits_bwd_kernel(const float* _
   }
 }
 
+// ------------------------------------------------------------------ pixel shuffle (nn.PixelShuffle, duc_hdc.py:22,30)
+// Source channel of output (c, oy, ox) is c*r*r + (oy % r)*r + (ox % r) at source pixel (oy / r, ox / r).  Pure
+// permutations: every output is one input element, so the results are exact.
+__global__ void __launch_bounds__(256) pixel_shuffle_fwd_kernel(const __nv_bfloat16* __restrict__ x, int ldx,
+                                                                __nv_bfloat16* __restrict__ y, int ldy, int N, int H, int W,
+                                                                int C, int r, int Ho, int Wo) {
+  const int64_t total = (int64_t)N * Ho * Wo * C;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int c = (int)(i % C);
+    int64_t t = i / C;
+    const int ox = (int)(t % Wo);
+    t /= Wo;
+    const int oy = (int)(t % Ho);
+    const int n = (int)(t / Ho);
+    const int sc = (c * r + oy % r) * r + ox % r;
+    y[(((int64_t)n * Ho + oy) * Wo + ox) * ldy + c] = x[(((int64_t)n * H + oy / r) * W + ox / r) * ldx + sc];
+  }
+}
+
+// dx = beta*dx + shuffle^T(dy); source positions the crop dropped get a zero gradient
+__global__ void __launch_bounds__(256) pixel_shuffle_bwd_kernel(const __nv_bfloat16* __restrict__ dy, int lddy,
+                                                                __nv_bfloat16* __restrict__ dx, int lddx, int N, int H, int W,
+                                                                int C, int r, int Ho, int Wo, float beta) {
+  const int Cr = C * r * r;
+  const int64_t total = (int64_t)N * H * W * Cr;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int sc = (int)(i % Cr);
+    int64_t t = i / Cr;
+    const int w = (int)(t % W);
+    t /= W;
+    const int h = (int)(t % H);
+    const int n = (int)(t / H);
+    const int c = sc / (r * r), oy = h * r + (sc / r) % r, ox = w * r + sc % r;
+    float v = 0.f;
+    if (oy < Ho && ox < Wo) v = bf2f(dy[(((int64_t)n * Ho + oy) * Wo + ox) * lddy + c]);
+    __nv_bfloat16* o = dx + (((int64_t)n * H + h) * W + w) * lddx + sc;
+    if (beta != 0.f) v += beta * bf2f(*o);
+    *o = f2bf(v);
+  }
+}
+
+// low-res NHWC bf16 [N,h,w,r*r*C] -> full-res NCHW fp32 [N,C,r*h,r*w]; threads run along ox for coalesced NCHW stores
+__global__ void __launch_bounds__(256) pixel_shuffle_logits_fwd_kernel(const __nv_bfloat16* __restrict__ x, int ldx,
+                                                                       float* __restrict__ y, int N, int h, int w, int C,
+                                                                       int r) {
+  const int Ho = h * r, Wo = w * r;
+  const int64_t total = (int64_t)N * C * Ho * Wo;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int ox = (int)(i % Wo);
+    int64_t t = i / Wo;
+    const int oy = (int)(t % Ho);
+    t /= Ho;
+    const int c = (int)(t % C);
+    const int n = (int)(t / C);
+    y[i] = bf2f(x[(((int64_t)n * h + oy / r) * w + ox / r) * ldx + (c * r + oy % r) * r + ox % r]);
+  }
+}
+
+// NCHW fp32 grad -> low-res NHWC bf16 grad (pitch lddx, channels >= r*r*C zero-filled up to lddx)
+__global__ void __launch_bounds__(256) pixel_shuffle_logits_bwd_kernel(const float* __restrict__ dy,
+                                                                       __nv_bfloat16* __restrict__ dx, int lddx, int N, int h,
+                                                                       int w, int C, int r) {
+  const int Cr = C * r * r, Ho = h * r, Wo = w * r;
+  const int64_t total = (int64_t)N * h * w * lddx;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int sc = (int)(i % lddx);
+    int64_t t = i / lddx;
+    const int x0 = (int)(t % w);
+    t /= w;
+    const int y0 = (int)(t % h);
+    const int n = (int)(t / h);
+    float v = 0.f;
+    if (sc < Cr) {
+      const int c = sc / (r * r), oy = y0 * r + (sc / r) % r, ox = x0 * r + sc % r;
+      v = dy[(((int64_t)n * C + c) * Ho + oy) * Wo + ox];
+    }
+    dx[i] = f2bf(v);
+  }
+}
+
 // ------------------------------------------------------------------ misc
 __global__ void nhwc_to_nchw_kernel(const void* __restrict__ x, int ldx, int x_dtype, float* __restrict__ y, int N, int H,
                                     int W, int C) {
@@ -1537,6 +1617,37 @@ int seg_bilinear_logits_bwd(const float* dy, void* dx, int lddx, int N, int Hi, 
       dy, BF(dx), lddx, N, Hi, Wi, Ho, Wo, C, align_corners, resize_scale(Hi, Ho, align_corners),
       resize_scale(Wi, Wo, align_corners));
   return check_launch("bilinear_logits_bwd");
+}
+
+int seg_pixel_shuffle_fwd(const void* x, int ldx, void* y, int ldy, int N, int H, int W, int C, int r, int Ho, int Wo,
+                          void* stream) {
+  SEG_REQUIRE(N > 0 && H > 0 && W > 0 && C > 0 && r >= 1, "pixel_shuffle: bad sizes");
+  SEG_REQUIRE(Ho >= 1 && Ho <= r * H && Wo >= 1 && Wo <= r * W, "pixel_shuffle: crop %dx%d outside %dx%d", Ho, Wo, r * H, r * W);
+  SEG_REQUIRE(ldx >= C * r * r && ldy >= C, "pixel_shuffle: pitch smaller than channel count");
+  pixel_shuffle_fwd_kernel<<<grid_for((int64_t)N * Ho * Wo * C, 256), 256, 0, ST(stream)>>>(CBF(x), ldx, BF(y), ldy, N, H, W, C,
+                                                                                              r, Ho, Wo);
+  return check_launch("pixel_shuffle_fwd");
+}
+int seg_pixel_shuffle_bwd(const void* dy, int lddy, void* dx, int lddx, int N, int H, int W, int C, int r, int Ho, int Wo,
+                          float beta, void* stream) {
+  SEG_REQUIRE(N > 0 && H > 0 && W > 0 && C > 0 && r >= 1, "pixel_shuffle: bad sizes");
+  SEG_REQUIRE(Ho >= 1 && Ho <= r * H && Wo >= 1 && Wo <= r * W, "pixel_shuffle: crop %dx%d outside %dx%d", Ho, Wo, r * H, r * W);
+  SEG_REQUIRE(lddx >= C * r * r && lddy >= C, "pixel_shuffle: pitch smaller than channel count");
+  pixel_shuffle_bwd_kernel<<<grid_for((int64_t)N * H * W * C * r * r, 256), 256, 0, ST(stream)>>>(CBF(dy), lddy, BF(dx), lddx, N,
+                                                                                                   H, W, C, r, Ho, Wo, beta);
+  return check_launch("pixel_shuffle_bwd");
+}
+int seg_pixel_shuffle_logits_fwd(const void* x, int ldx, float* y_nchw, int N, int h, int w, int C, int r, void* stream) {
+  SEG_REQUIRE(N > 0 && h > 0 && w > 0 && C > 0 && r >= 1 && ldx >= C * r * r, "pixel_shuffle_logits: bad sizes");
+  pixel_shuffle_logits_fwd_kernel<<<grid_for((int64_t)N * C * h * w * r * r, 256), 256, 0, ST(stream)>>>(CBF(x), ldx, y_nchw, N, h,
+                                                                                                          w, C, r);
+  return check_launch("pixel_shuffle_logits_fwd");
+}
+int seg_pixel_shuffle_logits_bwd(const float* dy_nchw, void* dx, int lddx, int N, int h, int w, int C, int r, void* stream) {
+  SEG_REQUIRE(N > 0 && h > 0 && w > 0 && C > 0 && r >= 1 && lddx >= C * r * r, "pixel_shuffle_logits: bad sizes");
+  pixel_shuffle_logits_bwd_kernel<<<grid_for((int64_t)N * h * w * lddx, 256), 256, 0, ST(stream)>>>(dy_nchw, BF(dx), lddx, N, h,
+                                                                                                     w, C, r);
+  return check_launch("pixel_shuffle_logits_bwd");
 }
 
 int seg_nhwc_to_nchw_f32(const void* x, int ldx, int x_dtype, float* y, int N, int H, int W, int C, void* stream) {

@@ -403,6 +403,109 @@ __global__ void ce_grad_from_fixed_kernel(const unsigned long long* __restrict__
     dlo[i] = (float)((double)(long long)acc[i] * inv);
 }
 
+// ---------------------------------------------------------------- fused pixel shuffle + loss (duc_hdc.py:30,233)
+// The logits of full-resolution pixel (oy, ox) are read in place from the low-resolution bf16 map as its nn.PixelShuffle(r)
+// view: class c sits at channel c*r*r + (oy % r)*r + ox % r of low-res pixel (oy / r, ox / r).  One thread per pixel.  Every
+// low-res element belongs to exactly one pixel, so the backward writes each gradient element once (no accumulation: the
+// result does not depend on the thread order) and zeroes the pad lanes r*r*C .. lddx-1.  MET: the eval_metrics counters,
+// counted as upsample_ce_kernel counts them (shared-memory histogram, one global atomic per non-zero bin).
+template <bool BWD, int K, bool MET = false>
+__global__ void __launch_bounds__(256) shuffle_ce_kernel(const __nv_bfloat16* __restrict__ lo, int ldlo,
+                                                         const int64_t* __restrict__ target, int N, int h, int w, int C, int r,
+                                                         int64_t ignore, LossArgs la, double* accum,
+                                                         const float* __restrict__ gscale, __nv_bfloat16* __restrict__ dx,
+                                                         int lddx, unsigned long long* __restrict__ counters) {
+  extern __shared__ unsigned int hist[];  // MET: [2 + 3C], as counters
+  if (MET) {
+    for (int i = threadIdx.x; i < 3 * C + 2; i += blockDim.x) hist[i] = 0u;
+    __syncthreads();
+  }
+  const int Ho = h * r, Wo = w * r, rr = r * r;
+  const int64_t total = (int64_t)N * Ho * Wo;
+  double loss = 0.0, cnt = 0.0;
+  unsigned int n_correct = 0u, n_labeled = 0u;
+  const float g = BWD ? loss_grad_g<K>(gscale, accum, la.mean) : 0.f;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int ox = (int)(i % Wo);
+    const int64_t t = i / Wo;
+    const int oy = (int)(t % Ho);
+    const int n = (int)(t / Ho);
+    const int64_t tg = target[i];
+    const bool valid = tg != ignore;
+    const bool labeled = MET && tg >= 0 && tg < C;
+    if (K == LOSS_FOCAL && !BWD) cnt += 1.0;
+    const int64_t px = ((int64_t)n * h + oy / r) * w + ox / r;
+    const int sub = (oy % r) * r + ox % r;
+    const __nv_bfloat16* z = lo + px * ldlo + sub;  // class c at z[c * rr]
+    __nv_bfloat16* d = BWD ? dx + px * lddx + sub : nullptr;
+    if (BWD) {
+      if (sub == 0)
+        for (int c = C * rr; c < lddx; ++c) d[c] = f2bf(0.f);
+      if (!valid) {
+        for (int c = 0; c < C; ++c) d[c * rr] = f2bf(0.f);
+        continue;
+      }
+    } else if (!valid && !labeled) {
+      continue;
+    }
+    float mx = -INFINITY;
+    int am = 0;
+    for (int c = 0; c < C; ++c) {
+      const float v = bf2f(z[c * rr]);
+      if (v > mx) {
+        mx = v;
+        am = c;
+      }
+    }
+    float se = 0.f, lt = 0.f;
+    for (int c = 0; c < C; ++c) {
+      const float v = bf2f(z[c * rr]);
+      se += expf(v - mx);
+      if (c == tg) lt = v;
+    }
+    if (!BWD) {
+      if (MET && labeled) {
+        ++n_labeled;
+        atomicAdd(&hist[2 + C + am], 1u);          // area_pred
+        atomicAdd(&hist[2 + 2 * C + (int)tg], 1u);  // area_lab
+        if (am == (int)tg) {
+          ++n_correct;
+          atomicAdd(&hist[2 + (int)tg], 1u);  // area_inter
+        }
+      }
+      if (valid) {
+        const float wt = K == LOSS_CE ? 1.f : class_weight(la, tg, C);
+        loss += (double)pixel_loss<K>(mx + logf(se) - lt, wt, la.gamma);
+        if (K == LOSS_CE) cnt += 1.0;
+        if (K == LOSS_WCE) cnt += (double)wt;
+      }
+    } else {
+      const float inv = 1.f / se;
+      const float gp = K == LOSS_CE ? g : g * pixel_grad_factor<K>(mx + logf(se) - lt, class_weight(la, tg, C), la.gamma);
+      for (int c = 0; c < C; ++c) {
+        const float v = bf2f(z[c * rr]);
+        d[c * rr] = f2bf((expf(v - mx) * inv - (c == tg ? 1.f : 0.f)) * gp);
+      }
+    }
+  }
+  if (!BWD) {
+    block_accum2(loss, cnt, accum);
+    if (MET) {
+      n_correct = __reduce_add_sync(0xffffffffu, n_correct);
+      n_labeled = __reduce_add_sync(0xffffffffu, n_labeled);
+      if ((threadIdx.x & 31) == 0) {
+        atomicAdd(&hist[0], n_correct);
+        atomicAdd(&hist[1], n_labeled);
+      }
+      __syncthreads();
+      for (int i = threadIdx.x; i < 3 * C + 2; i += blockDim.x) {
+        const unsigned int v = hist[i];
+        if (v != 0u) atomicAdd(counters + i, (unsigned long long)v);
+      }
+    }
+  }
+}
+
 __global__ void cast_pad_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ y, int64_t M, int C, int ld) {
   const int64_t total = M * ld;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
@@ -503,6 +606,36 @@ static int upsample_ce_bwd(const float* logits_lo, const int64_t* target, int N,
   return 0;
 }
 
+static int shuffle_ce_check(int N, int h, int w, int C, int r, int ld) {
+  SEG_REQUIRE(C <= MAXC, "shuffle_loss: C=%d > %d", C, MAXC);
+  SEG_REQUIRE(N > 0 && h > 0 && w > 0 && r >= 1, "shuffle_loss: bad sizes");
+  SEG_REQUIRE(ld >= C * r * r, "shuffle_loss: pitch %d < r*r*C = %d", ld, C * r * r);
+  return 0;
+}
+static unsigned shuffle_ce_blocks(int N, int h, int w, int r) {
+  return (unsigned)std::min<int64_t>(ceil_div64((int64_t)N * h * w * r * r, 256), (int64_t)num_sms() * 8);
+}
+template <int K>
+static int shuffle_ce_fwd(const void* lo, int ldlo, const int64_t* target, int N, int h, int w, int C, int r, int64_t ignore_index,
+                          LossArgs la, double* accum, int64_t* counters, cudaStream_t stream) {
+  if (shuffle_ce_check(N, h, w, C, r, ldlo)) return 1;
+  const bool met = counters != nullptr;
+  const auto kernel = met ? shuffle_ce_kernel<false, K, true> : shuffle_ce_kernel<false, K, false>;
+  kernel<<<shuffle_ce_blocks(N, h, w, r), 256, met ? (size_t)(3 * C + 2) * sizeof(unsigned int) : 0, stream>>>(
+      reinterpret_cast<const __nv_bfloat16*>(lo), ldlo, target, N, h, w, C, r, ignore_index, la, accum, nullptr, nullptr, 0,
+      reinterpret_cast<unsigned long long*>(counters));
+  return check_launch(met ? "shuffle_ce_fwd_metrics" : "shuffle_ce_fwd");
+}
+template <int K>
+static int shuffle_ce_bwd(const void* lo, int ldlo, const int64_t* target, int N, int h, int w, int C, int r, int64_t ignore_index,
+                          LossArgs la, const double* accum, const float* gscale, void* dx, int lddx, cudaStream_t stream) {
+  if (shuffle_ce_check(N, h, w, C, r, ldlo) || shuffle_ce_check(N, h, w, C, r, lddx)) return 1;
+  shuffle_ce_kernel<true, K><<<shuffle_ce_blocks(N, h, w, r), 256, 0, stream>>>(
+      reinterpret_cast<const __nv_bfloat16*>(lo), ldlo, target, N, h, w, C, r, ignore_index, la, const_cast<double*>(accum),
+      gscale, reinterpret_cast<__nv_bfloat16*>(dx), lddx, nullptr);
+  return check_launch("shuffle_ce_bwd");
+}
+
 // kind: LOSS_CE (weight NULL, a mean), LOSS_WCE (NULL weight = ones) or LOSS_FOCAL (weight optional)
 static int loss_args(const float* weight, int kind, float gamma, int mean, int C, LossArgs* la) {
   SEG_REQUIRE(C > 0, "loss: C=%d", C);
@@ -572,6 +705,23 @@ int seg_upsample_loss_bwd(const float* logits_lo, const int64_t* target, int N, 
   if (loss_args(weight, kind, gamma, mean, C, &la)) return 1;
   return SEG_LOSS_DISPATCH(kind, upsample_ce_bwd, logits_lo, target, N, Hi, Wi, Ho, Wo, C, align_corners, ignore_index, la, accum,
                            gscale, dlo_f32, dlo_fixed, dx, lddx, ST(stream));
+}
+
+int seg_shuffle_loss_fwd(const void* logits_lo, int ldlo, const int64_t* target, int N, int h, int w, int C, int r,
+                         int64_t ignore_index, const float* weight, int kind, float gamma, double* accum, int64_t* counters,
+                         void* stream) {
+  LossArgs la;
+  if (loss_args(weight, kind, gamma, 1, C, &la)) return 1;
+  return SEG_LOSS_DISPATCH(kind, shuffle_ce_fwd, logits_lo, ldlo, target, N, h, w, C, r, ignore_index, la, accum, counters,
+                           ST(stream));
+}
+int seg_shuffle_loss_bwd(const void* logits_lo, int ldlo, const int64_t* target, int N, int h, int w, int C, int r,
+                         int64_t ignore_index, const float* weight, int kind, float gamma, int mean, const double* accum,
+                         const float* gscale, void* dx, int lddx, void* stream) {
+  LossArgs la;
+  if (loss_args(weight, kind, gamma, mean, C, &la)) return 1;
+  return SEG_LOSS_DISPATCH(kind, shuffle_ce_bwd, logits_lo, ldlo, target, N, h, w, C, r, ignore_index, la, accum, gscale, dx, lddx,
+                           ST(stream));
 }
 
 }  // extern "C"

@@ -10,6 +10,7 @@ _LAZY = {
     "DeepLab": ("nets", "DeepLab"),
     "PSPNet": ("nets", "PSPNet"),
     "UperNet": ("nets", "UperNet"),
+    "DeepLab_DUC_HDC": ("nets", "DeepLab_DUC_HDC"),
     "CrossEntropyLoss2d": ("losses", "CrossEntropyLoss2d"),
     "DiceLoss": ("losses", "DiceLoss"),
     "FocalLoss": ("losses", "FocalLoss"),

@@ -215,6 +215,8 @@ class Tape:
                 sync, tk = self.sync, self.zalloc(1, wp.device)
         if spec.explicit:
             nchw = not isinstance(x, Act)
+            if not nchw and self.record and x.needs_grad and (spec.R, spec.S, spec.stride, spec.pad) != (1, 1, 1, 0):
+                raise NotImplementedError(f"{spec.name}: data gradient of an im2col conv is built for 1x1 convs only")
             src = x if nchw else x.t
             col = ops.im2col(src, spec.R, spec.S, spec.stride, spec.pad, spec.dil, spec.kpad, nchw_f32=nchw)
             y = ops.conv2d_fwd(col, wp, spec.K, 1, 1, out=out, out_dtype=out_dtype, bias=bias.detach() if bias is not None else None,
@@ -259,6 +261,13 @@ class Tape:
                 if (not spec.explicit) and isinstance(x, Act) and x.needs_grad:
                     gx, beta = x.grad_target()
                     ops.conv2d_dgrad(dy, wp, tuple(x.t.shape), R, S, stride, pad, dil, out=gx, beta=beta, impl=self.impl)
+                elif isinstance(x, Act) and x.needs_grad:
+                    # 1x1 im2col conv (C % 8 != 0, e.g. DUC_out.conv over the class scores): the columns are the input padded
+                    # to Kpad channels, so the dgrad over the columns is the data gradient; its pad lanes are zero because the
+                    # packed weight's are
+                    assert x.grad is None, "the input of an im2col conv must have a single consumer"
+                    x.grad = ops.conv2d_dgrad(dy, wp, tuple(xin.shape), 1, 1, 1, 0, 1, impl=self.impl)[..., : spec.C]
+                    x._written = True
                 ya.grad = None
             self._push_back(bwd, (spec.m.weight, bias))
         return ya, stats
@@ -439,6 +448,22 @@ class Tape:
             self.back.append(bwd)
         return ya
 
+    def pixel_shuffle(self, x, r, out=None, crop=None):
+        """nn.PixelShuffle(r) of x [N,H,W,r*r*C], cropped to crop = (Ho, Wo) (default r*H x r*W); `out`: a concat slice."""
+        N, H, W, _ = x.t.shape
+        Ho, Wo = crop if crop is not None else (H * r, W * r)
+        y = ops.pixel_shuffle_fwd(x.t, r, Ho, Wo, out=out)
+        ya = Act(y)
+        if self.record:
+            def bwd():
+                if ya.grad is None or not x.needs_grad:
+                    return
+                gx, beta = x.grad_target()
+                ops.pixel_shuffle_bwd(ya.grad, r, H, W, dx=gx, beta=beta)
+                ya.grad = None
+            self.back.append(bwd)
+        return ya
+
     def up_add(self, x, y):
         """up_and_add of the reference's FPN (models/upernet.py:89-90): bilinear(x -> size of y, align_corners=True) + y."""
         Hy, Wy = y.t.shape[1], y.t.shape[2]
@@ -498,3 +523,63 @@ class Tape:
             a.grad = g[..., off:off + c]
             off += c
         whole._written = False  # the consumer's dgrad overwrites (beta = 0) the pre-allocated buffer
+
+
+# ---------------------------------------------------------------------- output heads
+# A head owns how a model's last tape activation becomes the full-resolution NCHW fp32 logits `model(x)` returns, and the
+# fused loss that reads those logits in place (FusedTrainStep).  Both write the gradient of that activation.
+class BilinearHead:
+    """Low-resolution NHWC fp32 logits, bilinearly upsampled to (H, W) (deeplabv3_plus.py:361, pspnet.py:86, upernet.py:143)."""
+
+    def __init__(self, act, align_corners, H, W):
+        self.act, self.align_corners, self.H, self.W = act, align_corners, H, W
+
+    @property
+    def classes(self):
+        return self.act.t.shape[-1]
+
+    def logits(self):
+        return ops.bilinear_logits_fwd(self.act.t, self.H, self.W, self.align_corners)
+
+    def logits_bwd(self, dout):
+        C, t = self.classes, self.act.t
+        self.act.grad = ops.bilinear_logits_bwd(dout, t.shape[1], t.shape[2], self.align_corners, (C + 7) // 8 * 8)[..., :C]
+
+    def loss_fwd(self, target, ignore_index, weight, gamma, mean, reduce_fn=None, counters=None):
+        loss, accum, _ = ops.upsample_loss_fwd(self.act.t, target, self.align_corners, ignore_index, weight, gamma, mean,
+                                               reduce_fn=reduce_fn, counters=counters)
+        return loss, accum
+
+    def loss_bwd(self, target, ignore_index, accum, weight, gamma, mean, gscale=None):
+        C = self.classes
+        dx, _ = ops.upsample_loss_bwd(self.act.t, target, self.align_corners, ignore_index, accum, (C + 7) // 8 * 8, weight, gamma,
+                                      mean, gscale=gscale)
+        self.act.grad = dx[..., :C]
+
+
+class ShuffleHead:
+    """NHWC bf16 map [N,h,w,r*r*C] whose nn.PixelShuffle(r) is the output [N,C,r*h,r*w] (DeepLab_DUC_HDC, duc_hdc.py:233)."""
+
+    def __init__(self, act, r):
+        self.act, self.r = act, r
+
+    @property
+    def classes(self):
+        return self.act.t.shape[-1] // (self.r * self.r)
+
+    def _ld(self):
+        return (self.act.t.shape[-1] + 7) // 8 * 8
+
+    def logits(self):
+        return ops.pixel_shuffle_logits_fwd(self.act.t, self.r)
+
+    def logits_bwd(self, dout):
+        self.act.grad = ops.pixel_shuffle_logits_bwd(dout, self.r, self._ld())[..., : self.act.t.shape[-1]]
+
+    def loss_fwd(self, target, ignore_index, weight, gamma, mean, reduce_fn=None, counters=None):
+        return ops.shuffle_loss_fwd(self.act.t, self.r, target, ignore_index, weight, gamma, mean, reduce_fn=reduce_fn,
+                                    counters=counters)
+
+    def loss_bwd(self, target, ignore_index, accum, weight, gamma, mean, gscale=None):
+        dx = ops.shuffle_loss_bwd(self.act.t, self.r, target, ignore_index, accum, self._ld(), weight, gamma, mean, gscale=gscale)
+        self.act.grad = dx[..., : self.act.t.shape[-1]]

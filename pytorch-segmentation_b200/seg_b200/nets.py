@@ -3,13 +3,15 @@
     DeepLab(num_classes, in_channels=3, backbone='xception',  pretrained=None, output_stride=16, freeze_bn=False, **_)
     PSPNet (num_classes, in_channels=3, backbone='resnet152', pretrained=None, use_aux=True,   freeze_bn=False, **_)
     UperNet(num_classes, in_channels=3, backbone='resnet101', pretrained=None, use_aux=True, fpn_out=256, freeze_bn=False, **_)
+    DeepLab_DUC_HDC(num_classes, in_channels=3, pretrained=None, output_stride=8, freeze_bn=False, **_)
 
 (default backbones are the reference's; `pretrained`: the reference defaults to True and downloads ImageNet weights — there is
 no network here, so an explicit True raises and the default (None) initialises randomly with a logged warning)
 
 Same constructor contract, same `state_dict()` keys and OIHW fp32 parameter layout, same `get_backbone_params /
 get_decoder_params / freeze_bn` methods and the same forward contract (fp32 NCHW logits at input resolution; PSPNet
-returns `(out, aux)` in training) as models/deeplabv3_plus.py:336-377 and models/pspnet.py:41-105 — so train.py,
+returns `(out, aux)` in training; DeepLab_DUC_HDC's are at 4x its layer1 size) as models/deeplabv3_plus.py:336-377 and
+models/pspnet.py:41-105 — so train.py,
 BaseTrainer (base/base_trainer.py:46-57), torch.optim.SGD, checkpoints and `convert_model` keep working.
 
 The nn.Conv2d / nn.BatchNorm2d children are PARAMETER HOLDERS only: forward never calls them.  `forward` runs the
@@ -26,7 +28,7 @@ import torch
 import torch.nn as nn
 
 from . import ops
-from .engine import Act, ConvSpec, DwSpec, Tape
+from .engine import Act, BilinearHead, ConvSpec, DwSpec, ShuffleHead, Tape
 from .lib import IMPL_AUTO, require_device
 
 try:  # inside the reference tree: subclass its BaseModel so isinstance checks and logging behave identically
@@ -101,13 +103,16 @@ def _bottleneck(inplanes, planes, stride, dil, with_downsample):
 
 
 def _res_layers(blocks, inplanes, plan):
-    """plan: per layer (first-block stride, first-block dilation, other-block dilation)."""
+    """plan: per layer (first-block stride, first-block dilation, other-block dilation), or (first-block stride, [dilation
+    of every block]) for per-block rates such as HDC's (duc_hdc.py:78-103)."""
     layers = []
     for li, (n, planes) in enumerate(zip(blocks, (64, 128, 256, 512))):
-        stride, d0, d = plan[li]
+        stride, *d = plan[li]
+        dils = list(d[0]) if len(d) == 1 else [d[0]] + [d[1]] * (n - 1)
+        assert len(dils) == n, f"layer{li + 1}: {len(dils)} dilations for {n} blocks"
         seq = []
         for b in range(n):
-            seq.append(_bottleneck(inplanes, planes, stride if b == 0 else 1, d0 if b == 0 else d, b == 0))
+            seq.append(_bottleneck(inplanes, planes, stride if b == 0 else 1, dils[b], b == 0))
             inplanes = planes * 4
         layers.append(nn.Sequential(*seq))
     return layers
@@ -236,13 +241,10 @@ class _EngineFn(torch.autograd.Function):
         tape = ctx.tape
         if tape is None or not tape.record:
             raise RuntimeError("backward through a forward that ran without gradient recording")
-        for (lo_act, Hl, Wl, ac), dout in zip(ctx.heads, douts):
+        for head, dout in zip(ctx.heads, douts):
             if dout is None:
                 continue
-            C = dout.shape[1]
-            ldx = (C + 7) // 8 * 8
-            g = ops.bilinear_logits_bwd(dout.contiguous().float(), Hl, Wl, ac, ldx)
-            lo_act.grad = g[..., :C]
+            head.logits_bwd(dout.contiguous().float())
         tape.backward()
         grads = tape.grads
         if ctx.flat is not None:
@@ -461,10 +463,8 @@ class _EngineModel(BaseModel):
             with torch.cuda.graph(bwd, pool=e.pool, capture_error_mode=mode):
                 e.flat_grad.zero_()
                 e.wt.zero_wgrads()
-                for (lo_act, Hl, Wl, ac), d in zip(heads, e.douts):
-                    C = d.shape[1]
-                    g = ops.bilinear_logits_bwd(d, Hl, Wl, ac, (C + 7) // 8 * 8)
-                    lo_act.grad = g[..., :C]
+                for head, d in zip(heads, e.douts):
+                    head.logits_bwd(d)
                 tape.backward()
                 e.wt.unpack()
                 if self._dp_world() > 1:  # the gradient exchange is part of the captured backward (NCCL kernels replay)
@@ -595,16 +595,15 @@ class _EngineModel(BaseModel):
 
     def _run(self, x, training, record, tables=None, grads=None):
         x = x.contiguous().float()
-        H, W = x.shape[2], x.shape[3]
         tape = self._new_tape(training, record)
         if tables is not None:  # graph capture: persistent packed weights / packed weight-gradient accumulators
             tape.packed_override, tape.dw_buffers = tables.packed_bufs, tables.dw_bufs
         if grads is not None:
             tape.grads = dict(grads)  # pre-bound views: every parameter gradient lands in one flat buffer
         heads = self._forward_heads(tape, x)
-        outs = tuple(ops.bilinear_logits_fwd(lo.t, H, W, ac) for lo, ac in heads)
+        outs = tuple(h.logits() for h in heads)
         self._finish(tape)
-        return outs, tape, [(lo, lo.t.shape[1], lo.t.shape[2], ac) for lo, ac in heads]
+        return outs, tape, heads
 
     def freeze_bn(self):
         for module in self.modules():
@@ -738,8 +737,8 @@ class DeepLab(_EngineModel):
         return self._decoder(tape, self._aspp(tape, a), low)
 
     def _forward_heads(self, tape, x):
-        """[(stride-4 fp32 logits Act, align_corners of the final upsample)]  (deeplabv3_plus.py:361: True)"""
-        return [(self._features(tape, x), True)]
+        """[head of the stride-4 fp32 logits]  (deeplabv3_plus.py:361: align_corners=True)"""
+        return [BilinearHead(self._features(tape, x), True, x.shape[2], x.shape[3])]
 
     def get_backbone_params(self):
         return self.backbone.parameters()
@@ -806,12 +805,13 @@ class PSPNet(_EngineModel):
             if li == 3:
                 x_aux = a
         lo = self._psp_head(tape, a)
-        heads = [(lo, False)]  # pspnet.py:86,91: F.interpolate default align_corners=False; the crop is a no-op
+        H, W = x.shape[2], x.shape[3]
+        heads = [BilinearHead(lo, False, H, W)]  # pspnet.py:86,91: F.interpolate default align_corners=False; the crop is a no-op
         if self.training and self.use_aux:
             ab = self.auxiliary_branch
             ya = self._cbr(tape, x_aux, "auxiliary_branch.0", ab[0], ab[1], drop_p=ab[3].p, drop_channelwise=True)
             la, _ = tape.conv(ya, self._spec("auxiliary_branch.4", ab[4]), out_dtype=torch.float32)
-            heads.append((la, False))
+            heads.append(BilinearHead(la, False, H, W))
         return heads
 
     def _psp_head(self, tape, a):
@@ -932,10 +932,129 @@ class UperNet(_EngineModel):
         tape.bind_slices(cat2, parts)
         y = self._cbr(tape, cat2, "FPN.conv_fusion.0", F_.conv_fusion[0], F_.conv_fusion[1])
         lo, _ = tape.conv(y, self._spec("head", self.head), out_dtype=torch.float32)
-        return [(lo, False)]  # upernet.py:143: F.interpolate default align_corners=False
+        return [BilinearHead(lo, False, x.shape[2], x.shape[3])]  # upernet.py:143: F.interpolate default align_corners=False
 
     def get_backbone_params(self):
         return self.backbone.parameters()
 
     def get_decoder_params(self):
         return chain(self.PPN.parameters(), self.FPN.parameters(), self.head.parameters())
+
+
+# ----------------------------------------------------------------------------------------------- DeepLab_DUC_HDC
+def _duc(cin, cout, r):
+    """DUC holder (duc_hdc.py:15-31): 1x1 conv to cout*r*r channels without bias, BN, ReLU, PixelShuffle(r)."""
+    d = _Holder()
+    d.conv = nn.Conv2d(cin, cout * r * r, 1, bias=False)
+    d.bn = nn.BatchNorm2d(cout * r * r)
+    d.relu = nn.ReLU(inplace=True)
+    d.pixl_shf = nn.PixelShuffle(upscale_factor=r)
+    return d
+
+
+def _icnr_(conv, r):
+    """duc_hdc.py:33-49 (ICNR): the r*r output channels of one shuffle group share one kaiming-normal kernel."""
+    o, i, kh, kw = conv.weight.shape
+    sub = nn.init.kaiming_normal_(torch.empty(o // (r * r), i, kh, kw))
+    conv.weight.data.copy_(sub.repeat_interleave(r * r, dim=0))
+
+
+class DeepLab_DUC_HDC(_EngineModel):
+    """DeepLab v3+ with HDC dilations and DUC upsampling — replaces models/duc_hdc.py:214-245: a ResNet-101 trunk at output
+    stride 8 (layer3 / layer4 at stride 1 with per-block rates [1,2,3]*7+[2,2] and [3,4,5]; output_stride=4 also drops the
+    stem conv's stride), a six-branch ASPP + image pooling, a decoder whose x2 upsampling is DUC (1x1 conv, BN, ReLU,
+    PixelShuffle(2), cropped to the low-level size) and DUC_out = DUC(C, C, 4): the model returns the ReLU'd, pixel-shuffled
+    [N, C, 4*Hl, 4*Wl] scores (Hl, Wl: layer1 size; a 65x65 input gives 68x68, as in the reference).
+    Quirks kept: ICNR init on DUC_out.conv only (the decoder's initialize_weights overwrites decoder.DUC.conv).
+    (The reference constructor itself raises NameError: freeze_backbone, duc_hdc.py:225 — here the argument works.)"""
+
+    def __init__(self, num_classes, in_channels=3, pretrained=None, output_stride=8, freeze_bn=False, freeze_backbone=False, **_):
+        super().__init__()
+        _check_pretrained(self, pretrained)
+        assert output_stride in (4, 8), "Only output strides of 8 or 16 are suported"
+        self.num_classes, self.output_stride = num_classes, output_stride
+        bb = _Holder()
+        c0, b0 = nn.Conv2d(in_channels, 64, 7, stride=2 if output_stride == 8 else 1, padding=3, bias=False), nn.BatchNorm2d(64)
+        bb.layer0 = nn.Sequential(c0, b0, nn.ReLU(inplace=True), nn.MaxPool2d(kernel_size=3, stride=2, padding=1))
+        plan = [(1, [1] * 3), (2, [1] * 4), (1, [1, 2, 3] * 7 + [2, 2]), (1, [3, 4, 5])]
+        bb.layer1, bb.layer2, bb.layer3, bb.layer4 = _res_layers(RESNET_BLOCKS["resnet101"], 64, plan)
+        self.backbone = bb
+        a = _Holder()
+        for i, d in enumerate((1, 6, 12, 18, 24, 36), 1):
+            c, n = _cbn(2048, 256, 1 if i == 1 else 3, 1, d)
+            setattr(a, f"aspp{i}", nn.Sequential(c, n, nn.ReLU(inplace=True)))
+        c, n = _cbn(2048, 256, 1)
+        a.avg_pool = nn.Sequential(nn.AdaptiveAvgPool2d((1, 1)), c, n, nn.ReLU(inplace=True))
+        a.conv1, a.bn1 = _cbn(256 * 7, 256, 1)
+        a.relu, a.dropout = nn.ReLU(inplace=True), nn.Dropout(0.5)
+        self.ASSP = a
+        d = _Holder()
+        d.conv1, d.bn1 = _cbn(256, 48, 1)
+        d.relu = nn.ReLU(inplace=True)
+        d.DUC = _duc(256, 256, 2)
+        c1, n1 = _cbn(48 + 256, 256, 3)
+        c2, n2 = _cbn(256, 256, 3)
+        d.output = nn.Sequential(c1, n1, nn.ReLU(inplace=True), c2, n2, nn.ReLU(inplace=True), nn.Dropout(0.1),
+                                 nn.Conv2d(256, num_classes, 1, stride=1))
+        self.decoder = d
+        self.DUC_out = _duc(num_classes, num_classes, 4)
+        _init_like_torchvision_trunk(bb.layer1, bb.layer2, bb.layer3, bb.layer4)
+        _init_like_reference_head(bb.layer0, self.ASSP, self.decoder, self.DUC_out)
+        _icnr_(self.DUC_out.conv, 4)
+        if freeze_bn:
+            self.freeze_bn()
+        if freeze_backbone:
+            for p in self.backbone.parameters():
+                p.requires_grad = False
+
+    def _decoder(self, tape, f, low):
+        """Decoder.forward (duc_hdc.py:200-208): the DUC output is shuffled and cropped straight into the concat buffer
+        (low-level 48, upsampled 256); returns the bf16 class scores Act (pitch padded to 8 channels for DUC_out's im2col)."""
+        D = self.decoder
+        N, Hl, Wl = low.t.shape[0], low.t.shape[1], low.t.shape[2]
+        cat, sl = tape.concat(N, Hl, Wl, [48, 256], low.t.device)
+        l48 = self._cbr(tape, low, "decoder.conv1", D.conv1, D.bn1, out=sl[0])
+        u = self._cbr(tape, f, "decoder.DUC.conv", D.DUC.conv, D.DUC.bn)
+        up = tape.pixel_shuffle(u, 2, out=sl[1], crop=(Hl, Wl))
+        tape.bind_slices(cat, [l48, up])
+        y = self._cbr(tape, cat, "decoder.output.0", D.output[0], D.output[1])
+        y = self._cbr(tape, y, "decoder.output.3", D.output[3], D.output[4], drop_p=D.output[6].p)
+        C = self.num_classes
+        buf = torch.empty((N, Hl, Wl, (C + 7) // 8 * 8), dtype=y.t.dtype, device=y.t.device)[..., :C]
+        lo, _ = tape.conv(y, self._spec("decoder.output.7", D.output[7]), out=buf)
+        return lo
+
+    def _aspp(self, tape, a):
+        """ASSP.forward (duc_hdc.py:157-174): six branches + image pooling written straight into one 1792-channel buffer."""
+        N, Hf, Wf = a.t.shape[0], a.t.shape[1], a.t.shape[2]
+        A = self.ASSP
+        cat, sl = tape.concat(N, Hf, Wf, [256] * 7, a.t.device)
+        br = []
+        for i in range(1, 7):
+            seq = getattr(A, f"aspp{i}")
+            br.append(self._cbr(tape, a, f"ASSP.aspp{i}.0", seq[0], seq[1], out=sl[i - 1]))
+        g = tape.avgpool(a, 1)
+        g = self._cbr(tape, g, "ASSP.avg_pool.1", A.avg_pool[1], A.avg_pool[2])
+        br.append(tape.bilinear(g, Hf, Wf, True, out=sl[6]))
+        tape.bind_slices(cat, br)
+        return self._cbr(tape, cat, "ASSP.conv1", A.conv1, A.bn1, drop_p=A.dropout.p)
+
+    def _forward_heads(self, tape, x):
+        bb = self.backbone
+        a = self._cbr(tape, x, "backbone.layer0.0", bb.layer0[0], bb.layer0[1])
+        a = tape.maxpool(a)
+        low = None
+        for li in (1, 2, 3, 4):
+            for bi, blk in enumerate(getattr(bb, f"layer{li}")):
+                a = self._block(tape, a, f"backbone.layer{li}.{bi}.", blk)
+            if li == 1:
+                low = a
+        y = self._decoder(tape, self._aspp(tape, a), low)
+        z = self._cbr(tape, y, "DUC_out.conv", self.DUC_out.conv, self.DUC_out.bn)
+        return [ShuffleHead(z, 4)]
+
+    def get_backbone_params(self):
+        return self.backbone.parameters()
+
+    def get_decoder_params(self):
+        return chain(self.ASSP.parameters(), self.decoder.parameters(), self.DUC_out.parameters())

@@ -432,6 +432,48 @@ def bilinear_logits_bwd(dy_nchw, Hi, Wi, align_corners, ldx):
     return dx
 
 
+def pixel_shuffle_fwd(x, r, Ho, Wo, out=None):
+    """nn.PixelShuffle(r) on NHWC bf16 [N,H,W,r*r*C], cropped to [N,Ho,Wo,C] (Ho <= r*H, Wo <= r*W); `out` may be a channel slice."""
+    N, H, W, Cr = x.shape
+    C = Cr // (r * r)
+    assert C * r * r == Cr and x.dtype == torch.bfloat16
+    if out is None:
+        out = torch.empty((N, Ho, Wo, C), dtype=torch.bfloat16, device=x.device)
+    assert tuple(out.shape) == (N, Ho, Wo, C)
+    call("seg_pixel_shuffle_fwd", ptr(x), ld(x), ptr(out), ld(out), N, H, W, C, r, Ho, Wo)
+    return out
+
+
+def pixel_shuffle_bwd(dy, r, H, W, dx=None, beta=0.0):
+    """dx [N,H,W,r*r*C] = beta*dx + the inverse permutation of dy [N,Ho,Wo,C]; positions the crop dropped get zero."""
+    N, Ho, Wo, C = dy.shape
+    if dx is None:
+        dx = torch.empty((N, H, W, C * r * r), dtype=torch.bfloat16, device=dy.device)
+        beta = 0.0
+    assert tuple(dx.shape) == (N, H, W, C * r * r)
+    call("seg_pixel_shuffle_bwd", ptr(dy), ld(dy), ptr(dx), ld(dx), N, H, W, C, r, Ho, Wo, float(beta))
+    return dx
+
+
+def pixel_shuffle_logits_fwd(x, r):
+    """NHWC bf16 [N,h,w,r*r*C] -> the NCHW fp32 [N,C,r*h,r*w] logits of F.pixel_shuffle."""
+    N, h, w, Cr = x.shape
+    C = Cr // (r * r)
+    assert C * r * r == Cr and x.dtype == torch.bfloat16
+    y = torch.empty((N, C, h * r, w * r), dtype=torch.float32, device=x.device)
+    call("seg_pixel_shuffle_logits_fwd", ptr(x), ld(x), ptr(y), N, h, w, C, r)
+    return y
+
+
+def pixel_shuffle_logits_bwd(dy_nchw, r, ldx):
+    """NCHW fp32 grad [N,C,r*h,r*w] -> NHWC bf16 [N,h,w,ldx] (channels r*r*C.. zero)."""
+    N, C, Ho, Wo = dy_nchw.shape
+    assert dy_nchw.is_contiguous() and dy_nchw.dtype == torch.float32 and Ho % r == 0 and Wo % r == 0
+    dx = torch.empty((N, Ho // r, Wo // r, ldx), dtype=torch.bfloat16, device=dy_nchw.device)
+    call("seg_pixel_shuffle_logits_bwd", ptr(dy_nchw), ptr(dx), ldx, N, Ho // r, Wo // r, C, r)
+    return dx
+
+
 # ---------------------------------------------------------------- loss
 def _loss_kind(weight, gamma, mean):
     """SEG_LOSS_* of a per-pixel loss: focal when gamma is given; else unweighted cross-entropy for a mean without class
@@ -550,6 +592,41 @@ def upsample_loss_bwd(logits_lo, target, align_corners, ignore_index, accum, ldx
          ptr(weight), _loss_kind(weight, gamma, mean), float(gamma or 0.0), int(mean), ptr(accum), ptr(gscale), ptr(dlo),
          ptr(fixed), ptr(dx), ldx)
     return dx, dlo
+
+
+def _shuffle_loss_shapes(lo, r, target):
+    N, h, w, Cr = lo.shape
+    C = Cr // (r * r)
+    assert C * r * r == Cr and lo.dtype == torch.bfloat16 and target.dtype == torch.int64 and target.is_contiguous()
+    if tuple(target.shape) != (N, h * r, w * r):
+        raise ValueError(f"target size {tuple(target.shape[1:])} differs from the model output size {(h * r, w * r)}")
+    return N, h, w, C
+
+
+def shuffle_loss_fwd(logits_lo, r, target, ignore_index, weight=None, gamma=None, mean=True, reduce_fn=None, counters=None):
+    """loss_nchw_fwd on the F.pixel_shuffle(r) view of the NHWC bf16 map [N,h,w,r*r*C], read in place; returns (loss, accum).
+    counters: as for upsample_loss_fwd."""
+    N, h, w, C = _shuffle_loss_shapes(logits_lo, r, target)
+    assert weight is None or (weight.dtype == torch.float32 and weight.numel() == C and weight.is_contiguous())
+    if counters is not None:
+        _check_counters(counters, C)
+    accum = torch.zeros(2, dtype=torch.float64, device=logits_lo.device)
+    call("seg_shuffle_loss_fwd", ptr(logits_lo), ld(logits_lo), ptr(target), N, h, w, C, r, int(ignore_index), ptr(weight),
+         _loss_kind(weight, gamma, mean), float(gamma or 0.0), ptr(accum), ptr(counters))
+    if reduce_fn is not None:
+        reduce_fn(accum)
+    loss = torch.empty((), dtype=torch.float32, device=logits_lo.device)
+    call("seg_loss_finalize", ptr(accum), int(mean), ptr(loss))
+    return loss, accum
+
+
+def shuffle_loss_bwd(logits_lo, r, target, ignore_index, accum, ldx, weight=None, gamma=None, mean=True, gscale=None):
+    """Gradient of shuffle_loss_fwd's loss w.r.t. the low-res map: bf16 [N,h,w,ldx] (channels r*r*C.. zero)."""
+    N, h, w, C = _shuffle_loss_shapes(logits_lo, r, target)
+    dx = torch.empty((N, h, w, ldx), dtype=torch.bfloat16, device=logits_lo.device)
+    call("seg_shuffle_loss_bwd", ptr(logits_lo), ld(logits_lo), ptr(target), N, h, w, C, r, int(ignore_index), ptr(weight),
+         _loss_kind(weight, gamma, mean), float(gamma or 0.0), int(mean), ptr(accum), ptr(gscale), ptr(dx), ldx)
+    return dx
 
 
 # ---------------------------------------------------------------- misc

@@ -1,5 +1,5 @@
-"""Fused training step for the engine models: forward -> fused upsample+CE (no full-resolution logits in HBM) ->
-backward -> (NCCL gradient all-reduce) -> fused multi-tensor SGD.  Same arithmetic as one iteration of the
+"""Fused training step for the engine models: forward -> fused upsample (or pixel shuffle) + CE (no full-resolution
+logits in HBM) -> backward -> (NCCL gradient all-reduce) -> fused multi-tensor SGD.  Same arithmetic as one iteration of the
 reference's Trainer._train_epoch (trainer.py:55-71) with torch.optim.SGD and differential learning rates
 (base/base_trainer.py:46-57), minus the host synchronisations.  Optionally also the training metrics of trainer.py:84-86
 and the validation pass of Trainer._valid_epoch (trainer.py:109-165), from the same fused loss kernel.
@@ -8,7 +8,7 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
-from . import lib, ops
+from . import lib
 from . import metrics as _metrics
 from .engine import Tape
 
@@ -281,21 +281,20 @@ class FusedTrainStep:
         was = m.training
         m.training = False  # PSPNet builds its aux head only in training mode (pspnet.py:91); only the main head is scored
         try:
-            lo, ac = m._forward_heads(tape, x.contiguous().float())[0]
+            head = m._forward_heads(tape, x.contiguous().float())[0]
         finally:
             m.training = was
-        loss, _, _ = self._loss_fwd(lo.t, target, ac, self.seg_counters)
+        loss, _, _ = self._loss_fwd(head, target, self.seg_counters)
         return loss
 
-    def _loss_fwd(self, lo_t, target, ac, counters):
+    def _loss_fwd(self, head, target, counters):
         """(loss, fp64 accum, class weights) of one head.  Mean over the valid pixels of the GLOBAL batch, as
         nn.DataParallel's gathered logits give the reference (trainer.py:60-66): the (loss sum, denominator) pair is
         all-reduced (16 bytes); a 'sum' is the global sum."""
         rf = (lambda acc: dist.all_reduce(acc)) if self.world > 1 else None
         spec = self.loss_spec
-        cw = spec.weight_on(lo_t.device, lo_t.shape[-1])
-        loss, accum, _ = ops.upsample_loss_fwd(lo_t, target, ac, self.ignore_index, cw, spec.gamma, spec.mean, reduce_fn=rf,
-                                               counters=counters)
+        cw = spec.weight_on(head.act.t.device, head.classes)
+        loss, accum = head.loss_fwd(target, self.ignore_index, cw, spec.gamma, spec.mean, reduce_fn=rf, counters=counters)
         return loss, accum, cw
 
     def _invalidate_param_caches(self):
@@ -382,17 +381,14 @@ class FusedTrainStep:
         heads = m._forward_heads(tape, x.contiguous().float())
         total = None
         spec = self.loss_spec
-        for i, (lo, ac) in enumerate(heads):
-            C = lo.t.shape[-1]
+        for i, head in enumerate(heads):
             # the main head only is counted (trainer.py:62); the gradient is scaled by world because the exchanged
             # gradients are averaged over ranks below
-            loss, accum, cw = self._loss_fwd(lo.t, target, ac, self.seg_counters if i == 0 else None)
+            loss, accum, cw = self._loss_fwd(head, target, self.seg_counters if i == 0 else None)
             w = 1.0 if i == 0 else self.aux_weight
             wg = w * self.world
-            g = None if wg == 1.0 else torch.full((1,), wg, dtype=torch.float32, device=lo.t.device)
-            dx, _ = ops.upsample_loss_bwd(lo.t, target, ac, self.ignore_index, accum, (C + 7) // 8 * 8, cw, spec.gamma, spec.mean,
-                                          gscale=g)
-            lo.grad = dx[..., :C]
+            g = None if wg == 1.0 else torch.full((1,), wg, dtype=torch.float32, device=head.act.t.device)
+            head.loss_bwd(target, self.ignore_index, accum, cw, spec.gamma, spec.mean, gscale=g)
             total = loss if total is None else total + w * loss
         m._finish(tape)
         if self.world > 1 and self.buckets:
