@@ -168,7 +168,10 @@ int seg_counter_add(uint64_t* ctr, uint64_t inc, void* stream);
  * peer and leaves the WORLD's in sums[]; the consumer is seg_bn_bwd_apply with the world's count.
  * out == NULL with relu (both backward passes): the ReLU mask is recomputed from x with the forward's own coefficients
  * (sc = gamma/std, sh = fma(-mean, sc, beta)) instead of being read from the stored activation — valid for
- * conv -> BN(batch statistics) -> ReLU with no residual and no dropout; needs gamma and beta. */
+ * conv -> BN(batch statistics) -> ReLU with no residual and no dropout; needs gamma and beta.
+ * Dropout in the backward (all three backward entry points) needs relu != 0: the keep mask is read from the stored
+ * activation (out > 0), which without the ReLU does not tell a dropped element from a negative one, so relu == 0 with
+ * drop_p > 0 is rejected. */
 int seg_bn_bwd_reduce_slots(void);
 int seg_bn_bwd_reduce(const void* dout, int lddo, const void* out, int ldo, const void* x, int ldx,
                       const float* save_mean_istd, int64_t M, int C, int relu, float drop_p, float* sums, double* acc,

@@ -1480,6 +1480,7 @@ int seg_bn_bwd_reduce(const void* dout, int lddo, const void* out, int ldo, cons
                       void* stream) {
   SEG_REQUIRE(C % 8 == 0 && lddo % 8 == 0 && ldx % 8 == 0 && (!relu || !out || ldo % 8 == 0), "bn_bwd_reduce: alignment");
   SEG_REQUIRE(!(relu && !out) || (gamma && beta && drop_p == 0.f), "bn_bwd_reduce: out == NULL (mask recomputed from x) needs gamma, beta and no dropout");
+  SEG_REQUIRE(relu || drop_p == 0.f, "bn_bwd_reduce: dropout (drop_p > 0) needs relu: the keep mask is read from out > 0");
   SEG_REQUIRE(acc && ticket, "bn_bwd_reduce: zeroed fp64 accumulators [seg_bn_bwd_reduce_slots()][2C] and ticket word required");
   SEG_REQUIRE(!sync || 2 * C <= sync->n_max, "bn_bwd_reduce: 2*C exceeds the SyncBN buffer");
   const dim3 grid = reduce2_grid(M, C);
@@ -1493,6 +1494,7 @@ int seg_bn_bwd_apply(const void* dout, int lddo, const void* out, int ldo, const
                      void* dx, int lddx, void* dres, int lddres, float beta_res, const float* beta, void* stream) {
   SEG_REQUIRE(C % 8 == 0 && lddo % 8 == 0 && ldx % 8 == 0 && lddx % 8 == 0, "bn_bwd_apply: alignment");
   SEG_REQUIRE(!(relu && !out) || (beta && drop_p == 0.f), "bn_bwd_apply: out == NULL (mask recomputed from x) needs beta and no dropout");
+  SEG_REQUIRE(relu || drop_p == 0.f, "bn_bwd_apply: dropout (drop_p > 0) needs relu: the keep mask is read from out > 0");
   launch_pdl((relu && !out) ? bn_bwd_apply_kernel<true> : bn_bwd_apply_kernel<false>, rowmap_grid(M, C), dim3(256), 0, ST(stream),
              CBF(dout), lddo, CBF(out), ldo, CBF(x), ldx, save,
              gamma, sums, (float)(1.0 / count), M, C, relu, drop_p, BF(dx), lddx, BF(dres), lddres, beta_res, beta);
@@ -1533,6 +1535,7 @@ int seg_bn_bwd_fused(const void* dout, int lddo, const void* out, int ldo, const
   SEG_REQUIRE(C % 8 == 0 && lddo % 8 == 0 && ldx % 8 == 0 && lddx % 8 == 0 && (!out || ldo % 8 == 0) && (!dres || lddres % 8 == 0),
               "bn_bwd_fused: alignment");
   SEG_REQUIRE(!(relu && !out) || (beta && drop_p == 0.f), "bn_bwd_fused: out == NULL (mask recomputed from x) needs beta and no dropout");
+  SEG_REQUIRE(relu || drop_p == 0.f, "bn_bwd_fused: dropout (drop_p > 0) needs relu: the keep mask is read from out > 0");
   SEG_REQUIRE(sums && rows && tickets && gamma && save && dx && count_total > 0, "bn_bwd_fused: missing buffer");
   const bool remask = relu && !out;
   BnBwdFused p;

@@ -307,53 +307,6 @@ def test_dropout_statistics():
     assert not torch.equal(out, out3)
 
 
-def test_maxpool(gpu_out_dir):
-    g = torch.Generator().manual_seed(7)
-    x = F.relu(bf(torch.randn(2, 64, 33, 35, generator=g))).requires_grad_(True)  # ReLU zeros -> ties
-    y = F.max_pool2d(x, 3, 2, 1)
-    dy = bf(torch.randn(y.shape, generator=g))
-    y.backward(dy)
-    yd, idx = ops.maxpool3x3s2_fwd(to_nhwc_dev(x.detach()))
-    check("maxpool_fwd", yd.permute(0, 3, 1, 2), y, 0.0, gpu_out_dir)
-    dx = ops.maxpool3x3s2_bwd(to_nhwc_dev(dy), idx, (2, 33, 35, 64))
-    check("maxpool_bwd", dx.permute(0, 3, 1, 2), x.grad, 1e-2, gpu_out_dir)
-
-
-@pytest.mark.parametrize("bins", [1, 2, 3, 6])
-def test_adaptive_avgpool(bins, gpu_out_dir):
-    g = torch.Generator().manual_seed(8)
-    x = bf(torch.randn(2, 64, 15, 17, generator=g)).requires_grad_(True)
-    y = F.adaptive_avg_pool2d(x, bins)
-    dy = bf(torch.randn(y.shape, generator=g))
-    y.backward(dy)
-    yd = ops.adaptive_avgpool_fwd(to_nhwc_dev(x.detach()), bins)
-    check(f"avgpool_fwd b={bins}", yd.permute(0, 3, 1, 2), y, 1e-2, gpu_out_dir)
-    dx = ops.adaptive_avgpool_bwd(to_nhwc_dev(dy), (2, 15, 17, 64), bins)
-    check(f"avgpool_bwd b={bins}", dx.permute(0, 3, 1, 2), x.grad, 1e-2, gpu_out_dir)
-
-
-@pytest.mark.parametrize("ac", [True, False])
-@pytest.mark.parametrize("sizes", [((9, 9), (33, 33)), ((1, 1), (9, 9)), ((6, 6), (15, 15)), ((8, 8), (31, 29))])
-def test_bilinear(sizes, ac, gpu_out_dir):
-    (Hi, Wi), (Ho, Wo) = sizes
-    g = torch.Generator().manual_seed(9)
-    x = bf(torch.randn(2, 16, Hi, Wi, generator=g)).requires_grad_(True)
-    y = F.interpolate(x, size=(Ho, Wo), mode="bilinear", align_corners=ac)
-    dy = bf(torch.randn(y.shape, generator=g))
-    y.backward(dy)
-    yd = ops.bilinear_fwd(to_nhwc_dev(x.detach()), Ho, Wo, ac)
-    check(f"bilinear_fwd {sizes} ac={ac}", yd.permute(0, 3, 1, 2), y, 1e-2, gpu_out_dir)
-    dx = ops.bilinear_bwd(to_nhwc_dev(dy), Hi, Wi, ac)
-    check(f"bilinear_bwd {sizes} ac={ac}", dx.permute(0, 3, 1, 2), x.grad, 1e-2, gpu_out_dir)
-    # fp32 logits variant (NHWC fp32 -> NCHW fp32) and its backward
-    xl = x.detach().permute(0, 2, 3, 1).contiguous().to(DEV)
-    yl = ops.bilinear_logits_fwd(xl, Ho, Wo, ac)
-    check(f"bilinear_logits_fwd {sizes} ac={ac}", yl, y, 1e-5, gpu_out_dir)
-    dxl = ops.bilinear_logits_bwd(dy.to(DEV), Hi, Wi, ac, 24)
-    check(f"bilinear_logits_bwd {sizes} ac={ac}", dxl[..., :16].permute(0, 3, 1, 2), x.grad, 1e-2, gpu_out_dir)
-    assert dxl[..., 16:].abs().max().item() == 0
-
-
 @pytest.mark.parametrize("C,ignore", [(19, 255), (21, 255), (150, -1)])
 def test_cross_entropy(C, ignore, gpu_out_dir):
     g = torch.Generator().manual_seed(10)
@@ -459,17 +412,6 @@ def test_depthwise_conv(shape, gpu_out_dir):
     gw = torch.empty(C, 1, 3, 3, device=DEV)
     ops.dw_unpack_wgrad(g9, gw)
     check(f"dwconv_bwd_weight {shape}", gw, w.grad, 2e-3, gpu_out_dir)
-
-
-def test_relu_standalone(gpu_out_dir):
-    g = torch.Generator().manual_seed(14)
-    x = bf(torch.randn(2, 9, 9, 64, generator=g))
-    y = ops.relu_fwd(x.to(DEV, torch.bfloat16))
-    check("relu_fwd", y, x.clamp(min=0), 0.0, gpu_out_dir)
-    dy = bf(torch.randn(2, 9, 9, 64, generator=g))
-    dx = torch.ones(2, 9, 9, 64, device=DEV, dtype=torch.bfloat16)
-    ops.relu_bwd(dy.to(DEV, torch.bfloat16), y, dx, 1.0)
-    check("relu_bwd_beta1", dx, 1.0 + dy * (x > 0), 1e-2, gpu_out_dir)
 
 
 def test_lovasz_softmax_matches_reference_golden_and_oracle(gpu_out_dir):
