@@ -314,7 +314,9 @@ int seg_dice_nchw_bwd(const float* logits, const int64_t* target, int N, int C, 
  *   seg_lovasz_count: counts (int32 [C+1], zeroed here): valid pixels per class, counts[C] = all valid pixels.
  *   The caller reads counts back (the one host sync; the reference does C of them), then passes P = counts[C],
  *   n_present = #{c: counts[c] > 0}, two uint64 key buffers of P*n_present elements and a byte workspace.
- *   seg_lovasz_softmax_nchw: loss (fp32 scalar) and dlogits = d loss / d logits (NCHW fp32; also scratch). */
+ *   seg_lovasz_softmax_nchw: loss (fp32 scalar) and dlogits = d loss / d logits (NCHW fp32; also scratch).
+ *   Exactly tied errors take ranks in flat pixel order, and the loss is folded in a fixed order: two calls on the same
+ *   inputs give bit-identical results. */
 int seg_lovasz_count(const int64_t* target, int64_t npix, int C, int64_t ignore_index, int32_t* counts, void* stream);
 int64_t seg_lovasz_workspace_bytes(int64_t P, int n_present, int C);
 int seg_lovasz_softmax_nchw(const float* logits, const int64_t* target, int N, int C, int H, int W, int64_t ignore_index,

@@ -133,7 +133,8 @@ __global__ void __launch_bounds__(256) ce_nchw_bwd_kernel(const float* __restric
 
 // ---------------------------------------------------------------- Dice (utils/losses.py:33-50)
 // loss = 1 - (2*I + smooth) / (sum(softmax) + sum(onehot) + smooth),  I = sum_pixels softmax[target].
-// accum[0] += I, accum[1] += sum(softmax) (== #pixels up to rounding), accum[2] += #pixels (sum of the one-hot tensor).
+// accum[0] += I, accum[1] += #pixels.  Every softmax row sums to 1 and every pixel carries one label after the target
+// fix-up, so sum(softmax) and sum(onehot) both equal #pixels and D = 2 accum[1] + smooth (to within the softmax rounding).
 __global__ void __launch_bounds__(256) dice_nchw_fwd_kernel(const float* __restrict__ logits, const int64_t* __restrict__ target,
                                                             int N, int C, int H, int W, double* accum) {
   const int64_t HW = (int64_t)H * W, total = (int64_t)N * HW;
@@ -156,17 +157,15 @@ __global__ void __launch_bounds__(256) dice_nchw_fwd_kernel(const float* __restr
   block_accum2(inter, psum, accum);
 }
 
-// d loss / d logit_c = -(2 / D) * p_t * (delta_ct - p_c),  D = accum[1] + accum[2] + smooth
+// d loss / d logit_c = -(2 / D) * p_t * (delta_ct - p_c),  D = 2 accum[1] + smooth (see dice_nchw_fwd_kernel)
 __global__ void __launch_bounds__(256) dice_nchw_bwd_kernel(const float* __restrict__ logits, const int64_t* __restrict__ target,
                                                             int N, int C, int H, int W, const double* __restrict__ accum,
                                                             float smooth, const float* __restrict__ gscale,
                                                             float* __restrict__ dl, float beta) {
   const int64_t HW = (int64_t)H * W, total = (int64_t)N * HW;
-  const double I = accum[0], P = accum[1], T = accum[1];
-  const double D = P + T + (double)smooth;
+  const double D = accum[1] + accum[1] + (double)smooth;
   // d/dp_t of -(2I+s)/D with D depending on sum(p): the sum(p) term has zero gradient through softmax (rows sum to 1)
   const float g = (gscale ? *gscale : 1.f) * (float)(-2.0 / D);
-  (void)I;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
     const int64_t t = target[i];
     const int n = (int)(i / HW);

@@ -5,14 +5,18 @@
 // host sync (`fg.sum() == 0`).  Here every present class is handled at once, on the device:
 //   1. emit   : per valid pixel, softmax, then one 64-bit key per PRESENT class
 //                 [class rank : 8][~bits(|fg - p_c|) : 32][fg : 1][pixel index : 23]
-//               written to segment `rank` of a [n_present][P] array (slot order inside a segment is irrelevant).
+//               written to segment `rank` of a [n_present][P] array at slot = number of valid pixels before the pixel
+//               (per-chunk valid counts, an exclusive scan, a block-local rank), so every segment is in pixel order.
 //   2. sort   : one global LSD radix sort over bits 24..63 (5 passes x 8 bits: histogram, per-digit scan, stable
 //               scatter) -> each class segment sorted by error, descending; segments stay [rank*P, (rank+1)*P).
 //   3. jaccard: per class a tiled inclusive scan of the fg flags gives intersection / union at every rank, hence the
-//               Lovász gradient  d_i = J_i - J_{i-1};  loss_c = sum_i e_i d_i (fp64 accumulation), and
+//               Lovász gradient  d_i = J_i - J_{i-1};  loss_c = sum_i e_i d_i (fp64 per-tile partials), and
 //               dLoss/dp[pixel, c] = d_i * sign scattered into an NCHW scratch tensor.
-//   4. finish : loss = mean_c loss_c; the softmax Jacobian turns dLoss/dp into dLoss/dlogits in place.
-// Pure HBM-bound integer/byte work (no GEMM); ties in the sort do not change the loss value (telescoping sum).
+//   4. finish : loss = mean_c loss_c, folded from the tile partials in a fixed order; the softmax Jacobian turns dLoss/dp
+//               into dLoss/dlogits in place.
+// Pure HBM-bound integer/byte work (no GEMM).  Tie order: exactly tied errors take ranks in flat pixel order (the order a
+// stable sort of the reference's flattened error vector gives).  The loss value does not depend on it (the sum
+// telescopes) but the per-pixel gradient d_i does; a stable sort of pixel-ordered segments makes both reproducible.
 #include "seg_common.cuh"
 
 namespace seg {
@@ -50,15 +54,38 @@ __global__ void lv_rank_kernel(const int* __restrict__ counts, int C, int* __res
 }
 
 // ---------------------------------------------------------------- 1. softmax + key emission
-__global__ void __launch_bounds__(256)
+// Pixels are processed in chunks of LV_THREADS consecutive pixels, one chunk per block iteration (chunk j = pixels
+// [j*256, (j+1)*256)).  chunk_valid[j] = valid pixels of chunk j; lv_emit reads its exclusive scan.
+__global__ void __launch_bounds__(LV_THREADS)
+    lv_chunk_count_kernel(const int64_t* __restrict__ target, int64_t total, int64_t ignore, unsigned int* __restrict__ chunk_valid) {
+  const int64_t nchunks = ceil_div64(total, LV_THREADS);
+  for (int64_t ch = blockIdx.x; ch < nchunks; ch += gridDim.x) {
+    const int64_t i = ch * LV_THREADS + threadIdx.x;
+    const int n = __syncthreads_count(i < total && target[i] != ignore);
+    if (threadIdx.x == 0) chunk_valid[ch] = (unsigned int)n;
+  }
+}
+
+__global__ void __launch_bounds__(LV_THREADS)
     lv_emit_kernel(const float* __restrict__ logits, const int64_t* __restrict__ target, int N, int C, int H, int W,
                    int64_t ignore, const int* __restrict__ rank, long long P, unsigned long long* __restrict__ keys,
-                   unsigned int* __restrict__ slot_counter) {
+                   const unsigned int* __restrict__ chunk_off) {
   const int64_t HW = (int64_t)H * W, total = (int64_t)N * HW;
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-    const int64_t t = target[i];
-    if (t == ignore) continue;
-    const unsigned int slot = atomicAdd(slot_counter, 1u);
+  const int64_t nchunks = ceil_div64(total, LV_THREADS);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  __shared__ unsigned int wvalid[LV_THREADS / 32];
+  for (int64_t ch = blockIdx.x; ch < nchunks; ch += gridDim.x) {
+    const int64_t i = ch * LV_THREADS + threadIdx.x;
+    const int64_t t = i < total ? target[i] : ignore;
+    const bool ok = t != ignore;
+    // slot = valid pixels before chunk ch + valid pixels of this chunk before pixel i
+    const unsigned int ballot = __ballot_sync(0xffffffffu, ok);
+    if (lane == 0) wvalid[warp] = __popc(ballot);
+    __syncthreads();
+    unsigned int slot = chunk_off[ch] + __popc(ballot & ((1u << lane) - 1u));
+    for (int w = 0; w < warp; ++w) slot += wvalid[w];
+    __syncthreads();  // wvalid is rewritten by the next chunk
+    if (!ok) continue;
     const int n = (int)(i / HW);
     const float* l = logits + (int64_t)n * C * HW + (i - (int64_t)n * HW);
     float mx = -INFINITY;
@@ -229,7 +256,7 @@ __device__ __forceinline__ float lv_jaccard(float gts, float cumfg, float cumbg)
 __global__ void __launch_bounds__(256)
     lv_jaccard_kernel(const unsigned long long* __restrict__ keys, long long P, int tiles, const unsigned int* __restrict__ tile_off,
                       const unsigned int* __restrict__ gts_arr, const int* __restrict__ class_of_rank, int C, long long HW,
-                      double* __restrict__ loss_per_class, float* __restrict__ gprob /*NCHW scratch*/) {
+                      double* __restrict__ loss_part /*[n_present][tiles]*/, float* __restrict__ gprob /*NCHW scratch*/) {
   const int r = blockIdx.y, t = blockIdx.x;
   const long long cbase = (long long)r * P;
   const long long base = cbase + (long long)t * LV_JT;
@@ -283,7 +310,7 @@ __global__ void __launch_bounds__(256)
   if (threadIdx.x == 0) {
     double s = 0.0;
     for (int w = 0; w < 8; ++w) s += wsum[w];
-    atomicAdd(loss_per_class + r, s);
+    loss_part[(size_t)r * tiles + t] = s;
   }
 }
 
@@ -292,12 +319,26 @@ __global__ void lv_class_of_rank_kernel(const int* __restrict__ rank, int C, int
   if (c < C && rank[c] >= 0) class_of_rank[rank[c]] = c;
 }
 
-__global__ void lv_loss_kernel(const double* __restrict__ loss_per_class, int n_present, float* __restrict__ loss) {
-  if (threadIdx.x == 0 && blockIdx.x == 0) {
+// one block: loss_c = the tile partials of class c folded in a fixed order (strided per thread, then the warp and block
+// trees), loss = mean over the present classes; no atomics, so the value does not depend on the block schedule
+__global__ void __launch_bounds__(256) lv_loss_kernel(const double* __restrict__ loss_part, int n_present, int tiles,
+                                                      float* __restrict__ loss) {
+  __shared__ double wsum[8];
+  double total = 0.0;
+  for (int r = 0; r < n_present; ++r) {
     double s = 0.0;
-    for (int r = 0; r < n_present; ++r) s += loss_per_class[r];
-    *loss = n_present > 0 ? (float)(s / n_present) : 0.f;
+    for (int t = threadIdx.x; t < tiles; t += 256) s += loss_part[(size_t)r * tiles + t];
+    s = warp_sum_d(s);
+    if ((threadIdx.x & 31) == 0) wsum[threadIdx.x >> 5] = s;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      double c = 0.0;
+      for (int w = 0; w < 8; ++w) c += wsum[w];
+      total += c;
+    }
+    __syncthreads();
   }
+  if (threadIdx.x == 0) *loss = n_present > 0 ? (float)(total / n_present) : 0.f;
 }
 
 // ---------------------------------------------------------------- 4. softmax Jacobian, in place on the NCHW scratch
@@ -348,7 +389,7 @@ int seg_lovasz_count(const int64_t* target, int64_t npix, int C, int64_t ignore_
   return check_launch("lv_count");
 }
 
-// bytes of the integer workspace for P valid pixels and n_present classes (radix table + totals + tile sums + ...)
+// bytes of the workspace for P valid pixels and n_present classes (radix table + totals + tile sums + ...)
 int64_t seg_lovasz_workspace_bytes(int64_t P, int n_present, int C) {
   const int64_t nkeys = P * n_present;
   const int64_t nblocks = ceil_div64(nkeys, LV_TILE);
@@ -358,9 +399,9 @@ int64_t seg_lovasz_workspace_bytes(int64_t P, int n_present, int C) {
   b += 256 * 4 * 2;                       // totals + digit bases
   b += (int64_t)n_present * tiles * 4;    // tile sums / offsets
   b += (int64_t)n_present * 4;            // gts
-  b += (int64_t)n_present * 8;            // loss per class (fp64)
+  b += (int64_t)n_present * tiles * 8;    // loss per class and tile (fp64)
   b += (int64_t)C * 4 * 2;                // rank, class_of_rank
-  b += 64 + 16 * 16;                      // slot counter + alignment slack
+  b += 16 * 16;                           // alignment slack
   return b;
 }
 
@@ -390,23 +431,28 @@ int seg_lovasz_softmax_nchw(const float* logits, const int64_t* target, int N, i
   unsigned int* dbase = reinterpret_cast<unsigned int*>(take(256 * 4));
   unsigned int* tsum = reinterpret_cast<unsigned int*>(take((size_t)n_present * tiles * 4));
   unsigned int* gts = reinterpret_cast<unsigned int*>(take((size_t)n_present * 4));
-  double* lpc = reinterpret_cast<double*>(take((size_t)n_present * 8));
+  double* lpart = reinterpret_cast<double*>(take((size_t)n_present * tiles * 8));
   int* rank = reinterpret_cast<int*>(take((size_t)C * 4));
   int* cor = reinterpret_cast<int*>(take((size_t)C * 4));
-  unsigned int* slot = reinterpret_cast<unsigned int*>(take(16));
-  cudaMemsetAsync(slot, 0, 4, st);
-  cudaMemsetAsync(lpc, 0, (size_t)n_present * 8, st);
-  cudaMemsetAsync(dlogits, 0, (size_t)npix * C * sizeof(float), st);
 
   lv_rank_kernel<<<1, 32, 0, st>>>(counts, C, rank);
   if (check_launch("lv_rank")) return 1;
   lv_class_of_rank_kernel<<<ceil_div(C, 128), 128, 0, st>>>(rank, C, cor);
   if (check_launch("lv_class_of_rank")) return 1;
-  const int eb = (int)std::min<int64_t>(ceil_div64(npix, 256), (int64_t)num_sms() * 8);
+  // key slots: per-chunk valid counts and their exclusive scan, kept in dlogits (npix * C floats >= one word per chunk)
+  // until the emission has read them; dlogits is zeroed after it
+  const int64_t nchunks = ceil_div64(npix, LV_THREADS);
+  unsigned int* chunk_off = reinterpret_cast<unsigned int*>(dlogits);
+  const int eb = (int)std::min<int64_t>(nchunks, (int64_t)num_sms() * 8);
+  lv_chunk_count_kernel<<<eb, LV_THREADS, 0, st>>>(target, npix, ignore_index, chunk_off);
+  if (check_launch("lv_chunk_count")) return 1;
+  lv_radix_scan_rows_kernel<<<1, 1024, 0, st>>>(chunk_off, (int)nchunks, total);
+  if (check_launch("lv_chunk_scan")) return 1;
   unsigned long long* ka = reinterpret_cast<unsigned long long*>(keys0);
   unsigned long long* kb = reinterpret_cast<unsigned long long*>(keys1);
-  lv_emit_kernel<<<eb, 256, 0, st>>>(logits, target, N, C, H, W, ignore_index, rank, (long long)P, ka, slot);
+  lv_emit_kernel<<<eb, LV_THREADS, 0, st>>>(logits, target, N, C, H, W, ignore_index, rank, (long long)P, ka, chunk_off);
   if (check_launch("lv_emit")) return 1;
+  cudaMemsetAsync(dlogits, 0, (size_t)npix * C * sizeof(float), st);
   for (int pass = 0; pass < 5; ++pass) {
     const int shift = 24 + 8 * pass;
     lv_radix_hist_kernel<<<nblocks, LV_THREADS, 0, st>>>(ka, nkeys, shift, table, nblocks);
@@ -426,9 +472,9 @@ int seg_lovasz_softmax_nchw(const float* logits, const int64_t* target, int N, i
   if (check_launch("lv_tile_sums")) return 1;
   lv_class_scan_kernel<<<n_present, 1024, 0, st>>>(tsum, tiles, gts);
   if (check_launch("lv_class_scan")) return 1;
-  lv_jaccard_kernel<<<jg, 256, 0, st>>>(ka, (long long)P, tiles, tsum, gts, cor, C, HW, lpc, dlogits);
+  lv_jaccard_kernel<<<jg, 256, 0, st>>>(ka, (long long)P, tiles, tsum, gts, cor, C, HW, lpart, dlogits);
   if (check_launch("lv_jaccard")) return 1;
-  lv_loss_kernel<<<1, 32, 0, st>>>(lpc, n_present, loss);
+  lv_loss_kernel<<<1, 256, 0, st>>>(lpart, n_present, tiles, loss);
   if (check_launch("lv_loss")) return 1;
   lv_softmax_bwd_kernel<<<eb, 256, 0, st>>>(logits, target, N, C, H, W, ignore_index, rank, 1.f / (float)n_present, dlogits);
   return check_launch("lv_softmax_bwd");
