@@ -300,6 +300,15 @@ int seg_shuffle_loss_fwd(const void* logits_lo, int ldlo, const int64_t* target,
 int seg_shuffle_loss_bwd(const void* logits_lo, int ldlo, const int64_t* target, int N, int h, int w, int C, int r,
                          int64_t ignore_index, const float* weight, int kind, float gamma, int mean, const double* accum,
                          const float* gscale, void* dx, int lddx, void* stream);
+/* The same losses on logits that are already at the output resolution: UNetResnet's conv7 output (unet.py:204 +
+ * trainer.py:60), NHWC fp32 [N,H,W,C] with pitch ld (C <= 160), read in place; target int64 [N,H,W].  kind, weight, gamma,
+ * mean, accum, gscale and counters as for seg_shuffle_loss_* (these are its r = 1 instance over an fp32 map).
+ * Backward: dx (bf16 [N,H,W,lddx], channels C .. lddx-1 zero) written once per element: deterministic, no atomics. */
+int seg_nhwc_loss_fwd(const float* logits, int ld, const int64_t* target, int N, int H, int W, int C, int64_t ignore_index,
+                      const float* weight, int kind, float gamma, double* accum, int64_t* counters, void* stream);
+int seg_nhwc_loss_bwd(const float* logits, int ld, const int64_t* target, int N, int H, int W, int C, int64_t ignore_index,
+                      const float* weight, int kind, float gamma, int mean, const double* accum, const float* gscale, void* dx,
+                      int lddx, void* stream);
 /* DiceLoss (utils/losses.py:33-50): softmax over C, intersection with the one-hot target, whole-batch ratio.
  * accum (fp64 [2], zeroed by the caller) receives (sum p[target], #pixels); loss = 1 - (2I+s)/(2*#pixels+s).
  * The caller applies the reference's in-place target fix-up (losses.py:40-42) before calling. */

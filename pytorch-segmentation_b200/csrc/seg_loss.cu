@@ -408,8 +408,11 @@ __global__ void ce_grad_from_fixed_kernel(const unsigned long long* __restrict__
 // low-res element belongs to exactly one pixel, so the backward writes each gradient element once (no accumulation: the
 // result does not depend on the thread order) and zeroes the pad lanes r*r*C .. lddx-1.  MET: the eval_metrics counters,
 // counted as upsample_ce_kernel counts them (shared-memory histogram, one global atomic per non-zero bin).
-template <bool BWD, int K, bool MET = false>
-__global__ void __launch_bounds__(256) shuffle_ce_kernel(const __nv_bfloat16* __restrict__ lo, int ldlo,
+// T: the storage type of the map — bf16 for DUC_HDC's shuffle; fp32 at r = 1 for full-resolution NHWC logits (UNetResnet).
+__device__ __forceinline__ float logit_f(__nv_bfloat16 v) { return bf2f(v); }
+__device__ __forceinline__ float logit_f(float v) { return v; }
+template <bool BWD, int K, bool MET = false, typename T = __nv_bfloat16>
+__global__ void __launch_bounds__(256) shuffle_ce_kernel(const T* __restrict__ lo, int ldlo,
                                                          const int64_t* __restrict__ target, int N, int h, int w, int C, int r,
                                                          int64_t ignore, LossArgs la, double* accum,
                                                          const float* __restrict__ gscale, __nv_bfloat16* __restrict__ dx,
@@ -435,7 +438,7 @@ __global__ void __launch_bounds__(256) shuffle_ce_kernel(const __nv_bfloat16* __
     if (K == LOSS_FOCAL && !BWD) cnt += 1.0;
     const int64_t px = ((int64_t)n * h + oy / r) * w + ox / r;
     const int sub = (oy % r) * r + ox % r;
-    const __nv_bfloat16* z = lo + px * ldlo + sub;  // class c at z[c * rr]
+    const T* z = lo + px * ldlo + sub;  // class c at z[c * rr]
     __nv_bfloat16* d = BWD ? dx + px * lddx + sub : nullptr;
     if (BWD) {
       if (sub == 0)
@@ -450,7 +453,7 @@ __global__ void __launch_bounds__(256) shuffle_ce_kernel(const __nv_bfloat16* __
     float mx = -INFINITY;
     int am = 0;
     for (int c = 0; c < C; ++c) {
-      const float v = bf2f(z[c * rr]);
+      const float v = logit_f(z[c * rr]);
       if (v > mx) {
         mx = v;
         am = c;
@@ -458,7 +461,7 @@ __global__ void __launch_bounds__(256) shuffle_ce_kernel(const __nv_bfloat16* __
     }
     float se = 0.f, lt = 0.f;
     for (int c = 0; c < C; ++c) {
-      const float v = bf2f(z[c * rr]);
+      const float v = logit_f(z[c * rr]);
       se += expf(v - mx);
       if (c == tg) lt = v;
     }
@@ -482,7 +485,7 @@ __global__ void __launch_bounds__(256) shuffle_ce_kernel(const __nv_bfloat16* __
       const float inv = 1.f / se;
       const float gp = K == LOSS_CE ? g : g * pixel_grad_factor<K>(mx + logf(se) - lt, class_weight(la, tg, C), la.gamma);
       for (int c = 0; c < C; ++c) {
-        const float v = bf2f(z[c * rr]);
+        const float v = logit_f(z[c * rr]);
         d[c * rr] = f2bf((expf(v - mx) * inv - (c == tg ? 1.f : 0.f)) * gp);
       }
     }
@@ -614,25 +617,36 @@ static int shuffle_ce_check(int N, int h, int w, int C, int r, int ld) {
 static unsigned shuffle_ce_blocks(int N, int h, int w, int r) {
   return (unsigned)std::min<int64_t>(ceil_div64((int64_t)N * h * w * r * r, 256), (int64_t)num_sms() * 8);
 }
-template <int K>
+template <int K, typename T = __nv_bfloat16>
 static int shuffle_ce_fwd(const void* lo, int ldlo, const int64_t* target, int N, int h, int w, int C, int r, int64_t ignore_index,
                           LossArgs la, double* accum, int64_t* counters, cudaStream_t stream) {
   if (shuffle_ce_check(N, h, w, C, r, ldlo)) return 1;
   const bool met = counters != nullptr;
-  const auto kernel = met ? shuffle_ce_kernel<false, K, true> : shuffle_ce_kernel<false, K, false>;
+  const auto kernel = met ? shuffle_ce_kernel<false, K, true, T> : shuffle_ce_kernel<false, K, false, T>;
   kernel<<<shuffle_ce_blocks(N, h, w, r), 256, met ? (size_t)(3 * C + 2) * sizeof(unsigned int) : 0, stream>>>(
-      reinterpret_cast<const __nv_bfloat16*>(lo), ldlo, target, N, h, w, C, r, ignore_index, la, accum, nullptr, nullptr, 0,
+      reinterpret_cast<const T*>(lo), ldlo, target, N, h, w, C, r, ignore_index, la, accum, nullptr, nullptr, 0,
       reinterpret_cast<unsigned long long*>(counters));
   return check_launch(met ? "shuffle_ce_fwd_metrics" : "shuffle_ce_fwd");
 }
-template <int K>
+template <int K, typename T = __nv_bfloat16>
 static int shuffle_ce_bwd(const void* lo, int ldlo, const int64_t* target, int N, int h, int w, int C, int r, int64_t ignore_index,
                           LossArgs la, const double* accum, const float* gscale, void* dx, int lddx, cudaStream_t stream) {
   if (shuffle_ce_check(N, h, w, C, r, ldlo) || shuffle_ce_check(N, h, w, C, r, lddx)) return 1;
-  shuffle_ce_kernel<true, K><<<shuffle_ce_blocks(N, h, w, r), 256, 0, stream>>>(
-      reinterpret_cast<const __nv_bfloat16*>(lo), ldlo, target, N, h, w, C, r, ignore_index, la, const_cast<double*>(accum),
+  shuffle_ce_kernel<true, K, false, T><<<shuffle_ce_blocks(N, h, w, r), 256, 0, stream>>>(
+      reinterpret_cast<const T*>(lo), ldlo, target, N, h, w, C, r, ignore_index, la, const_cast<double*>(accum),
       gscale, reinterpret_cast<__nv_bfloat16*>(dx), lddx, nullptr);
   return check_launch("shuffle_ce_bwd");
+}
+// full-resolution NHWC fp32 logits: the shuffle loss at r = 1 over an fp32 map
+template <int K>
+static int nhwc_ce_fwd(const float* logits, int ld, const int64_t* target, int N, int H, int W, int C, int64_t ignore_index,
+                       LossArgs la, double* accum, int64_t* counters, cudaStream_t stream) {
+  return shuffle_ce_fwd<K, float>(logits, ld, target, N, H, W, C, 1, ignore_index, la, accum, counters, stream);
+}
+template <int K>
+static int nhwc_ce_bwd(const float* logits, int ld, const int64_t* target, int N, int H, int W, int C, int64_t ignore_index,
+                       LossArgs la, const double* accum, const float* gscale, void* dx, int lddx, cudaStream_t stream) {
+  return shuffle_ce_bwd<K, float>(logits, ld, target, N, H, W, C, 1, ignore_index, la, accum, gscale, dx, lddx, stream);
 }
 
 // kind: LOSS_CE (weight NULL, a mean), LOSS_WCE (NULL weight = ones) or LOSS_FOCAL (weight optional)
@@ -720,6 +734,21 @@ int seg_shuffle_loss_bwd(const void* logits_lo, int ldlo, const int64_t* target,
   LossArgs la;
   if (loss_args(weight, kind, gamma, mean, C, &la)) return 1;
   return SEG_LOSS_DISPATCH(kind, shuffle_ce_bwd, logits_lo, ldlo, target, N, h, w, C, r, ignore_index, la, accum, gscale, dx, lddx,
+                           ST(stream));
+}
+
+int seg_nhwc_loss_fwd(const float* logits, int ld, const int64_t* target, int N, int H, int W, int C, int64_t ignore_index,
+                      const float* weight, int kind, float gamma, double* accum, int64_t* counters, void* stream) {
+  LossArgs la;
+  if (loss_args(weight, kind, gamma, 1, C, &la)) return 1;
+  return SEG_LOSS_DISPATCH(kind, nhwc_ce_fwd, logits, ld, target, N, H, W, C, ignore_index, la, accum, counters, ST(stream));
+}
+int seg_nhwc_loss_bwd(const float* logits, int ld, const int64_t* target, int N, int H, int W, int C, int64_t ignore_index,
+                      const float* weight, int kind, float gamma, int mean, const double* accum, const float* gscale, void* dx,
+                      int lddx, void* stream) {
+  LossArgs la;
+  if (loss_args(weight, kind, gamma, mean, C, &la)) return 1;
+  return SEG_LOSS_DISPATCH(kind, nhwc_ce_bwd, logits, ld, target, N, H, W, C, ignore_index, la, accum, gscale, dx, lddx,
                            ST(stream));
 }
 

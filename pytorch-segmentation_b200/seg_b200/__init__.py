@@ -11,6 +11,7 @@ _LAZY = {
     "PSPNet": ("nets", "PSPNet"),
     "UperNet": ("nets", "UperNet"),
     "DeepLab_DUC_HDC": ("nets", "DeepLab_DUC_HDC"),
+    "UNetResnet": ("nets", "UNetResnet"),
     "CrossEntropyLoss2d": ("losses", "CrossEntropyLoss2d"),
     "DiceLoss": ("losses", "DiceLoss"),
     "FocalLoss": ("losses", "FocalLoss"),

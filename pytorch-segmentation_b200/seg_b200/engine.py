@@ -14,7 +14,7 @@ Conventions
 import torch
 
 from . import ops
-from .lib import IMPL_AUTO
+from .lib import IMPL_AUTO, IMPL_TC
 
 BN_EPS = 1e-5
 BN_MOM = 0.1
@@ -47,13 +47,23 @@ class Act:
 
 
 class ConvSpec:
-    """Static description of one nn.Conv2d holder + its packed bf16 weight cache."""
+    """Static description of one nn.Conv2d (or nn.ConvTranspose2d) holder + its packed bf16 weight cache.
+
+    A ConvTranspose2d(Cin -> Cout, k, s, p) weight [Cin, Cout, k, k] is read as the OIHW weight of the Conv2d(Cout -> Cin, k,
+    s, p) whose data gradient the transposed conv is (`transposed`; K = Cin, C = Cout): packing, the batched pack / unpack
+    tables and the packed weight gradient [k*k][Cin][Cout] are those of that conv, unchanged."""
 
     def __init__(self, name, module, explicit_im2col=False):
         self.name = name
         self.m = module
         w = module.weight
         self.K, self.C, self.R, self.S = w.shape
+        self.transposed = bool(getattr(module, "transposed", False))
+        if self.transposed and (module.groups != 1 or tuple(module.dilation) != (1, 1) or tuple(module.output_padding) != (0, 0)
+                                or module.bias is not None or self.R != self.S or module.stride[0] != module.stride[1]
+                                or module.padding[0] != module.padding[1] or self.C % 8 != 0):
+            raise NotImplementedError(f"{name}: the engine's ConvTranspose2d is square, groups 1, dilation 1, output_padding 0, "
+                                      f"no bias, with a multiple of 8 output channels (got {module!r})")
         assert module.stride[0] == module.stride[1] and module.padding[0] == module.padding[1]
         assert module.dilation[0] == module.dilation[1] and module.groups == 1
         self.explicit = explicit_im2col or (self.C % 8 != 0)
@@ -271,6 +281,40 @@ class Tape:
                 ya.grad = None
             self._push_back(bwd, (spec.m.weight, bias))
         return ya, stats
+
+    def conv_transpose(self, x, spec, out=None):
+        """nn.ConvTranspose2d (spec.transposed) of x [N,h,w,Cin] -> [N,(h-1)s-2p+k,(w-1)s-2p+k,Cout]; `out` may be a concat slice.
+        forward = the dgrad of the Conv2d(Cout -> Cin) (its stride-s parity classes write the strided sub-grids of the
+        output), data gradient = that conv's fprop over dY, weight gradient = its wgrad with the operands swapped.  The
+        wgmma kernels run these shapes; AUTO therefore asks for them (IMPL_TC), so an unsupported call raises instead of
+        silently taking the CUDA-core path."""
+        assert spec.transposed
+        wp = self.packed_override.get(spec)
+        if wp is None:
+            wp = spec.packed()
+        impl = IMPL_TC if self.impl == IMPL_AUTO else self.impl
+        k, s, p = spec.R, spec.stride, spec.pad
+        N, h, w, _ = x.t.shape
+        y_shape = (N, (h - 1) * s - 2 * p + k, (w - 1) * s - 2 * p + k, spec.C)
+        y = ops.conv2d_dgrad(x.t, wp, y_shape, k, k, s, p, 1, out=out, impl=impl)
+        ya = Act(y)
+        if self.record:
+            def bwd():
+                dy = ya.grad
+                if dy is None:
+                    return
+                if spec.m.weight.requires_grad and spec in self.dw_buffers:
+                    ops.conv2d_wgrad(x.t, dy, k, k, s, p, 1, out=self.dw_buffers[spec], impl=impl)
+                    self.touched.add(spec.m.weight)
+                elif spec.m.weight.requires_grad:
+                    dwp = ops.conv2d_wgrad(x.t, dy, k, k, s, p, 1, impl=impl)
+                    self._param_grad(spec.m.weight, lambda g, beta: ops.unpack_wgrad(dwp, tuple(spec.m.weight.shape), beta=beta, out=g))
+                if x.needs_grad:
+                    gx, beta = x.grad_target()
+                    ops.conv2d_fwd(dy, wp, spec.K, k, k, s, p, 1, out=gx, beta=beta, impl=impl)
+                ya.grad = None
+            self._push_back(bwd, (spec.m.weight,))
+        return ya
 
     def dwconv(self, x, spec, want_stats=False):
         """Depthwise 3x3 (SeparableConv2d.conv1).  Returns (raw output Act, BN statistics or None)."""
@@ -524,6 +568,15 @@ class Tape:
             off += c
         whole._written = False  # the consumer's dgrad overwrites (beta = 0) the pre-allocated buffer
 
+    def shared_slice(self, act):
+        """`act` was produced into a concat slice (and bound by `bind_slices`) and has consumers of its own besides the
+        concat's (a skip connection taken from the residual stream).  Call right after `bind_slices`: in the backward this
+        runs once the concat's consumer has written the slice (beta = 0), so act's own consumers then ADD to it."""
+        if self.record:
+            def bwd():
+                act._written = True
+            self.back.append(bwd)
+
 
 # ---------------------------------------------------------------------- output heads
 # A head owns how a model's last tape activation becomes the full-resolution NCHW fp32 logits `model(x)` returns, and the
@@ -583,3 +636,31 @@ class ShuffleHead:
     def loss_bwd(self, target, ignore_index, accum, weight, gamma, mean, gscale=None):
         dx = ops.shuffle_loss_bwd(self.act.t, self.r, target, ignore_index, accum, self._ld(), weight, gamma, mean, gscale=gscale)
         self.act.grad = dx[..., : self.act.t.shape[-1]]
+
+
+class FullResHead:
+    """NHWC fp32 logits [N,H,W,C] (a pitch is allowed) already at the output resolution (UNetResnet's conv7, unet.py:204)."""
+
+    def __init__(self, act):
+        self.act = act
+
+    @property
+    def classes(self):
+        return self.act.t.shape[-1]
+
+    def _ld(self):
+        return (self.classes + 7) // 8 * 8
+
+    def logits(self):
+        return ops.nhwc_to_nchw_f32(self.act.t)
+
+    def logits_bwd(self, dout):
+        # the NCHW fp32 -> NHWC bf16 transpose with zero pad lanes is the pixel shuffle's at r = 1
+        self.act.grad = ops.pixel_shuffle_logits_bwd(dout, 1, self._ld())[..., : self.classes]
+
+    def loss_fwd(self, target, ignore_index, weight, gamma, mean, reduce_fn=None, counters=None):
+        return ops.nhwc_loss_fwd(self.act.t, target, ignore_index, weight, gamma, mean, reduce_fn=reduce_fn, counters=counters)
+
+    def loss_bwd(self, target, ignore_index, accum, weight, gamma, mean, gscale=None):
+        dx = ops.nhwc_loss_bwd(self.act.t, target, ignore_index, accum, self._ld(), weight, gamma, mean, gscale=gscale)
+        self.act.grad = dx[..., : self.classes]

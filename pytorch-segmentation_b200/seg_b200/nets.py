@@ -4,6 +4,7 @@
     PSPNet (num_classes, in_channels=3, backbone='resnet152', pretrained=None, use_aux=True,   freeze_bn=False, **_)
     UperNet(num_classes, in_channels=3, backbone='resnet101', pretrained=None, use_aux=True, fpn_out=256, freeze_bn=False, **_)
     DeepLab_DUC_HDC(num_classes, in_channels=3, pretrained=None, output_stride=8, freeze_bn=False, **_)
+    UNetResnet(num_classes, in_channels=3, backbone='resnet50', pretrained=None, freeze_bn=False, **_)
 
 (default backbones are the reference's; `pretrained`: the reference defaults to True and downloads ImageNet weights — there is
 no network here, so an explicit True raises and the default (None) initialises randomly with a logged warning)
@@ -28,7 +29,7 @@ import torch
 import torch.nn as nn
 
 from . import ops
-from .engine import Act, BilinearHead, ConvSpec, DwSpec, ShuffleHead, Tape
+from .engine import Act, BilinearHead, ConvSpec, DwSpec, FullResHead, ShuffleHead, Tape
 from .lib import IMPL_AUTO, require_device
 
 try:  # inside the reference tree: subclass its BaseModel so isinstance checks and logging behave identically
@@ -484,8 +485,9 @@ class _EngineModel(BaseModel):
         return s
 
     def all_conv_specs(self):
-        """ConvSpec of every dense nn.Conv2d holder (names = module paths, as used by the forward code)."""
-        return [self._spec(n, m) for n, m in self.named_modules() if isinstance(m, nn.Conv2d) and m.groups == 1]
+        """ConvSpec of every dense nn.Conv2d / nn.ConvTranspose2d holder (names = module paths, as used by the forward code)."""
+        return [self._spec(n, m) for n, m in self.named_modules()
+                if isinstance(m, (nn.Conv2d, nn.ConvTranspose2d)) and m.groups == 1]
 
     def all_dw_specs(self):
         return [self._dwspec(n, m) for n, m in self.named_modules() if isinstance(m, nn.Conv2d) and m.groups > 1]
@@ -549,13 +551,13 @@ class _EngineModel(BaseModel):
         y, st = tape.conv(x, self._spec(name, conv), want_stats=True)
         return tape.bn_act(y, bn, st, relu=relu, res=res, out=out, drop_p=drop_p, drop_channelwise=drop_channelwise)
 
-    def _block(self, tape, x, prefix, blk):
+    def _block(self, tape, x, prefix, blk, out=None):
         a = self._cbr(tape, x, prefix + "conv1", blk.conv1, blk.bn1)
         a = self._cbr(tape, a, prefix + "conv2", blk.conv2, blk.bn2)
         r = x
         if blk.downsample is not None:
             r = self._cbr(tape, x, prefix + "downsample.0", blk.downsample[0], blk.downsample[1], relu=False)
-        return self._cbr(tape, a, prefix + "conv3", blk.conv3, blk.bn3, relu=True, res=r)
+        return self._cbr(tape, a, prefix + "conv3", blk.conv3, blk.bn3, relu=True, res=r, out=out)
 
     def _finish(self, tape):
         if tape.bn_modules:
@@ -1058,3 +1060,111 @@ class DeepLab_DUC_HDC(_EngineModel):
 
     def get_decoder_params(self):
         return chain(self.ASSP.parameters(), self.decoder.parameters(), self.DUC_out.parameters())
+
+
+# ----------------------------------------------------------------------------------------------- UNetResnet
+class UNetResnet(_EngineModel):
+    """U-Net decoder over the deep-stem dilated ResNet — replaces models/unet.py:126-209.  The trunk is PSPNet's (`initial`
+    = deep stem + bn1 + ReLU + max-pool, layer3 / layer4 at stride 1 with dilations 2 / 4: x2, x3 and x4 are all at 1/8).
+    Decoder: convs WITH bias and no BN / ReLU, ConvTranspose2d(4, 2, 1) x2 upsamplings, bilinear(align_corners=True)
+    resamples to each skip's size, concat (upsampled, skip), and conv7 (1x1, no bias) on a map at input resolution: the
+    model returns full-resolution logits for any input size (a 65x65 input reaches 68x68 after upconv5 and is resampled).
+    Quirks kept: initialize_weights runs over the whole model (trunk included: kaiming-normal convs, BN gamma 1 / beta
+    1e-4); conv biases and the ConvTranspose2d weights keep PyTorch's default initialisation.
+    The skips x1, x2, x3 are written by the trunk straight into the concat buffers' second slices and read from there by
+    the next trunk stage; the x2 upsamplings write into the first slices (directly when no resample is needed)."""
+
+    DECODER = (("conv1", 2048, 192), ("upconv1", 192, 128), ("conv2", 1152, 128), ("upconv2", 128, 96), ("conv3", 608, 96),
+               ("upconv3", 96, 64), ("conv4", 320, 64), ("upconv4", 64, 48), ("conv5", 48, 48), ("upconv5", 48, 32),
+               ("conv6", 32, 32))
+    UP_CHANNELS = {3: 128, 2: 96, 1: 64}  # channels of the upsampled slice of the concat at skip x_i (upconv1, 2, 3)
+
+    def __init__(self, num_classes, in_channels=3, backbone="resnet50", pretrained=None, freeze_bn=False, freeze_backbone=False,
+                 **_):
+        super().__init__()
+        if backbone not in RESNET_BLOCKS:
+            raise NotImplementedError(f"seg_b200.UNetResnet: backbone {backbone!r} not built (the decoder expects the 2048 "
+                                      f"channels of resnet50/101/152)")
+        _check_pretrained(self, pretrained)
+        if in_channels != 3:
+            raise NotImplementedError("in_channels != 3 swaps the deep stem for a 64-channel 7x7 conv that bn1 cannot take "
+                                      "(unet.py:131-132); not built")
+        self.num_classes = num_classes
+        s1, n1 = _cbn(3, 64, 3, 2, 1)
+        s2, n2 = _cbn(64, 64, 3, 1, 1)
+        s3 = nn.Conv2d(64, 128, 3, stride=1, padding=1, bias=False)
+        stem = nn.Sequential(s1, n1, nn.ReLU(inplace=True), s2, n2, nn.ReLU(inplace=True), s3)
+        self.initial = nn.Sequential(stem, nn.BatchNorm2d(128), nn.ReLU(inplace=True), nn.MaxPool2d(kernel_size=3, stride=2, padding=1))
+        plan = [(1, 1, 1), (2, 1, 1), (1, 1, 2), (1, 2, 4)]  # resnet.py:190-210, as PSPNet
+        self.layer1, self.layer2, self.layer3, self.layer4 = _res_layers(RESNET_BLOCKS[backbone], 128, plan)
+        for name, cin, cout in self.DECODER:
+            if name.startswith("up"):
+                setattr(self, name, nn.ConvTranspose2d(cin, cout, 4, 2, 1, bias=False))
+            else:
+                setattr(self, name, nn.Conv2d(cin, cout, kernel_size=3, stride=1, padding=1))
+        self.conv7 = nn.Conv2d(32, num_classes, kernel_size=1, bias=False)
+        _init_like_reference_head(self)
+        if freeze_bn:
+            self.freeze_bn()
+        if freeze_backbone:
+            for p in self.get_backbone_params():
+                p.requires_grad = False
+
+    def _conv(self, tape, x, name):
+        y, _ = tape.conv(x, self._spec(name, getattr(self, name)))
+        return y
+
+    def _up(self, tape, x, name, skip_hw, out):
+        """upconvN (x2), resampled to the skip's size (bilinear, align_corners=True) unless it already has it, into `out`."""
+        spec = self._spec(name, getattr(self, name))
+        h, w = x.t.shape[1], x.t.shape[2]
+        if (2 * h, 2 * w) == tuple(skip_hw):  # bilinear at equal size with align_corners=True is the identity
+            return tape.conv_transpose(x, spec, out=out)
+        return tape.bilinear(tape.conv_transpose(x, spec), skip_hw[0], skip_hw[1], True, out=out)
+
+    def _forward_heads(self, tape, x):
+        N, H, W = x.shape[0], x.shape[2], x.shape[3]
+        dev = x.device
+        stem = self.initial[0]
+        a = self._cbr(tape, x, "initial.0.0", stem[0], stem[1])
+        a = self._cbr(tape, a, "initial.0.3", stem[3], stem[4])
+        a = self._cbr(tape, a, "initial.0.6", stem[6], self.initial[1])
+        a = tape.maxpool(a)
+        # concat buffers (upsampled, skip) at the sizes of x1, x2, x3: the last block of layers 1-3 writes its output into
+        # the skip slice, and the next layer reads it from there
+        cats, skips = {}, {}
+        for li in (1, 2, 3, 4):
+            layer = getattr(self, f"layer{li}")
+            out = None
+            if li < 4:
+                s = layer[0].conv2.stride[0]
+                h, w = (a.t.shape[1] - 1) // s + 1, (a.t.shape[2] - 1) // s + 1
+                cout = layer[-1].conv3.out_channels
+                cats[li] = tape.concat(N, h, w, [self.UP_CHANNELS[li], cout], dev)
+                out = cats[li][1][1]
+            for bi, blk in enumerate(layer):
+                a = self._block(tape, a, f"layer{li}.{bi}.", blk, out=out if bi == len(layer) - 1 else None)
+            if li < 4:
+                skips[li] = a
+        y = self._conv(tape, a, "conv1")
+        for li, (up, conv) in zip((3, 2, 1), (("upconv1", "conv2"), ("upconv2", "conv3"), ("upconv3", "conv4"))):
+            whole, sl = cats[li]
+            skip = skips[li]
+            u = self._up(tape, y, up, skip.t.shape[1:3], sl[0])
+            tape.bind_slices(whole, [u, skip])
+            tape.shared_slice(skip)  # the skip also feeds the next trunk layer: its two gradients add
+            y = self._conv(tape, whole, conv)
+        y = self._conv(tape, tape.conv_transpose(y, self._spec("upconv4", self.upconv4)), "conv5")
+        y = tape.conv_transpose(y, self._spec("upconv5", self.upconv5))
+        if (y.t.shape[1], y.t.shape[2]) != (H, W):  # unet.py:201-202
+            y = tape.bilinear(y, H, W, True)
+        y = self._conv(tape, y, "conv6")
+        lo, _ = tape.conv(y, self._spec("conv7", self.conv7), out_dtype=torch.float32)
+        return [FullResHead(lo)]
+
+    def get_backbone_params(self):
+        return chain(self.initial.parameters(), self.layer1.parameters(), self.layer2.parameters(), self.layer3.parameters(),
+                     self.layer4.parameters())
+
+    def get_decoder_params(self):
+        return chain(*(getattr(self, n).parameters() for n, _, _ in self.DECODER), self.conv7.parameters())

@@ -629,6 +629,40 @@ def shuffle_loss_bwd(logits_lo, r, target, ignore_index, accum, ldx, weight=None
     return dx
 
 
+def _nhwc_loss_shapes(logits, target):
+    N, H, W, C = logits.shape
+    assert logits.dtype == torch.float32 and target.dtype == torch.int64 and target.is_contiguous()
+    if tuple(target.shape) != (N, H, W):
+        raise ValueError(f"target size {tuple(target.shape[1:])} differs from the model output size {(H, W)}")
+    return N, H, W, C
+
+
+def nhwc_loss_fwd(logits, target, ignore_index, weight=None, gamma=None, mean=True, reduce_fn=None, counters=None):
+    """loss_nchw_fwd on full-resolution NHWC fp32 logits [N,H,W,C] (a pitch is allowed), read in place; returns (loss, accum).
+    counters: as for upsample_loss_fwd."""
+    N, H, W, C = _nhwc_loss_shapes(logits, target)
+    assert weight is None or (weight.dtype == torch.float32 and weight.numel() == C and weight.is_contiguous())
+    if counters is not None:
+        _check_counters(counters, C)
+    accum = torch.zeros(2, dtype=torch.float64, device=logits.device)
+    call("seg_nhwc_loss_fwd", ptr(logits), ld(logits), ptr(target), N, H, W, C, int(ignore_index), ptr(weight),
+         _loss_kind(weight, gamma, mean), float(gamma or 0.0), ptr(accum), ptr(counters))
+    if reduce_fn is not None:
+        reduce_fn(accum)
+    loss = torch.empty((), dtype=torch.float32, device=logits.device)
+    call("seg_loss_finalize", ptr(accum), int(mean), ptr(loss))
+    return loss, accum
+
+
+def nhwc_loss_bwd(logits, target, ignore_index, accum, ldx, weight=None, gamma=None, mean=True, gscale=None):
+    """Gradient of nhwc_loss_fwd's loss w.r.t. the logits: bf16 [N,H,W,ldx] (channels C.. zero)."""
+    N, H, W, C = _nhwc_loss_shapes(logits, target)
+    dx = torch.empty((N, H, W, ldx), dtype=torch.bfloat16, device=logits.device)
+    call("seg_nhwc_loss_bwd", ptr(logits), ld(logits), ptr(target), N, H, W, C, int(ignore_index), ptr(weight),
+         _loss_kind(weight, gamma, mean), float(gamma or 0.0), int(mean), ptr(accum), ptr(gscale), ptr(dx), ldx)
+    return dx
+
+
 # ---------------------------------------------------------------- misc
 def nhwc_to_nchw_f32(x):
     N, H, W, C = x.shape
