@@ -164,6 +164,93 @@ __device__ __forceinline__ void stage_acc(const float* acc, const float* acc1, u
 
 // ================================ fprop / dgrad: persistent ping-pong kernel ================================
 
+// Epilogue phase 3 of conv_gemm_pp: the staged 128 x BN tile (XOR-swizzled, ESIZE-byte elements) -> global memory in 16-byte
+// chunks, optionally beta-accumulated onto the old values, optionally onto a strided sub-grid.  128 is a multiple of the
+// chunks per row, so each thread keeps one chunk column and walks every (128 / CPR)-th row.  Whole bf16 chunks under
+// beta != 0 go in batches of 8 rows whose old values are all loaded before the first store of the batch: distinct rows never
+// share an address, but the compiler cannot see that, and issued one by one the loads would cost a tile one global-load
+// latency per row.  The arithmetic is that of the one-chunk path: staged bf16 -> fp32, + beta * old, rounded once.
+template <int BN, int ESIZE>
+__device__ __forceinline__ void store_tile(const TcParams& p, const uint8_t* stage, int tid, int m0, int n0, int ncols_tile) {
+  constexpr int CPR = BN * ESIZE / 16;  // 16-byte chunks per staged row
+  constexpr int swz = (CPR >= 32 ? 31 : CPR - 1);
+  constexpr int RSTEP = 128 / CPR;      // rows between two chunks of a thread
+  constexpr int NCH = BM / RSTEP;       // chunks per thread
+  constexpr int BATCH = 8;
+  static_assert(128 % CPR == 0 && NCH % BATCH == 0, "chunk walk of the staged tile");
+  const int c16 = tid % CPR;
+  const int nchunks = (ncols_tile * ESIZE + 15) >> 4;  // 16-byte chunks that hold valid data
+  if (c16 >= nchunks) return;
+  const bool vec_ok = ((p.ldo * ESIZE) & 15) == 0 && ((reinterpret_cast<uintptr_t>(p.out) + (size_t)n0 * ESIZE) & 15) == 0;
+  const int first_col = (c16 << 4) / ESIZE;
+  const bool full = first_col + 16 / ESIZE <= ncols_tile;
+  auto row_dst = [&](int tr) {
+    const int grow = m0 + tr;
+    long long pixel = grow;
+    if (p.out_strided) {
+      const int n = grow / p.PQ;
+      const int rem = grow - n * p.PQ;
+      const int i = rem / p.Q, jj = rem - i * p.Q;
+      pixel = ((long long)n * p.out_H + (i * p.osy + p.opy)) * p.out_W + (jj * p.osx + p.opx);
+    }
+    return reinterpret_cast<uint8_t*>(p.out) + ((size_t)pixel * p.ldo + n0) * ESIZE + ((size_t)c16 << 4);
+  };
+  auto row_src = [&](int tr) { return stage + (size_t)tr * (BN * ESIZE) + ((c16 ^ (tr & swz)) << 4); };
+  if (ESIZE == 2 && vec_ok && full && p.beta != 0.f) {
+    // whole bf16 chunks, beta-accumulated
+    for (int b = 0; b < NCH; b += BATCH) {
+      uint8_t* dst[BATCH];
+      uint4 old[BATCH];
+#pragma unroll
+      for (int u = 0; u < BATCH; ++u) {
+        const int tr = tid / CPR + (b + u) * RSTEP;
+        dst[u] = m0 + tr < p.M ? row_dst(tr) : nullptr;
+        old[u] = dst[u] ? *reinterpret_cast<const uint4*>(dst[u]) : make_uint4(0u, 0u, 0u, 0u);
+      }
+#pragma unroll
+      for (int u = 0; u < BATCH; ++u) {
+        if (!dst[u]) continue;
+        float a[8], o[8];
+        unpack8(*reinterpret_cast<const bf16x8*>(row_src(tid / CPR + (b + u) * RSTEP)), a);
+        unpack8(*reinterpret_cast<const bf16x8*>(&old[u]), o);
+#pragma unroll
+        for (int k = 0; k < 8; ++k) a[k] += p.beta * o[k];
+        *reinterpret_cast<bf16x8*>(dst[u]) = pack8(a);
+      }
+    }
+    return;
+  }
+  // one chunk at a time: stores without beta, partial chunks, unaligned pitches and fp32 outputs
+  for (int tr = tid / CPR; tr < BM; tr += RSTEP) {
+    if (m0 + tr >= p.M) break;
+    const uint8_t* src = row_src(tr);
+    uint8_t* dst = row_dst(tr);
+    if (ESIZE == 2 && vec_ok && full) {
+      *reinterpret_cast<bf16x8*>(dst) = *reinterpret_cast<const bf16x8*>(src);  // beta == 0 here
+    } else if (ESIZE == 2) {
+      float a[8];
+      unpack8(*reinterpret_cast<const bf16x8*>(src), a);
+      __nv_bfloat16* d = reinterpret_cast<__nv_bfloat16*>(dst);
+      for (int k = 0; k < 8; ++k)
+        if (first_col + k < ncols_tile) {
+          float o = a[k];
+          if (p.beta != 0.f) o += p.beta * bf2f(d[k]);
+          d[k] = f2bf(o);
+        }
+    } else {
+      const float4 val = *reinterpret_cast<const float4*>(src);
+      const float a[4] = {val.x, val.y, val.z, val.w};
+      float* d = reinterpret_cast<float*>(dst);
+      if (vec_ok && full && p.beta == 0.f) {
+        *reinterpret_cast<float4*>(d) = val;
+      } else {
+        for (int k = 0; k < 4; ++k)
+          if (first_col + k < ncols_tile) d[k] = (p.beta != 0.f) ? a[k] + p.beta * d[k] : a[k];
+      }
+    }
+  }
+}
+
 // Ring depth per tile width.  Each consumer has a private staging tile of 128 rows x 256 B (BN * esize <= 256: fp32 outputs
 // take BN = 64) and a private statistics scratch, because the ring never idles and cannot double as the staging area.
 template <int BN>
@@ -310,12 +397,27 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_gemm_pp(const __grid_constan
       if (part < parts) {
         const int byte = c * esize;
         int g = part * rpp / p.stat_rows;
+        auto load = [&](int r) {
+          const uint8_t* src = stage + (size_t)r * (BN * esize) + ((((byte >> 4) ^ (r & swz))) << 4) + (byte & 15);
+          return out_f32 ? *reinterpret_cast<const float*>(src) : bf2f(*reinterpret_cast<const __nv_bfloat16*>(src));
+        };
         for (int rg = part * rpp; rg < (part + 1) * rpp; rg += p.stat_rows, ++g) {
           float s1 = 0.f, s2 = 0.f;
           const int rend = min(rg + p.stat_rows, rvalid);
-          for (int r = rg; r < rend; ++r) {
-            const uint8_t* src = stage + (size_t)r * (BN * esize) + ((((byte >> 4) ^ (r & swz))) << 4) + (byte & 15);
-            const float x = out_f32 ? *reinterpret_cast<const float*>(src) : bf2f(*reinterpret_cast<const __nv_bfloat16*>(src));
+          int r = rg;
+          // rows in batches of 8: the loads of a batch are issued before its adds, which keep the row order
+          for (; r + 8 <= rend; r += 8) {
+            float x[8];
+#pragma unroll
+            for (int u = 0; u < 8; ++u) x[u] = load(r + u);
+#pragma unroll
+            for (int u = 0; u < 8; ++u) {
+              s1 += x[u];
+              s2 = fmaf(x[u], x[u], s2);
+            }
+          }
+          for (; r < rend; ++r) {
+            const float x = load(r);
             s1 += x;
             s2 = fmaf(x, x, s2);
           }
@@ -326,62 +428,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_gemm_pp(const __grid_constan
     }
 
     // -------- phase 3: coalesced 16-byte stores of the staged tile --------
-    {
-      const int nchunks = (ncols_tile * esize + 15) >> 4;  // 16-byte chunks that hold valid data
-      const bool vec_ok = ((p.ldo * esize) & 15) == 0 && ((reinterpret_cast<uintptr_t>(p.out) + (size_t)n0 * esize) & 15) == 0;
-      for (int idx = tid; idx < BM * CPR; idx += 128) {
-        const int tr = idx / CPR;
-        const int c16 = idx - tr * CPR;
-        if (c16 >= nchunks) continue;
-        const int grow = m0 + tr;
-        if (grow >= p.M) continue;
-        long long pixel = grow;
-        if (p.out_strided) {
-          const int n = grow / p.PQ;
-          const int rem = grow - n * p.PQ;
-          const int i = rem / p.Q, jj = rem - i * p.Q;
-          pixel = ((long long)n * p.out_H + (i * p.osy + p.opy)) * p.out_W + (jj * p.osx + p.opx);
-        }
-        const uint8_t* src = stage + (size_t)tr * (BN * esize) + ((c16 ^ (tr & swz)) << 4);
-        uint8_t* dst = reinterpret_cast<uint8_t*>(p.out) + ((size_t)pixel * p.ldo + n0) * esize + ((size_t)c16 << 4);
-        const int first_col = (c16 << 4) / esize;
-        const bool full = first_col + 16 / esize <= ncols_tile;
-        if (!out_f32) {
-          bf16x8 val = *reinterpret_cast<const bf16x8*>(src);
-          if (vec_ok && full) {
-            if (p.beta != 0.f) {
-              float a[8], b[8];
-              unpack8(val, a);
-              unpack8(*reinterpret_cast<const bf16x8*>(dst), b);
-#pragma unroll
-              for (int k = 0; k < 8; ++k) a[k] += p.beta * b[k];
-              val = pack8(a);
-            }
-            *reinterpret_cast<bf16x8*>(dst) = val;
-          } else {
-            float a[8];
-            unpack8(val, a);
-            __nv_bfloat16* d = reinterpret_cast<__nv_bfloat16*>(dst);
-            for (int k = 0; k < 8; ++k)
-              if (first_col + k < ncols_tile) {
-                float o = a[k];
-                if (p.beta != 0.f) o += p.beta * bf2f(d[k]);
-                d[k] = f2bf(o);
-              }
-          }
-        } else {
-          const float4 val = *reinterpret_cast<const float4*>(src);
-          const float a[4] = {val.x, val.y, val.z, val.w};
-          float* d = reinterpret_cast<float*>(dst);
-          if (vec_ok && full && p.beta == 0.f) {
-            *reinterpret_cast<float4*>(d) = val;
-          } else {
-            for (int k = 0; k < 4; ++k)
-              if (first_col + k < ncols_tile) d[k] = (p.beta != 0.f) ? a[k] + p.beta * d[k] : a[k];
-          }
-        }
-      }
-    }
+    if (out_f32)
+      store_tile<BN, 4>(p, stage, tid, m0, n0, ncols_tile);
+    else
+      store_tile<BN, 2>(p, stage, tid, m0, n0, ncols_tile);
     if (j == ntiles - 1 && tid == 0) pdl_trigger();  // the CTA's last tile is stored
 
     // -------- phase 4: this tile's column sums are added to the layer's totals with fp64 atomics.  Each contribution is an
