@@ -96,8 +96,9 @@ int seg_conv2d_wgrad(const seg_conv_desc* d, const void* dy, const void* x, floa
 /* ---- depthwise 3x3 (atrous) convolution: SeparableConv2d.conv1 of the Aligned-Xception backbone
  *      (models/deeplabv3_plus.py:77-78, groups = C).  desc: K == C, R = S = 3.  Packed weights: fp32 [9][C]. ---- */
 int64_t seg_dwconv_scratch_floats(int C);
-/* y = dw(x); stats (optional, fp64 [2C], zero at launch) += per-channel sum / sum of squares of y (exact fp64 accumulation);
- * sync / sync_ticket: as seg_conv2d_fwd */
+/* y = dw(x); stats (optional, fp64 [2C], zero at launch) += per-channel sum / sum of squares of y as stored (bf16-rounded)
+ * (exact fp64 accumulation); sync / sync_ticket: as seg_conv2d_fwd.  All four entry points refuse C or pitches that are
+ * not multiples of 8 and x / y / dy / dx base pointers that are not 16-byte aligned. */
 int seg_dwconv3x3_fwd(const seg_conv_desc* d, const void* x, const float* w9, void* y, double* stats,
                       const seg_sync_desc* sync, void* sync_ticket, void* stream);
 /* dx = beta*dx + dw^T(dy) */

@@ -96,8 +96,10 @@ __global__ void __launch_bounds__(256)
           for (int i = 0; i < 8; ++i) o[i] = fmaf(f[i], w[r * 3 + s][i], o[i]);
         }
       }
-      *reinterpret_cast<bf16x8*>(y + row * ldy + co) = pack8(o);
+      const bf16x8 v = pack8(o);
+      *reinterpret_cast<bf16x8*>(y + row * ldy + co) = v;
       if (stats) {
+        unpack8(v, o);  // the statistics are of y as stored (bf16-rounded): the values bn_apply normalises
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
           acc[0][i] += o[i];
@@ -252,9 +254,13 @@ extern "C" {
 // scratch of seg_dwconv3x3_bwd_weight: fp64 accumulators [9][C] + a ticket, as floats
 int64_t seg_dwconv_scratch_floats(int C) { return (int64_t)2 * 9 * C + 32; }
 
-static int dw_check(const seg_conv_desc* d) {
+// xs: the x-side tensor (x or dx), ys: the y-side tensor (y or dy).  Every load and store is a 16-byte bf16x8, so besides
+// C and the pitches the base pointers must be 16-byte aligned (a channel slice must start at a multiple of 8 channels).
+static int dw_check(const seg_conv_desc* d, const void* xs, const void* ys) {
   SEG_REQUIRE(d && d->R == 3 && d->S == 3 && d->K == d->C, "dwconv: 3x3 depthwise (K == C) only");
   SEG_REQUIRE(d->C % 8 == 0 && d->ldx % 8 == 0 && d->ldy % 8 == 0, "dwconv: C / pitches must be multiples of 8");
+  SEG_REQUIRE((reinterpret_cast<uintptr_t>(xs) & 15) == 0 && (reinterpret_cast<uintptr_t>(ys) & 15) == 0,
+              "dwconv: x / y / dy / dx base pointers must be 16-byte aligned (channel offset a multiple of 8)");
   const int P = (d->H + 2 * d->pad - d->dil * 2 - 1) / d->stride + 1, Q = (d->W + 2 * d->pad - d->dil * 2 - 1) / d->stride + 1;
   SEG_REQUIRE(P == d->P && Q == d->Q, "dwconv: output size mismatch");
   return 0;
@@ -262,7 +268,7 @@ static int dw_check(const seg_conv_desc* d) {
 
 int seg_dwconv3x3_fwd(const seg_conv_desc* d, const void* x, const float* w9, void* y, double* stats,
                       const seg_sync_desc* sync, void* sync_ticket, void* stream) {
-  if (dw_check(d)) return 1;
+  if (dw_check(d, x, y)) return 1;
   SEG_REQUIRE(!sync || (stats && sync_ticket && 4 * d->C <= sync->n_max), "dwconv fwd: SyncBN needs stats, a zeroed ticket and 4*C <= n_max");
   const int64_t M = (int64_t)d->N * d->P * d->Q;
   dwconv_fwd_kernel<<<dw_grid(M, d->C), 256, 0, ST(stream)>>>(CBF(x), d->ldx, w9, BF(y), d->ldy, d->N, d->H, d->W, d->C, d->P, d->Q,
@@ -272,7 +278,7 @@ int seg_dwconv3x3_fwd(const seg_conv_desc* d, const void* x, const float* w9, vo
 }
 
 int seg_dwconv3x3_bwd_data(const seg_conv_desc* d, const void* dy, const float* w9, void* dx, float beta, void* stream) {
-  if (dw_check(d)) return 1;
+  if (dw_check(d, dx, dy)) return 1;
   const int64_t M = (int64_t)d->N * d->H * d->W;
   dwconv_bwd_data_kernel<<<dw_grid(M, d->C), 256, 0, ST(stream)>>>(CBF(dy), d->ldy, w9, BF(dx), d->ldx, d->N, d->H, d->W, d->C,
                                                                    d->P, d->Q, d->stride, d->pad, d->dil, beta);
@@ -281,7 +287,7 @@ int seg_dwconv3x3_bwd_data(const seg_conv_desc* d, const void* dy, const float* 
 
 int seg_dwconv3x3_bwd_weight(const seg_conv_desc* d, const void* dy, const void* x, float* dw9, float beta, float* scratch,
                              void* stream) {
-  if (dw_check(d)) return 1;
+  if (dw_check(d, x, dy)) return 1;
   SEG_REQUIRE(scratch != nullptr && (reinterpret_cast<uintptr_t>(scratch) & 7) == 0,
               "dwconv bwd_weight: 8-byte aligned scratch of seg_dwconv_scratch_floats(C) floats required");
   const int64_t M = (int64_t)d->N * d->P * d->Q;

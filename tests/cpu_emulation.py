@@ -110,11 +110,12 @@ def _dw_w(w9):
 def dwconv_fwd(x, w9, stride=1, pad=1, dil=1, out=None, stats=None, sync=None, sync_ticket=None):
     C = x.shape[-1]
     y = F.conv2d(_nchw(x), _w_round(_dw_w(w9)), None, stride, pad, dil, groups=C).permute(0, 2, 3, 1)
-    if stats is not None:
-        stats[:C] += y.reshape(-1, C).sum(0)
-        stats[C:] += (y * y).reshape(-1, C).sum(0)
     if out is None:
         out = torch.empty(y.shape, dtype=ACT_DTYPE)
+    if stats is not None:  # sums of y AS STORED (rounded to the output type), as conv2d_fwd
+        ys = y.to(out.dtype).double()
+        stats[:C] += ys.reshape(-1, C).sum(0)
+        stats[C:] += (ys * ys).reshape(-1, C).sum(0)
     return _store(out, y)
 
 
