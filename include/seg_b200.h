@@ -347,7 +347,8 @@ int seg_nhwc_to_nchw_f32(const void* x, int ldx, int x_dtype, float* y, int N, i
 /* y[M][ldy] (bf16) = beta*y + x[M][ldx] (bf16) */
 int seg_axpby_bf16(const void* x, int ldx, void* y, int ldy, int64_t M, int C, float beta, void* stream);
 /* multi-tensor SGD step (torch.optim.SGD semantics: wd, momentum, dampening 0, no nesterov;
- * base/base_trainer.py:57): n tensors described by device arrays of pointers/sizes */
+ * base/base_trainer.py:57): n tensors described by device arrays of pointers/sizes; one block row per tensor, so
+ * n <= 65535 (a larger n is refused before any launch) */
 int seg_sgd_step(float* const* params, float* const* grads, float* const* momentum_bufs, const int64_t* sizes,
                  const float* lrs, int n, float momentum, float weight_decay, int first_step, float grad_scale,
                  void* stream);

@@ -1680,6 +1680,7 @@ int seg_counter_add(uint64_t* ctr, uint64_t inc, void* stream) {
 int seg_sgd_step(float* const* params, float* const* grads, float* const* bufs, const int64_t* sizes, const float* lrs,
                  int n, float momentum, float weight_decay, int first_step, float grad_scale, void* stream) {
   if (n <= 0) return 0;
+  SEG_REQUIRE(n <= 65535, "sgd_step: at most 65535 tensors per launch (one block row per tensor)");
   SgdChunkArgs a{params, grads, bufs, sizes, lrs};
   dim3 grid(64, (unsigned)n, 1);
   sgd_kernel<<<grid, 256, 0, ST(stream)>>>(a, momentum, weight_decay, first_step, grad_scale, nullptr);
@@ -1689,6 +1690,7 @@ int seg_sgd_step_dev(float* const* params, float* const* grads, float* const* bu
                      int n, const float* hyper, int first_step, float grad_scale, void* stream) {
   if (n <= 0) return 0;
   SEG_REQUIRE(hyper != nullptr, "sgd_step_dev: hyper (device [momentum, weight_decay]) is required");
+  SEG_REQUIRE(n <= 65535, "sgd_step_dev: at most 65535 tensors per launch (one block row per tensor)");
   SgdChunkArgs a{params, grads, bufs, sizes, lrs};
   dim3 grid(64, (unsigned)n, 1);
   sgd_kernel<<<grid, 256, 0, ST(stream)>>>(a, 0.f, 0.f, first_step, grad_scale, hyper);
