@@ -206,6 +206,18 @@ int seg_maxpool3x3s2_fwd(const void* x, void* y, uint8_t* idx, int N, int H, int
                          void* stream);
 int seg_maxpool3x3s2_bwd(const void* dy, const uint8_t* idx, void* dx, int N, int H, int W, int C, int P, int Q,
                          void* stream);
+/* nn.MaxPool2d(2, 2, return_indices=True) (segnet.py:30, called at segnet.py:87-103) and nn.MaxUnpool2d(2, 2) with
+ * output_size = the pre-pool size (segnet.py:62, called at segnet.py:106-118).  H, W: the PRE-pool size (H, W >= 2);
+ * P = H/2, Q = W/2 (floor: an odd last row / column is never read).  code[N,P,Q,C] (uint8) = 2r + s of the window
+ * element chosen by ATen's rule (row-major scan, v > best || isnan(v): first maximum on ties, last NaN wins).  C % 8 == 0.
+ * Selections of raw bf16 bits; every output element is written exactly once (no memset, no beta). */
+int seg_maxpool2x2_fwd(const void* x, void* y, uint8_t* code, int N, int H, int W, int C, void* stream);
+/* dx[N,H,W,C] = dy at the coded position of each window, 0 elsewhere and on a dropped odd row / column */
+int seg_maxpool2x2_bwd(const void* dy, const uint8_t* code, void* dx, int N, int H, int W, int C, void* stream);
+/* y[N,H,W,C] from x[N,P,Q,C]: x at the coded position, zeros in the other three and past rows 2P / columns 2Q */
+int seg_maxunpool2x2_fwd(const void* x, const uint8_t* code, void* y, int N, int H, int W, int C, void* stream);
+/* dx[N,P,Q,C] = dy[N,H,W,C] gathered at the coded positions */
+int seg_maxunpool2x2_bwd(const void* dy, const uint8_t* code, void* dx, int N, int H, int W, int C, void* stream);
 /* nn.AdaptiveAvgPool2d(bins) (deeplabv3_plus.py:274 bins=1; pspnet.py:26 bins 1,2,3,6): y[N,b,b,C] bf16 */
 int seg_adaptive_avgpool_fwd(const void* x, int ldx, void* y, int N, int H, int W, int C, int bins, void* stream);
 /* dx = beta*dx + scatter(dy) */

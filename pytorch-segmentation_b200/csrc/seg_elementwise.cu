@@ -847,6 +847,123 @@ __global__ void __launch_bounds__(256) maxpool_bwd_kernel(const __nv_bfloat16* _
   }
 }
 
+// ---- 2x2 / stride-2 max pool with indices and max unpool (SegNet).  Floor mode, no padding: the windows never overlap,
+// so all four ops are selections and move raw bf16 bits.  One uint8 code per pooled element, code = 2r + s.  Pointers
+// are in 16-byte vectors (8 channels); G = C / 8.
+union Raw8 {
+  uint4 u;
+  unsigned short h[8];
+};
+
+__device__ __forceinline__ float bf16_bits_to_float(unsigned short b) { return __uint_as_float((uint32_t)b << 16); }
+
+// ATen's rule (max_pool2d_with_indices): scan the window in row-major order from -inf, take v > best || isnan(v); the
+// index starts at the window's first element.  Starting from that element instead gives the same value and index.
+__global__ void __launch_bounds__(256) maxpool2x2_fwd_kernel(const uint4* __restrict__ x, uint4* __restrict__ y,
+                                                             uint2* __restrict__ code, int N, int H, int W, int G, int P, int Q) {
+  const int64_t total = (int64_t)N * P * Q * G;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int g = (int)(i % G);
+    int64_t t = i / G;
+    const int q = (int)(t % Q);
+    t /= Q;
+    const int p = (int)(t % P);
+    const int n = (int)(t / P);
+    const int64_t b = (((int64_t)n * H + 2 * p) * W + 2 * q) * G + g;
+    Raw8 v[4], o;
+    v[0].u = x[b];
+    v[1].u = x[b + G];
+    v[2].u = x[b + (int64_t)W * G];
+    v[3].u = x[b + (int64_t)W * G + G];
+    uint32_t lo = 0, hi = 0;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      unsigned short bits = v[0].h[j];
+      float best = bf16_bits_to_float(bits);
+      uint32_t c = 0;
+#pragma unroll
+      for (int k = 1; k < 4; ++k) {
+        const float f = bf16_bits_to_float(v[k].h[j]);
+        if (f > best || isnan(f)) {
+          best = f;
+          bits = v[k].h[j];
+          c = k;
+        }
+      }
+      o.h[j] = bits;
+      if (j < 4) lo |= c << (8 * j);
+      else hi |= c << (8 * (j - 4));
+    }
+    y[i] = o.u;
+    code[i] = make_uint2(lo, hi);
+  }
+}
+
+// pooled [N,P,Q] -> full [N,H,W]: the value at its coded position of each window, zeros in the other three and on the row /
+// column that floor mode dropped (H or W odd).  Writes every output element once.  The max-pool backward (dy -> dx) and
+// the max-unpool forward (x -> y) are both this scatter.
+__global__ void __launch_bounds__(256) unpool2x2_scatter_kernel(const uint4* __restrict__ src, const uint2* __restrict__ code,
+                                                                uint4* __restrict__ dst, int N, int H, int W, int G, int P, int Q) {
+  const int P2 = (H + 1) >> 1, Q2 = (W + 1) >> 1;
+  const int64_t total = (int64_t)N * P2 * Q2 * G;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int g = (int)(i % G);
+    int64_t t = i / G;
+    const int q = (int)(t % Q2);
+    t /= Q2;
+    const int p = (int)(t % P2);
+    const int n = (int)(t / P2);
+    Raw8 o[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) o[k].u = make_uint4(0u, 0u, 0u, 0u);
+    if (p < P && q < Q) {
+      const int64_t pi = (((int64_t)n * P + p) * Q + q) * G + g;
+      Raw8 v;
+      v.u = src[pi];
+      const uint2 c = code[pi];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const uint32_t cj = ((j < 4 ? c.x : c.y) >> (8 * (j & 3))) & 0xffu;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) o[k].h[j] = (cj == (uint32_t)k) ? v.h[j] : (unsigned short)0;
+      }
+    }
+    const int64_t b = (((int64_t)n * H + 2 * p) * W + 2 * q) * G + g;
+    const bool r1 = 2 * p + 1 < H, s1 = 2 * q + 1 < W;
+    dst[b] = o[0].u;
+    if (s1) dst[b + G] = o[1].u;
+    if (r1) dst[b + (int64_t)W * G] = o[2].u;
+    if (r1 && s1) dst[b + (int64_t)W * G + G] = o[3].u;
+  }
+}
+
+// full [N,H,W] -> pooled [N,P,Q]: each pooled element takes the value at its coded position (the max-unpool backward).
+__global__ void __launch_bounds__(256) unpool2x2_gather_kernel(const uint4* __restrict__ src, const uint2* __restrict__ code,
+                                                               uint4* __restrict__ dst, int N, int H, int W, int G, int P, int Q) {
+  const int64_t total = (int64_t)N * P * Q * G;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int g = (int)(i % G);
+    int64_t t = i / G;
+    const int q = (int)(t % Q);
+    t /= Q;
+    const int p = (int)(t % P);
+    const int n = (int)(t / P);
+    const int64_t b = (((int64_t)n * H + 2 * p) * W + 2 * q) * G + g;
+    Raw8 v[4], o;
+    v[0].u = src[b];
+    v[1].u = src[b + G];
+    v[2].u = src[b + (int64_t)W * G];
+    v[3].u = src[b + (int64_t)W * G + G];
+    const uint2 c = code[i];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const uint32_t cj = ((j < 4 ? c.x : c.y) >> (8 * (j & 3))) & 0xffu;
+      o.h[j] = cj == 0 ? v[0].h[j] : cj == 1 ? v[1].h[j] : cj == 2 ? v[2].h[j] : v[3].h[j];
+    }
+    dst[i] = o.u;
+  }
+}
+
 __device__ __forceinline__ int bin_lo(int i, int L, int b) { return (i * L) / b; }
 __device__ __forceinline__ int bin_hi(int i, int L, int b) { return ((i + 1) * L + b - 1) / b; }
 
@@ -1577,6 +1694,43 @@ int seg_maxpool3x3s2_bwd(const void* dy, const uint8_t* idx, void* dx, int N, in
   SEG_REQUIRE(C % 8 == 0, "maxpool: C %% 8");
   maxpool_bwd_kernel<<<grid_for((int64_t)N * H * W * (C / 8), 256), 256, 0, ST(stream)>>>(CBF(dy), idx, BF(dx), N, H, W, C, P, Q);
   return check_launch("maxpool_bwd");
+}
+
+static int check_pool2x2(const char* what, const void* a, const void* b, const void* code, int N, int H, int W, int C) {
+  SEG_REQUIRE(N > 0 && H >= 2 && W >= 2, "%s: needs N >= 1 and H, W >= 2 (got %d x %d x %d)", what, N, H, W);
+  SEG_REQUIRE(C > 0 && C % 8 == 0, "%s: C = %d is not a positive multiple of 8", what, C);
+  SEG_REQUIRE(((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b)) & 15) == 0 &&
+                  (reinterpret_cast<uintptr_t>(code) & 7) == 0,
+              "%s: activations must be 16-byte and codes 8-byte aligned", what);
+  return 0;
+}
+int seg_maxpool2x2_fwd(const void* x, void* y, uint8_t* code, int N, int H, int W, int C, void* stream) {
+  if (check_pool2x2("maxpool2x2_fwd", x, y, code, N, H, W, C)) return 1;
+  const int P = H / 2, Q = W / 2;
+  maxpool2x2_fwd_kernel<<<grid_for((int64_t)N * P * Q * (C / 8), 256), 256, 0, ST(stream)>>>(
+      reinterpret_cast<const uint4*>(x), reinterpret_cast<uint4*>(y), reinterpret_cast<uint2*>(code), N, H, W, C / 8, P, Q);
+  return check_launch("maxpool2x2_fwd");
+}
+static int launch_unpool2x2_scatter(const char* what, const void* src, const uint8_t* code, void* dst, int N, int H, int W,
+                                    int C, void* stream) {
+  if (check_pool2x2(what, src, dst, code, N, H, W, C)) return 1;
+  unpool2x2_scatter_kernel<<<grid_for((int64_t)N * ((H + 1) / 2) * ((W + 1) / 2) * (C / 8), 256), 256, 0, ST(stream)>>>(
+      reinterpret_cast<const uint4*>(src), reinterpret_cast<const uint2*>(code), reinterpret_cast<uint4*>(dst), N, H, W, C / 8,
+      H / 2, W / 2);
+  return check_launch(what);
+}
+int seg_maxpool2x2_bwd(const void* dy, const uint8_t* code, void* dx, int N, int H, int W, int C, void* stream) {
+  return launch_unpool2x2_scatter("maxpool2x2_bwd", dy, code, dx, N, H, W, C, stream);
+}
+int seg_maxunpool2x2_fwd(const void* x, const uint8_t* code, void* y, int N, int H, int W, int C, void* stream) {
+  return launch_unpool2x2_scatter("maxunpool2x2_fwd", x, code, y, N, H, W, C, stream);
+}
+int seg_maxunpool2x2_bwd(const void* dy, const uint8_t* code, void* dx, int N, int H, int W, int C, void* stream) {
+  if (check_pool2x2("maxunpool2x2_bwd", dy, dx, code, N, H, W, C)) return 1;
+  const int P = H / 2, Q = W / 2;
+  unpool2x2_gather_kernel<<<grid_for((int64_t)N * P * Q * (C / 8), 256), 256, 0, ST(stream)>>>(
+      reinterpret_cast<const uint4*>(dy), reinterpret_cast<const uint2*>(code), reinterpret_cast<uint4*>(dx), N, H, W, C / 8, P, Q);
+  return check_launch("maxunpool2x2_bwd");
 }
 int seg_adaptive_avgpool_fwd(const void* x, int ldx, void* y, int N, int H, int W, int C, int bins, void* stream) {
   SEG_REQUIRE(C % 8 == 0 && ldx % 8 == 0, "avgpool: alignment");

@@ -12,6 +12,7 @@ _LAZY = {
     "UperNet": ("nets", "UperNet"),
     "DeepLab_DUC_HDC": ("nets", "DeepLab_DUC_HDC"),
     "UNetResnet": ("nets", "UNetResnet"),
+    "SegNet": ("nets", "SegNet"),
     "CrossEntropyLoss2d": ("losses", "CrossEntropyLoss2d"),
     "DiceLoss": ("losses", "DiceLoss"),
     "FocalLoss": ("losses", "FocalLoss"),

@@ -466,6 +466,39 @@ class Tape:
             self.back.append(bwd)
         return ya
 
+    def maxpool2x2(self, x):
+        """nn.MaxPool2d(2, 2, return_indices=True) (segnet.py:30).  Returns (pooled Act, record): the record holds the
+        codes and the pre-pool shape, for `maxunpool2x2`.  x must be the pool's only consumer (as in SegNet)."""
+        y, code = ops.maxpool2x2_fwd(x.t)
+        ya = Act(y)
+        if self.record:
+            def bwd():
+                if ya.grad is None or not x.needs_grad:
+                    return
+                assert x.grad is None, "maxpool2x2 input must have a single consumer"
+                x.grad = ops.maxpool2x2_bwd(ya.grad, code, tuple(x.t.shape))
+                x._written = True
+                ya.grad = None
+            self.back.append(bwd)
+        return ya, (code, tuple(x.t.shape))
+
+    def maxunpool2x2(self, x, record):
+        """nn.MaxUnpool2d(2, 2) of x to the pre-pool size of the max-pool that wrote `record` (segnet.py:106-118).  x must
+        be the unpool's only consumer (as in SegNet)."""
+        code, shape = record
+        y = ops.maxunpool2x2_fwd(x.t, code, shape[1:3])
+        ya = Act(y)
+        if self.record:
+            def bwd():
+                if ya.grad is None or not x.needs_grad:
+                    return
+                assert x.grad is None, "maxunpool2x2 input must have a single consumer"
+                x.grad = ops.maxunpool2x2_bwd(ya.grad, code)
+                x._written = True
+                ya.grad = None
+            self.back.append(bwd)
+        return ya
+
     def avgpool(self, x, bins):
         y = ops.adaptive_avgpool_fwd(x.t, bins)
         ya = Act(y)

@@ -5,6 +5,7 @@
     UperNet(num_classes, in_channels=3, backbone='resnet101', pretrained=None, use_aux=True, fpn_out=256, freeze_bn=False, **_)
     DeepLab_DUC_HDC(num_classes, in_channels=3, pretrained=None, output_stride=8, freeze_bn=False, **_)
     UNetResnet(num_classes, in_channels=3, backbone='resnet50', pretrained=None, freeze_bn=False, **_)
+    SegNet(num_classes, in_channels=3, pretrained=None, freeze_bn=False, freeze_backbone=False, **_)
 
 (default backbones are the reference's; `pretrained`: the reference defaults to True and downloads ImageNet weights — there is
 no network here, so an explicit True raises and the default (None) initialises randomly with a logged warning)
@@ -1168,3 +1169,108 @@ class UNetResnet(_EngineModel):
 
     def get_decoder_params(self):
         return chain(*(getattr(self, n).parameters() for n, _, _ in self.DECODER), self.conv7.parameters())
+
+
+# ----------------------------------------------------------------------------------------------- SegNet
+def _vgg_stage(cin, widths):
+    """(Conv2d 3x3 p1 with bias, BatchNorm2d, ReLU) per width: the nn.Sequential index layout of torchvision's vgg16_bn
+    features, so that `stageN_encoder.3.weight` etc. line up with the reference."""
+    mods = []
+    for w in widths:
+        mods += [nn.Conv2d(cin, w, kernel_size=3, stride=1, padding=1), nn.BatchNorm2d(w), nn.ReLU(inplace=True)]
+        cin = w
+    return nn.Sequential(*mods)
+
+
+class SegNet(_EngineModel):
+    """VGG16-BN encoder-decoder with max-pool indices — replaces models/segnet.py:13-132.  Encoder stages 64², 128², 256³,
+    512³, 512³ (vgg16_bn's features without the pools); decoder stages 1-5 are the reversed encoder convs (9, 9, 9, 6 and 6
+    modules) with the channel-changing ones rebuilt as 512->256, 256->128 and 128->64 plus a new BatchNorm, then
+    `stage5_decoder.6` = Conv2d(64, num_classes, 3, p1).  Every conv has a bias.  Each encoder stage ends in
+    MaxPool2d(2, 2, return_indices=True); each decoder stage starts with MaxUnpool2d(2, 2) to the size of the matching
+    encoder map, so the logits are at input resolution for any input of at least 32 x 32 (smaller ones leave the fifth pool
+    empty and raise ValueError).
+    Init as the reference: the encoder keeps torchvision's VGG init (kaiming-normal fan_out convs, bias 0, BN 1 / 0; with
+    in_channels != 3 `stage1_encoder.0` is a default-initialised Conv2d), the decoder gets kaiming-normal (fan_in) convs,
+    bias 0, BN 1 / 0.  Parameter groups as the reference's: no backbone group, every parameter in the decoder group."""
+
+    ENCODER = ((64, 64), (128, 128), (256, 256, 256), (512, 512, 512), (512, 512, 512))
+    DECODER = ((512, (512, 512, 512)), (512, (512, 512, 256)), (256, (256, 256, 128)), (128, (128, 64)), (64, (64, 64)))
+    MIN_SIZE = 32
+
+    def __init__(self, num_classes, in_channels=3, pretrained=None, freeze_bn=False, freeze_backbone=False, **_):
+        super().__init__()
+        _check_pretrained(self, pretrained)
+        self.num_classes = num_classes
+        cin = 3
+        for i, widths in enumerate(self.ENCODER):
+            setattr(self, f"stage{i + 1}_encoder", _vgg_stage(cin, widths))
+            cin = widths[-1]
+        for m in self.modules():  # torchvision VGG._initialize_weights (no weights: the reference's shimmed vgg16_bn)
+            if isinstance(m, nn.Conv2d):
+                nn.init.kaiming_normal_(m.weight, mode="fan_out", nonlinearity="relu")
+                nn.init.constant_(m.bias, 0)
+            elif isinstance(m, nn.BatchNorm2d):
+                nn.init.constant_(m.weight, 1)
+                nn.init.constant_(m.bias, 0)
+        if in_channels != 3:
+            self.stage1_encoder[0] = nn.Conv2d(in_channels, 64, kernel_size=3, stride=1, padding=1)
+        self.pool = nn.MaxPool2d(kernel_size=2, stride=2, return_indices=True)  # holder: the engine runs Tape.maxpool2x2
+        for i, (cin, widths) in enumerate(self.DECODER):
+            setattr(self, f"stage{i + 1}_decoder", _vgg_stage(cin, widths))
+        self.stage5_decoder.append(nn.Conv2d(64, num_classes, kernel_size=3, stride=1, padding=1))
+        self.unpool = nn.MaxUnpool2d(kernel_size=2, stride=2)
+        for i in range(1, 6):  # segnet.py:69-78
+            for m in getattr(self, f"stage{i}_decoder").modules():
+                if isinstance(m, nn.Conv2d):
+                    nn.init.kaiming_normal_(m.weight)
+                    m.bias.data.zero_()
+                elif isinstance(m, nn.BatchNorm2d):
+                    m.weight.data.fill_(1)
+                    m.bias.data.zero_()
+        if freeze_bn:
+            self.freeze_bn()
+        if freeze_backbone:
+            for i in range(1, 6):
+                for p in getattr(self, f"stage{i}_encoder").parameters():
+                    p.requires_grad = False
+
+    def _spec(self, name, module):
+        # the network input (NCHW fp32, any channel count) always goes through the explicit im2col conv
+        s = self._specs.get(name)
+        if s is None or s.m is not module:
+            s = ConvSpec(name, module, explicit_im2col=(name == "stage1_encoder.0"))
+            self._specs[name] = s
+        return s
+
+    def _check_size(self, x):
+        H, W = x.shape[-2], x.shape[-1]
+        if H < self.MIN_SIZE or W < self.MIN_SIZE:
+            raise ValueError(f"SegNet needs an input of at least {self.MIN_SIZE}x{self.MIN_SIZE} (five 2x2 max-pools); got {H}x{W}")
+
+    def forward(self, x):
+        self._check_size(x)
+        return super().forward(x)
+
+    def _stage(self, tape, a, name):
+        seq = getattr(self, name)
+        for j in range(0, len(seq) - len(seq) % 3, 3):  # (conv, BN, ReLU) triples; stage5_decoder.6 is the classifier
+            a = self._cbr(tape, a, f"{name}.{j}", seq[j], seq[j + 1])
+        return a
+
+    def _forward_heads(self, tape, x):
+        self._check_size(x)
+        a, records = x, []
+        for i in range(1, 6):
+            a, rec = tape.maxpool2x2(self._stage(tape, a, f"stage{i}_encoder"))
+            records.append(rec)
+        for i in range(1, 6):
+            a = self._stage(tape, tape.maxunpool2x2(a, records[5 - i]), f"stage{i}_decoder")
+        lo, _ = tape.conv(a, self._spec("stage5_decoder.6", self.stage5_decoder[6]), out_dtype=torch.float32)
+        return [FullResHead(lo)]
+
+    def get_backbone_params(self):
+        return []
+
+    def get_decoder_params(self):
+        return self.parameters()

@@ -382,6 +382,42 @@ def maxpool3x3s2_bwd(dy, idx, x_shape):
     return dx
 
 
+def maxpool2x2_fwd(x):
+    """nn.MaxPool2d(2, 2, return_indices=True), floor mode: (y [N,H//2,W//2,C] bf16, codes uint8 of y's shape, 2r + s)."""
+    N, H, W, C = x.shape
+    assert x.is_contiguous()
+    y = torch.empty((N, H // 2, W // 2, C), dtype=torch.bfloat16, device=x.device)
+    code = torch.empty(y.shape, dtype=torch.uint8, device=x.device)
+    call("seg_maxpool2x2_fwd", ptr(x), ptr(y), ptr(code), N, H, W, C)
+    return y, code
+
+
+def maxpool2x2_bwd(dy, code, x_shape):
+    N, H, W, C = x_shape
+    assert dy.is_contiguous() and tuple(dy.shape) == (N, H // 2, W // 2, C) and code.shape == dy.shape
+    dx = torch.empty(x_shape, dtype=torch.bfloat16, device=dy.device)
+    call("seg_maxpool2x2_bwd", ptr(dy), ptr(code), ptr(dx), N, H, W, C)
+    return dx
+
+
+def maxunpool2x2_fwd(x, code, out_hw):
+    """nn.MaxUnpool2d(2, 2) with output_size = out_hw, the pre-pool size whose max-pool wrote `code`."""
+    N, P, Q, C = x.shape
+    H, W = out_hw
+    assert x.is_contiguous() and (P, Q) == (H // 2, W // 2) and code.shape == x.shape
+    y = torch.empty((N, H, W, C), dtype=torch.bfloat16, device=x.device)
+    call("seg_maxunpool2x2_fwd", ptr(x), ptr(code), ptr(y), N, H, W, C)
+    return y
+
+
+def maxunpool2x2_bwd(dy, code):
+    N, H, W, C = dy.shape
+    assert dy.is_contiguous() and tuple(code.shape) == (N, H // 2, W // 2, C)
+    dx = torch.empty(code.shape, dtype=torch.bfloat16, device=dy.device)
+    call("seg_maxunpool2x2_bwd", ptr(dy), ptr(code), ptr(dx), N, H, W, C)
+    return dx
+
+
 def adaptive_avgpool_fwd(x, bins):
     N, H, W, C = x.shape
     y = torch.empty((N, bins, bins, C), dtype=torch.bfloat16, device=x.device)
