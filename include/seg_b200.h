@@ -433,7 +433,9 @@ int seg_window_add_nchw_f32(const float* src, int64_t planes, int Hs, int Ws, fl
                             int w, int flip_x, float alpha, void* stream);
 /* x[p] /= count  (count fp32 [H,W]; inference.py:55) */
 int seg_div_by_count_nchw_f32(float* x, int64_t planes, int H, int W, const float* count_hw, void* stream);
-/* labels int64 [N,H,W] = argmax over the C planes, first maximum wins (inference.py:156 without the softmax pass) */
+/* labels int64 [N,H,W] = softmax(dim=C).argmax of inference.py:156 without the softmax pass: 0 where a pixel's scores hold
+ * a NaN or +inf (the reference's softmax column is all NaN), else the first maximum.  Two finite top scores closer than a
+ * float64 softmax resolves (both under ~2e-9) may tie in the reference, which keeps the first; here the larger wins. */
 int seg_argmax_nchw_f32(const float* scores, int N, int C, int H, int W, int64_t* labels, void* stream);
 /* ---- SyncBN one-shot exchange over NVLink peer memory (replaces ReduceAddCoalesced + Broadcast,
  *      sync_batchnorm/batchnorm.py:117,120 and the thread pipes of sync_batchnorm/comm.py) ----

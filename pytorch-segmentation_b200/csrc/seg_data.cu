@@ -171,7 +171,7 @@ __global__ void __launch_bounds__(256) augment_scale_u8_kernel(const uint8_t* __
   }
 }
 
-// ------------------------------------------------------------------ scale + ROTATE + tail (experimental: never run on a GPU)
+// ------------------------------------------------------------------ scale + ROTATE + tail
 // base_dataset.py:77-83 rotates the resized float image (cv2.warpAffine INTER_LINEAR) and label (INTER_NEAREST) about the
 // centre by a drawn angle, constant-0 border.  OpenCV's walk, restated bit-exactly in oracle/data.py::cv_warp_affine: the
 // inverse matrix (float64, from the host) gives fixed-point source coordinates with 10 fractional bits,
@@ -179,8 +179,7 @@ __global__ void __launch_bounds__(256) augment_scale_u8_kernel(const uint8_t* __
 // INTER_LINEAR keeps 5 fractional bits (a 1/32-pixel grid) and blends the four taps with float32 weight products; taps
 // outside the resized image are 0.  Each tap of the RESIZED image is itself the cv2.resize interpolation of the raw image
 // (augment_scale_u8_kernel's arithmetic, NOT truncated: the rotation consumes the float image), so an output pixel costs up
-// to 16 raw taps and no intermediate image exists.  Written after the round's GPU budget was spent: compiled, exported,
-// reachable only through DeviceBatcher.stage_full / tests gated by SEG_EXPERIMENTAL=1.
+// to 16 raw taps and no intermediate image exists.  Reached through DeviceBatcher.stage_full.
 __device__ __forceinline__ void resized_pixel_f32(const uint8_t* __restrict__ img, const seg_aug_full_entry& e, int ry, int rx, float* out3) {
   if (ry < 0 || ry >= e.h || rx < 0 || rx >= e.w) {
     out3[0] = out3[1] = out3[2] = 0.f;
@@ -371,8 +370,13 @@ __global__ void __launch_bounds__(256) div_by_count_kernel(float* __restrict__ x
     x[i] = __fdiv_rn(x[i], count[i % hw]);
 }
 
-// labels[n][y][x] = first index of the maximum over the C planes (torch.argmax's tie rule); softmax is monotone, so this
-// is `F.softmax(prediction, dim=0).argmax(0)` of inference.py:156 without the softmax pass
+// labels[n][y][x] = `F.softmax(prediction, dim=0).argmax(0)` of inference.py:156 without the softmax pass:
+//   * a pixel whose scores hold a NaN or a +inf has label 0 (its float64 softmax column is all NaN, and argmax returns the
+//     first NaN);
+//   * otherwise the first index of the maximum score (the softmax is monotone on finite and -inf scores, and argmax keeps
+//     the first of equal values).
+// One class of finite inputs differs: two top scores that differ by less than a float64 softmax resolves (both under about
+// 2e-9 in magnitude) can round to equal probabilities, where the reference keeps the first; here the larger score wins.
 __global__ void __launch_bounds__(256) argmax_nchw_kernel(const float* __restrict__ s, int N, int C, int64_t hw,
                                                           int64_t* __restrict__ labels) {
   const int64_t total = (int64_t)N * hw;
@@ -381,14 +385,16 @@ __global__ void __launch_bounds__(256) argmax_nchw_kernel(const float* __restric
     const float* p = s + n * C * hw + q;
     float best = p[0];
     int arg = 0;
+    bool nonfinite = !(best < INFINITY);  // NaN or +inf
     for (int c = 1; c < C; ++c) {
       const float v = p[(int64_t)c * hw];
+      nonfinite |= !(v < INFINITY);
       if (v > best) {
         best = v;
         arg = c;
       }
     }
-    labels[i] = arg;
+    labels[i] = nonfinite ? 0 : arg;
   }
 }
 

@@ -71,6 +71,16 @@ def draw_crop_flip(h, w, crop_size, flip=True, rng=random):
     return y0, x0, f
 
 
+def check_crop_origins(crop, dims):
+    """dims: (h, w, y0, x0) per sample, h x w the image the crop is taken from.  The kernels trust the table, and a negative
+    origin would read before the image, so an origin outside [0, max(h, crop) - crop] is refused before anything is staged."""
+    for b, (h, w, y0, x0) in enumerate(dims):
+        ym, xm = max(int(h), crop) - crop, max(int(w), crop) - crop
+        if not (0 <= int(y0) <= ym and 0 <= int(x0) <= xm):
+            raise ValueError(f"DeviceBatcher: sample {b}: crop origin (y0={y0}, x0={x0}) outside [0, {ym}] x [0, {xm}] "
+                             f"for a {h} x {w} image and crop {crop}")
+
+
 class DeviceBatcher:
     def __init__(self, mean, std, crop_size, device, max_bytes=64 << 20):
         assert _ENTRY.itemsize == lib.load().seg_aug_entry_bytes()
@@ -86,6 +96,7 @@ class DeviceBatcher:
         """samples: sequence of (image uint8 [h,w,3], label uint8|int32 [h,w] or None, y0, x0, flip).  Packs them into
         pinned memory, copies once, launches the kernel on the current stream.  Returns (images, labels)."""
         B = len(samples)
+        check_crop_origins(self.crop, [(np.shape(s[0])[0], np.shape(s[0])[1], s[2], s[3]) for s in samples])
         slot = self._slot
         self._slot ^= 1
         if self._events[slot] is not None:
@@ -131,6 +142,7 @@ class DeviceBatcher:
         — in one kernel, without a resized intermediate (`seg_augment_scale_batch_u8`)."""
         assert _SCALE_ENTRY.itemsize == lib.load().seg_aug_scale_entry_bytes()
         B = len(samples)
+        check_crop_origins(self.crop, [(s[2], s[3], s[4], s[5]) for s in samples])
         slot = self._slot
         self._slot ^= 1
         if self._events[slot] is not None:
@@ -176,6 +188,7 @@ class DeviceBatcher:
         centre (base_dataset.py:77-83), pad / crop / flip / normalise — one kernel (`seg_augment_full_batch_u8`)."""
         assert _FULL_ENTRY.itemsize == lib.load().seg_aug_full_entry_bytes()
         B = len(samples)
+        check_crop_origins(self.crop, [(s[2], s[3], s[5], s[6]) for s in samples])
         slot = self._slot
         self._slot ^= 1
         if self._events[slot] is not None:

@@ -84,6 +84,10 @@ def sliding_predict(model, image, num_classes, flip=True):
     count = np.zeros((H, W), dtype=np.float32)
     with torch.no_grad():
         for (y0, y1, x0, x1) in wins:
+            if y1 <= y0 or x1 <= x0:
+                # an empty window (portrait images: the one stride, from the tile height, can start a column at or past
+                # the right edge); the reference predicts on a padded empty tile and adds nothing from it
+                continue
             padded = pad_image(image[:, :, y0:y1, x0:x1], tile)
             pred = model(padded).contiguous().float()
             h, w = y1 - y0, x1 - x0
@@ -100,7 +104,9 @@ def sliding_predict(model, image, num_classes, flip=True):
 
 
 def predict_labels(scores):
-    """Label map of inference.py:156 (`softmax(dim=0).argmax(0)`; the softmax is monotone) as an int64 device tensor."""
+    """Label map of inference.py:156 (`softmax(dim=0).argmax(0)`) as an int64 device tensor: 0 where a pixel's scores hold
+    a NaN or +inf (the reference's softmax column is then all NaN), elsewhere the first maximum score.  Pixels that no
+    sliding window covers hold NaN scores (0 / 0, as in the reference) and get label 0."""
     s = scores if scores.dim() == 4 else scores.unsqueeze(0)
     _require_cuda(s)
     lab = ops.argmax_nchw(s.contiguous().float())

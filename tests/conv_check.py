@@ -230,8 +230,9 @@ def check_stats(case, stats, stored, chain, show=8):
 
 
 # ------------------------------------------------------------------------------------------------ guarded buffers
-SENTINEL_BITS = {torch.bfloat16: 0x7FA5, torch.float32: 0x7FA5A5A5}  # NaN bit patterns (quiet bit clear: no kernel makes them)
-_INT = {torch.bfloat16: torch.int16, torch.float32: torch.int32}
+SENTINEL_BITS = {torch.bfloat16: 0x7FA5, torch.float32: 0x7FA5A5A5,  # NaN bit patterns (quiet bit clear: no kernel makes them)
+                 torch.int64: 0x5A5A5A5A5A5A5A5A}  # int64 label maps: outside the int32 range every label comes from
+_INT = {torch.bfloat16: torch.int16, torch.float32: torch.int32, torch.int64: torch.int64}
 
 
 def sentinel_fill(t):

@@ -7,6 +7,7 @@ import numpy as np
 import torch
 
 from oracle import data as od
+from data_check import fused_emulation
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "data_tail.npz")
 
@@ -62,6 +63,14 @@ def test_oracle_resize_is_opencvs_own_arithmetic():
             lbl = rs.randint(0, 21, (sh, sw)).astype(np.int32)
             assert np.array_equal(cv2.resize(img.astype(np.float32), (dw, dh), interpolation=cv2.INTER_LINEAR), od.cv_resize_linear_f32(img, dw, dh))
             assert np.array_equal(cv2.resize(lbl, (dw, dh), interpolation=cv2.INTER_NEAREST), od.cv_resize_nearest(lbl, dw, dh))
+        # the geometry of the GPU sweep: 1-pixel sources, x300 up-scales, 2000 -> 30 down-scales
+        for (sh, sw, dh, dw) in ((1, 1, 7, 5), (1, 50, 13, 3), (50, 1, 2, 40), (1, 1, 300, 300), (2, 3, 600, 900),
+                                 (2000, 2000, 30, 30), (2000, 37, 30, 300), (9, 2000, 1, 30)):
+            img = rs.randint(0, 256, (sh, sw, 3)).astype(np.uint8)
+            lbl = rs.randint(0, 21, (sh, sw)).astype(np.int32)
+            assert np.array_equal(cv2.resize(img.astype(np.float32), (dw, dh), interpolation=cv2.INTER_LINEAR),
+                                  od.cv_resize_linear_f32(img, dw, dh)), (sh, sw, dh, dw)
+            assert np.array_equal(cv2.resize(lbl, (dw, dh), interpolation=cv2.INTER_NEAREST), od.cv_resize_nearest(lbl, dw, dh))
     finally:
         cv2.ipp.setUseIPP(had)
 
@@ -83,11 +92,14 @@ def test_oracle_rotation_is_opencvs_arithmetic():
     IPP on or off (warpAffine's fixed-point coordinate walk is OpenCV's own code either way)."""
     cv2 = __import__("pytest").importorskip("cv2")
     rs = np.random.RandomState(8)
-    for _ in range(40):
+    extra = (45, -45, 90, -90, 180, -170)   # the GPU sweep's angles beyond the reference's draw of [-10, 10]
+    for k in range(40 + 2 * len(extra)):
         h, w = int(rs.randint(20, 140)), int(rs.randint(20, 140))
+        if k >= 40 and k % 2:
+            h, w = (1, 1) if k % 4 == 1 else (1, 50)
         img = (rs.rand(h, w, 3) * 255).astype(np.float32)
         lbl = rs.randint(0, 21, (h, w)).astype(np.int32)
-        angle = int(rs.randint(-10, 11))
+        angle = int(rs.randint(-10, 11)) if k < 40 else extra[(k - 40) // 2]
         M = od.cv_rotation_matrix((w / 2, h / 2), angle)
         assert np.array_equal(M, cv2.getRotationMatrix2D((w / 2, h / 2), angle, 1.0))
         assert np.array_equal(cv2.warpAffine(img, M, (w, h), flags=cv2.INTER_LINEAR), od.cv_warp_affine(img, M, w, h, True))
@@ -111,67 +123,6 @@ def test_oracle_scale_rotate_tail_against_reference():
         assert (d > 0).float().mean().item() < 0.01, (i, (d > 0).float().mean().item())
 
 
-def _fused_emulation(image, label, h, w, angle, crop, y0, x0, flip, mean, std):
-    """numpy transcription of augment_full_u8_kernel (seg_data.cu): per OUTPUT pixel, fixed-point rotated coordinates ->
-    four taps of the resized image, each interpolated on the fly from the raw image -> truncate -> normalise.  No resized or
-    rotated intermediate, exactly the kernel's operation order."""
-    from seg_b200.data import inverse_rotation
-    H, W = image.shape[:2]
-    sx_scale, sy_scale = 1.0 / (w / W), 1.0 / (h / H)
-    a11, a12, b1, a21, a22, b2 = inverse_rotation(w, h, angle)
-    raw = image.astype(np.float32)
-    f32 = np.float32
-
-    def coord(d, scale, src, clamp):
-        fv = ((d.astype(np.float64) + 0.5) * scale - 0.5).astype(np.float32)
-        fl = np.floor(fv)
-        s = fl.astype(np.int64)
-        f = (fv - fl).astype(np.float32)
-        if clamp:
-            lo, hi = s < 0, s >= src - 1
-            f = np.where(lo | hi, f32(0), f)
-            s = np.where(lo, 0, np.where(hi, src - 1, s))
-        return s, f
-
-    def resized(ry, rx):  # float value of the resized image at integer (ry, rx); 0 outside
-        ok = (ry >= 0) & (ry < h) & (rx >= 0) & (rx < w)
-        ryc, rxc = np.clip(ry, 0, h - 1), np.clip(rx, 0, w - 1)
-        sx, fx = coord(rxc, sx_scale, W, True)
-        sy, fy = coord(ryc, sy_scale, H, False)
-        sx1 = np.minimum(sx + 1, W - 1)
-        y0c, y1c = np.clip(sy, 0, H - 1), np.clip(sy + 1, 0, H - 1)
-        ax0, ay0 = (f32(1) - fx)[..., None], (f32(1) - fy)[..., None]
-        fx_, fy_ = fx[..., None], fy[..., None]
-        h0 = raw[y0c, sx] * ax0 + raw[y0c, sx1] * fx_
-        h1 = raw[y1c, sx] * ax0 + raw[y1c, sx1] * fx_
-        return np.where(ok[..., None], h0 * ay0 + h1 * fy_, f32(0)).astype(np.float32)
-
-    ys, xs = np.meshgrid(np.arange(crop), np.arange(crop), indexing="ij")
-    xs = crop - 1 - xs if flip else xs
-    dy, dx = ys + y0, xs + x0
-    inside = (dy < h) & (dx < w)
-    rnd = lambda v: np.rint(v).astype(np.int64)  # noqa: E731
-    colX, colY = rnd(a11 * dx.astype(np.float64) * 1024.0), rnd(a21 * dx.astype(np.float64) * 1024.0)
-    rowX, rowY = rnd((a12 * dy.astype(np.float64) + b1) * 1024.0), rnd((a22 * dy.astype(np.float64) + b2) * 1024.0)
-    X, Y = rowX + 16 + colX, rowY + 16 + colY
-    Xf, Yf = X >> 5, Y >> 5
-    xi, yi = Xf >> 5, Yf >> 5
-    fx, fy = (Xf & 31).astype(np.float32) / f32(32), (Yf & 31).astype(np.float32) / f32(32)
-    w00, w01 = ((f32(1) - fy) * (f32(1) - fx))[..., None], ((f32(1) - fy) * fx)[..., None]
-    w10, w11 = (fy * (f32(1) - fx))[..., None], (fy * fx)[..., None]
-    v = resized(yi, xi) * w00 + resized(yi, xi + 1) * w01 + resized(yi + 1, xi) * w10 + resized(yi + 1, xi + 1) * w11
-    u8 = np.where(inside[..., None], np.clip(np.where(v > 0, v, 0).astype(np.int64), 0, 255), 0).astype(np.uint8)
-    Xn, Yn = (rowX + 512 + colX) >> 10, (rowY + 512 + colY) >> 10
-    okl = inside & (Yn >= 0) & (Yn < h) & (Xn >= 0) & (Xn < w)
-    lx = np.minimum(np.floor(np.clip(Xn, 0, w - 1).astype(np.float64) * sx_scale).astype(np.int64), W - 1)
-    ly = np.minimum(np.floor(np.clip(Yn, 0, h - 1).astype(np.float64) * sy_scale).astype(np.int64), H - 1)
-    lab = np.where(okl, np.asarray(label)[ly, lx], 0).astype(np.int64)
-    t = torch.from_numpy(u8).permute(2, 0, 1).contiguous().to(torch.float32).div(255)
-    m = torch.as_tensor(mean, dtype=torch.float32).view(-1, 1, 1)
-    s = torch.as_tensor(std, dtype=torch.float32).view(-1, 1, 1)
-    return t.sub_(m).div_(s), torch.from_numpy(lab)
-
-
 def test_fused_scale_rotate_formulation_equals_staged_oracle():
     """The experimental kernel computes every output pixel from the raw sample in one go (no resized / rotated image).  Its
     numpy transcription must equal the staged oracle (resize, then warpAffine, then the tail) bit for bit — with and without
@@ -182,7 +133,7 @@ def test_fused_scale_rotate_formulation_equals_staged_oracle():
     for i in range(int(g["n"])):
         h, w, angle, y0, x0, flip = (int(v) for v in g[f"r{i}/draw"])
         for ang in (angle, None, -10, 0):
-            x, y = _fused_emulation(g[f"{i}/image"], g[f"{i}/label"], h, w, ang, crop, y0, x0, bool(flip), mean, std)
+            x, y = fused_emulation(g[f"{i}/image"], g[f"{i}/label"], h, w, ang, crop, y0, x0, bool(flip), mean, std)
             rx, ry = od.sample_scale_tail(g[f"{i}/image"], g[f"{i}/label"], h, w, crop, y0, x0, bool(flip), mean, std, angle=ang)
             assert torch.equal(y, ry), (i, ang)
             assert torch.equal(x, rx), (i, ang, (x - rx).abs().max().item())

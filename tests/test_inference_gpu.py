@@ -10,6 +10,7 @@ import torch
 
 pytestmark = pytest.mark.gpu
 
+import data_check as dc
 from oracle import inference as oi
 from oracle import synth, weights
 
@@ -44,61 +45,16 @@ def test_device_tta_matches_reference_golden(tag, gpu_out_dir):
     for k, v in got.items():
         ref = g[f"{tag}/{k}"]
         e = rel(v.cpu().double().numpy(), ref)
-        lab = di.predict_labels(v).cpu().numpy()
-        ref_lab = torch.softmax(torch.from_numpy(ref), dim=0).argmax(0).numpy()  # inference.py:156
-        agree = float((lab == ref_lab).mean())
-        msg = f"[inference {tag}/{k}] scores relerr {e:.2e}  label agreement {agree:.5f}"
+        lab = di.predict_labels(v)
+        # every score is within TOL max|ref| of the reference (asserted below), so a label may differ from the
+        # reference's (inference.py:156) only where the top-two margin is within twice that
+        acc = torch.full(ref.shape, TOL * float(np.abs(ref).max()), dtype=torch.float64)
+        free = dc.check_tta_labels(f"inference {tag}/{k}", lab, torch.from_numpy(ref), acc)
+        msg = f"[inference {tag}/{k}] scores relerr {e:.2e}  pixels without a clear label margin {free}"
         print(msg)
         with open(os.path.join(gpu_out_dir, "model_parity.txt"), "a") as f:
             f.write(msg + "\n")
         assert e < TOL, msg
-        assert agree > 0.995, msg  # near-ties between two classes may flip within TOL
-
-
-def test_resize_flip_window_kernels_vs_aten():
-    gen = torch.Generator().manual_seed(5)
-    x = torch.randn(2, 3, 29, 41, generator=gen).cuda()
-    for (Hd, Wd) in ((29, 41), (44, 30), (13, 97)):
-        for ac in (True, False):
-            ref = torch.nn.functional.interpolate(x, size=(Hd, Wd), mode="bilinear", align_corners=ac)
-            got = ops.resize_nchw(x, Hd, Wd, align_corners=ac)
-            assert (got - ref).abs().max().item() < 2e-6
-            got_f = ops.resize_nchw(x, Hd, Wd, align_corners=ac, flip_x=True)
-            assert (got_f - ref.flip(-1)).abs().max().item() < 2e-6
-    assert torch.equal(ops.resize_nchw(x, 29, 41, flip_x=True), x.flip(-1)), "same-size resize must be an exact flip"
-    acc = torch.ones(2, 3, 44, 30, device="cuda")
-    ops.resize_nchw(x, 44, 30, alpha=0.25, out=acc, beta=2.0)
-    ref = 2.0 + 0.25 * torch.nn.functional.interpolate(x, size=(44, 30), mode="bilinear", align_corners=True)
-    assert (acc - ref).abs().max().item() < 2e-6
-    dst = torch.zeros(2, 3, 50, 60, device="cuda")
-    ops.window_add_nchw(x, dst, 7, 11, 20, 33, alpha=0.5)
-    ops.window_add_nchw(x, dst, 7, 11, 20, 33, flip_x=True, alpha=0.5)
-    ref = torch.zeros_like(dst)
-    ref[:, :, 7:27, 11:44] = 0.5 * x[:, :, :20, :33] + 0.5 * x.flip(-1)[:, :, :20, :33]
-    assert (dst - ref).abs().max().item() < 1e-6
-    cnt = torch.randint(1, 4, (50, 60), generator=gen).float().cuda()
-    assert torch.equal(ops.div_by_count_nchw(dst.clone(), cnt), dst / cnt)
-    s = torch.randn(2, 7, 19, 23, generator=gen).cuda()
-    s[:, 3] = s[:, 1]  # ties: the first maximum wins
-    assert torch.equal(ops.argmax_nchw(s), s.argmax(1))
-
-
-def test_zoom_mode_matches_scipy_including_its_black_edge():
-    """seg_resize_nchw_f32 mode 2 against scipy.ndimage.zoom(order=1, prefilter=False) itself — including the size pairs
-    (e.g. 48 -> 84) where scipy's float64 coordinate of the last column rounds past the last sample and the column is
-    filled with 0 (mode='constant')."""
-    from scipy import ndimage
-    gen = torch.Generator().manual_seed(11)
-    saw_black = False
-    for (H, W) in ((64, 48), (37, 53), (97, 129)):
-        x = torch.randn(1, 3, H, W, generator=gen) + 4.0
-        for s in (0.75, 1.25, 1.5, 1.75, 2.0, 2.25):
-            ref = ndimage.zoom(x.numpy(), (1.0, 1.0, float(s), float(s)), order=1, prefilter=False)
-            got = ops.resize_nchw(x.cuda(), ref.shape[2], ref.shape[3], zoom=True).cpu().numpy()
-            assert got.shape == ref.shape == (1, 3, int(round(H * s)), int(round(W * s)))
-            assert np.abs(got - ref).max() < 2e-6, (H, W, s, np.abs(got - ref).max())
-            saw_black |= bool((ref[..., :, -1] == 0).all() or (ref[..., -1, :] == 0).all())
-    assert saw_black, "the parameter list is meant to include a pair that triggers scipy's constant-fill edge"
 
 
 def test_engine_model_multi_scale_shapes_and_agreement(gpu_out_dir):
