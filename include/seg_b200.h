@@ -153,10 +153,12 @@ int seg_bn_apply(const void* x, int ldx, const float* scale_shift, const void* r
 /* stats: fp64 [2C] from seg_conv2d_fwd / seg_dwconv3x3_fwd / seg_bn_stats over `count` elements (under SyncBN the world's
  * totals and the WORLD's element count).
  * seg_bn_finalize + seg_bn_apply in ONE launch (training mode): coefficients are derived from the batch sums inside the
- * kernel; save[2C] = (mean, 1/std) for the backward pass and the running statistics are written by one block row. */
+ * kernel; save[2C] = (mean, 1/std) for the backward pass and the running statistics are written by one block row.
+ * mask (optional, needs relu): the ReLU bit mask for the backward passes, uint8 [M][C/8] with its own pitch C/8 (independent
+ * of ldo): bit j of mask[m][g] = (stored out[m][8g+j] > 0). */
 int seg_bn_apply_train(const void* x, int ldx, const double* stats, double count, const float* gamma, const float* beta,
                        float eps, float momentum, int clamp_eps, float* running_mean, float* running_var, float* save,
-                       const void* res, int ldr, void* out, int ldo, int64_t M, int C, int relu, float drop_p,
+                       const void* res, int ldr, void* out, int ldo, uint8_t* mask, int64_t M, int C, int relu, float drop_p,
                        uint64_t seed, const uint64_t* step_ctr, int drop_hw, void* stream);
 /* device-side step counter (*ctr += inc): mixed into dropout seeds and SyncBN epochs so a captured CUDA graph of the
  * train step stays correct on every replay */
@@ -172,15 +174,18 @@ int seg_counter_add(uint64_t* ctr, uint64_t inc, void* stream);
  * conv -> BN(batch statistics) -> ReLU with no residual and no dropout; needs gamma and beta.
  * Dropout in the backward (all three backward entry points) needs relu != 0: the keep mask is read from the stored
  * activation (out > 0), which without the ReLU does not tell a dropped element from a negative one, so relu == 0 with
- * drop_p > 0 is rejected. */
+ * drop_p > 0 is rejected.
+ * mask != NULL with relu (all three backward entry points): the ReLU / dropout keep mask is read from the bit mask that
+ * seg_bn_apply_train wrote for this activation (1/16 of the bytes of out; out is then not read); it takes precedence over
+ * out and over the recomputation. */
 int seg_bn_bwd_reduce_slots(void);
-int seg_bn_bwd_reduce(const void* dout, int lddo, const void* out, int ldo, const void* x, int ldx,
+int seg_bn_bwd_reduce(const void* dout, int lddo, const void* out, int ldo, const uint8_t* mask, const void* x, int ldx,
                       const float* save_mean_istd, int64_t M, int C, int relu, float drop_p, float* sums, double* acc,
                       void* ticket, float* dgamma, float* dbeta, int accumulate, const float* gamma, const float* beta,
                       const seg_sync_desc* sync, void* stream);
 /* backward, pass 2: dx = gamma*istd*(dz - sums0/count - xhat*sums1/count); dres = beta_res*dres + dz (optional).
  * `sums` are the sums over `count` elements (under SyncBN the world's, from seg_bn_bwd_reduce). */
-int seg_bn_bwd_apply(const void* dout, int lddo, const void* out, int ldo, const void* x, int ldx,
+int seg_bn_bwd_apply(const void* dout, int lddo, const void* out, int ldo, const uint8_t* mask, const void* x, int ldx,
                      const float* save_mean_istd, const float* gamma, const float* sums, double count, int64_t M,
                      int C, int relu, float drop_p, void* dx, int lddx, void* dres, int lddres, float beta_res,
                      const float* beta, void* stream);
@@ -192,7 +197,7 @@ int seg_bn_bwd_apply(const void* dout, int lddo, const void* out, int ldo, const
  * under SyncBN).  Workspace from seg_bn_bwd_fused_workspace: rows (uninitialised floats) and tickets (uint32, ZERO at launch).
  * The grid is sized to be co-resident. */
 int seg_bn_bwd_fused_workspace(int64_t M, int C, int64_t* rows_floats, int64_t* tickets);
-int seg_bn_bwd_fused(const void* dout, int lddo, const void* out, int ldo, const void* x, int ldx,
+int seg_bn_bwd_fused(const void* dout, int lddo, const void* out, int ldo, const uint8_t* mask, const void* x, int ldx,
                      const float* save_mean_istd, const float* gamma, const float* beta, double count_total, int64_t M,
                      int C, int relu, float drop_p, float* sums, float* rows, void* tickets, float* dgamma, float* dbeta,
                      int accumulate, void* dx, int lddx, void* dres, int lddres, float beta_res, int zero_sums,

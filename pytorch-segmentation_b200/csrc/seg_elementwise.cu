@@ -299,7 +299,8 @@ __global__ void __launch_bounds__(256, 4) bn_apply_kernel(const __nv_bfloat16* _
                                                        const float* __restrict__ ss, const __nv_bfloat16* __restrict__ res,
                                                        int ldr, __nv_bfloat16* __restrict__ out, int ldo, int64_t M, int C,
                                                        int relu, float drop_p, uint64_t seed,
-                                                       const uint64_t* __restrict__ step_ctr, int drop_hw, const BnTrain tr) {
+                                                       const uint64_t* __restrict__ step_ctr, int drop_hw, const BnTrain tr,
+                                                       uint8_t* __restrict__ mask /*[M][C/8] or null*/) {
   pdl_wait();
   const RowMap rm = row_map(C);
   if (step_ctr) seed += (*step_ctr) * 0x9E3779B97F4A7C15ull;  // device-side step counter keeps CUDA-graph replays fresh
@@ -379,11 +380,41 @@ __global__ void __launch_bounds__(256, 4) bn_apply_kernel(const __nv_bfloat16* _
             f[j] = (uu >= drop_p) ? f[j] * keep_scale : 0.f;
           }
         }
-        *reinterpret_cast<bf16x8*>(out + r * ldo + co) = pack8(f);
+        const bf16x8 a = pack8(f);
+        *reinterpret_cast<bf16x8*>(out + r * ldo + co) = a;
+        if (mask) {
+          // bit j = (stored bf16 A > 0): the predicate the activation-reading backward evaluates, on the same values
+          float o[8];
+          unpack8(a, o);
+          unsigned b = 0;
+#pragma unroll
+          for (int j = 0; j < 8; ++j) b |= (o[j] > 0.f ? 1u : 0u) << j;
+          mask[r * (C >> 3) + rm.g] = (uint8_t)b;
+        }
       }
     }
   }
   pdl_trigger();
+}
+
+// Where the backward passes take the ReLU (and dropout keep) mask from:
+//   ACT        the stored activation A (out > 0)
+//   RECOMPUTE  x with the forward's own coefficients (BN -> ReLU with nothing in between, batch statistics, no dropout)
+//   BITS       the bit mask bn_apply wrote in the forward: one byte per (row, 8-channel group), bit j = A[8g+j] > 0 —
+//              1/16 of the bytes of A
+enum class MaskSrc { ACT, RECOMPUTE, BITS };
+// mask source of a backward call: the bit mask when given, else the stored activation, else (relu, out == NULL) recomputed
+static MaskSrc mask_src(int relu, const void* out, const uint8_t* mask) {
+  if (!relu) return MaskSrc::ACT;  // no mask at all (the ACT variants test relu at run time)
+  return mask ? MaskSrc::BITS : out ? MaskSrc::ACT : MaskSrc::RECOMPUTE;
+}
+template <class K>
+static K by_mask_src(MaskSrc ms, K act, K recompute, K bits) {
+  return ms == MaskSrc::BITS ? bits : ms == MaskSrc::RECOMPUTE ? recompute : act;
+}
+__device__ __forceinline__ void apply_mask_bits(unsigned b, float keep_scale, float* dz) {
+#pragma unroll
+  for (int j = 0; j < 8; ++j) dz[j] = ((b >> j) & 1u) ? dz[j] * keep_scale : 0.f;
 }
 
 __device__ __noinline__ void bn_bwd_reduce_finalize(const double* acc, float* final_sums, float* dgamma, float* dbeta, int accumulate,
@@ -405,19 +436,20 @@ __device__ __noinline__ void bn_bwd_reduce_finalize(const double* acc, float* fi
   }
 }
 
-template <bool REMASK>
+template <MaskSrc MS>
 __global__ void __launch_bounds__(256, 4)
     bn_bwd_reduce_kernel(const __nv_bfloat16* __restrict__ dout, int lddo, const __nv_bfloat16* __restrict__ out, int ldo,
-                         const __nv_bfloat16* __restrict__ x, int ldx, const float* __restrict__ save, int64_t M, int C,
+                         const uint8_t* __restrict__ mask, const __nv_bfloat16* __restrict__ x, int ldx,
+                         const float* __restrict__ save, int64_t M, int C,
                          int relu, float drop_p, double* acc /*[RED_SLOTS][2C] fp64, zero at launch*/, unsigned* ticket, float* final_sums,
                          float* dgamma, float* dbeta, int accumulate, const float* __restrict__ gamma,
                          const float* __restrict__ beta, const SyncDesc sync) {
+  constexpr bool REMASK = MS == MaskSrc::RECOMPUTE;
   pdl_wait();
   const float keep_scale = drop_p > 0.f ? 1.f / (1.f - drop_p) : 1.f;
   const RowMap rm = row_map(C);
-  // ReLU mask: from the stored activation, or (out == null: BN -> ReLU with nothing in between, training statistics)
-  // recomputed from x with exactly the forward's coefficients  sc = gamma*istd, sh = fma(-mean, sc, beta)  — one operand
-  // stream less to read
+  // ReLU mask (MaskSrc): RECOMPUTE derives it from x with exactly the forward's coefficients  sc = gamma*istd,
+  // sh = fma(-mean, sc, beta)
   float mean[8], wi[8], sc[REMASK ? 8 : 1], sh[REMASK ? 8 : 1];
   if (rm.active) {
     ld8(save + rm.g * 8, mean);
@@ -442,6 +474,8 @@ __global__ void __launch_bounds__(256, 4)
     if constexpr (REMASK) {
 #pragma unroll
       for (int i = 0; i < 8; ++i) dz[i] = (fmaf(xv[i], sc[i], sh[i]) > 0.f) ? dz[i] : 0.f;
+    } else if constexpr (MS == MaskSrc::BITS) {
+      apply_mask_bits(mask[row * (C >> 3) + g], keep_scale, dz);
     } else if (relu) {
       float o[8];
       unpack8(*reinterpret_cast<const bf16x8*>(out + row * ldo + g * 8), o);
@@ -463,13 +497,15 @@ __global__ void __launch_bounds__(256, 4)
 }
 
 // dx = A*dz + B*x + Cc with A = gamma*istd, B = -gamma*istd^2*s1/count, Cc = -gamma*istd*s0/count + gamma*istd^2*mean*s1/count
-template <bool REMASK>
+template <MaskSrc MS>
 __global__ void __launch_bounds__(256, 4)
     bn_bwd_apply_kernel(const __nv_bfloat16* __restrict__ dout, int lddo, const __nv_bfloat16* __restrict__ out, int ldo,
-                        const __nv_bfloat16* __restrict__ x, int ldx, const float* __restrict__ save,
+                        const uint8_t* __restrict__ mask, const __nv_bfloat16* __restrict__ x, int ldx,
+                        const float* __restrict__ save,
                         const float* __restrict__ gamma, const float* __restrict__ sums, float inv_count, int64_t M, int C,
                         int relu, float drop_p, __nv_bfloat16* __restrict__ dx, int lddx, __nv_bfloat16* dres, int lddres,
                         float beta_res, const float* __restrict__ beta) {
+  constexpr bool REMASK = MS == MaskSrc::RECOMPUTE;
   pdl_wait();
   const RowMap rm = row_map(C);
   const float keep_scale = drop_p > 0.f ? 1.f / (1.f - drop_p) : 1.f;
@@ -507,6 +543,8 @@ __global__ void __launch_bounds__(256, 4)
     if constexpr (REMASK) {
 #pragma unroll
       for (int j = 0; j < 8; ++j) dz[j] = (fmaf(xv[j], cA[j], sh[j]) > 0.f) ? dz[j] : 0.f;
+    } else if constexpr (MS == MaskSrc::BITS) {
+      apply_mask_bits(mask[row * (C >> 3) + rm.g], keep_scale, dz);
     } else if (relu) {
       float o[8];
       unpack8(*reinterpret_cast<const bf16x8*>(out + row * ldo + co), o);
@@ -568,6 +606,7 @@ __device__ __forceinline__ void grid_barrier(unsigned* ctr, unsigned target) {
 
 struct BnBwdFused {
   const __nv_bfloat16 *dout, *out, *x;
+  const uint8_t* mask;  // [M][C/8] ReLU bits (MaskSrc::BITS)
   int lddo, ldo, ldx;
   const float *save, *gamma, *beta;
   int64_t M;
@@ -584,8 +623,9 @@ struct BnBwdFused {
   SyncDesc sync;
 };
 
-template <bool REMASK>
+template <MaskSrc MS>
 __global__ void __launch_bounds__(256, 3) bn_bwd_fused_kernel(const BnBwdFused p) {
+  constexpr bool REMASK = MS == MaskSrc::RECOMPUTE;
   const RowMap rm = row_map(p.C);
   const int C = p.C;
   const int co = rm.g * 8;
@@ -622,6 +662,8 @@ __global__ void __launch_bounds__(256, 3) bn_bwd_fused_kernel(const BnBwdFused p
         if constexpr (REMASK) {
 #pragma unroll
           for (int j = 0; j < 8; ++j) dz[j] = (fmaf(xv[j], gm[j] * istd[j], sh[j]) > 0.f) ? dz[j] : 0.f;
+        } else if constexpr (MS == MaskSrc::BITS) {
+          apply_mask_bits(p.mask[row * (C >> 3) + rm.g], keep_scale, dz);
         } else if (p.relu) {
           float o[8];
           unpack8(*reinterpret_cast<const bf16x8*>(p.out + row * p.ldo + co), o);
@@ -724,6 +766,8 @@ __global__ void __launch_bounds__(256, 3) bn_bwd_fused_kernel(const BnBwdFused p
       if constexpr (REMASK) {
 #pragma unroll
         for (int j = 0; j < 8; ++j) dz[j] = (fmaf(xv[j], cA[j], sh[j]) > 0.f) ? dz[j] : 0.f;
+      } else if constexpr (MS == MaskSrc::BITS) {
+        apply_mask_bits(p.mask[row * (C >> 3) + rm.g], keep_scale, dz);
       } else if (p.relu) {
         float o[8];
         unpack8(*reinterpret_cast<const bf16x8*>(p.out + row * p.ldo + co), o);
@@ -1573,61 +1617,75 @@ int seg_bn_apply(const void* x, int ldx, const float* ss, const void* res, int l
   BnTrain tr;
   memset(&tr, 0, sizeof(tr));
   launch_pdl(bn_apply_kernel, rowmap_grid(M, C), dim3(256), 0, ST(stream), CBF(x), ldx, ss, CBF(res), ldr, BF(out), ldo, M, C, relu,
-             drop_p, seed, step_ctr, drop_hw, tr);
+             drop_p, seed, step_ctr, drop_hw, tr, (uint8_t*)nullptr);
   return check_launch("bn_apply");
 }
 int seg_bn_apply_train(const void* x, int ldx, const double* stats, double count, const float* gamma, const float* beta,
                        float eps, float momentum, int clamp_eps, float* running_mean, float* running_var, float* save,
-                       const void* res, int ldr, void* out, int ldo, int64_t M, int C, int relu, float drop_p,
+                       const void* res, int ldr, void* out, int ldo, uint8_t* mask, int64_t M, int C, int relu, float drop_p,
                        uint64_t seed, const uint64_t* step_ctr, int drop_hw, void* stream) {
   SEG_REQUIRE(C % 8 == 0 && ldx % 8 == 0 && ldo % 8 == 0 && (!res || ldr % 8 == 0), "bn_apply_train: alignment");
   SEG_REQUIRE(stats && gamma && beta && save && count > 0, "bn_apply_train: stats, gamma, beta, save required");
+  SEG_REQUIRE(!mask || relu, "bn_apply_train: the ReLU bit mask needs relu");
   BnTrain tr = {stats, count, gamma, beta, eps, momentum, clamp_eps, running_mean, running_var, save};
   launch_pdl(bn_apply_kernel, rowmap_grid(M, C), dim3(256), 0, ST(stream), CBF(x), ldx, (const float*)nullptr, CBF(res), ldr, BF(out),
-             ldo, M, C, relu, drop_p, seed, step_ctr, drop_hw, tr);
+             ldo, M, C, relu, drop_p, seed, step_ctr, drop_hw, tr, mask);
   return check_launch("bn_apply_train");
 }
 // reductions end with a block fold + 2C atomics per block: fewer, fatter blocks (>= 32 rows per thread)
 static dim3 reduce2_grid(int64_t M, int C) { return rowmap_grid(M, C, 32); }
 
 int seg_bn_bwd_reduce_slots(void) { return RED_SLOTS; }
-int seg_bn_bwd_reduce(const void* dout, int lddo, const void* out, int ldo, const void* x, int ldx, const float* save,
-                      int64_t M, int C, int relu, float drop_p, float* sums, double* acc, void* ticket, float* dgamma,
-                      float* dbeta, int accumulate, const float* gamma, const float* beta, const seg_sync_desc* sync,
-                      void* stream) {
-  SEG_REQUIRE(C % 8 == 0 && lddo % 8 == 0 && ldx % 8 == 0 && (!relu || !out || ldo % 8 == 0), "bn_bwd_reduce: alignment");
-  SEG_REQUIRE(!(relu && !out) || (gamma && beta && drop_p == 0.f), "bn_bwd_reduce: out == NULL (mask recomputed from x) needs gamma, beta and no dropout");
+int seg_bn_bwd_reduce(const void* dout, int lddo, const void* out, int ldo, const uint8_t* mask, const void* x, int ldx,
+                      const float* save, int64_t M, int C, int relu, float drop_p, float* sums, double* acc, void* ticket,
+                      float* dgamma, float* dbeta, int accumulate, const float* gamma, const float* beta,
+                      const seg_sync_desc* sync, void* stream) {
+  const MaskSrc ms = mask_src(relu, out, mask);
+  SEG_REQUIRE(C % 8 == 0 && lddo % 8 == 0 && ldx % 8 == 0 && (ms != MaskSrc::ACT || !relu || ldo % 8 == 0), "bn_bwd_reduce: alignment");
+  SEG_REQUIRE(ms != MaskSrc::RECOMPUTE || (gamma && beta && drop_p == 0.f), "bn_bwd_reduce: out == NULL (mask recomputed from x) needs gamma, beta and no dropout");
   SEG_REQUIRE(relu || drop_p == 0.f, "bn_bwd_reduce: dropout (drop_p > 0) needs relu: the keep mask is read from out > 0");
   SEG_REQUIRE(acc && ticket, "bn_bwd_reduce: zeroed fp64 accumulators [seg_bn_bwd_reduce_slots()][2C] and ticket word required");
   SEG_REQUIRE(!sync || 2 * C <= sync->n_max, "bn_bwd_reduce: 2*C exceeds the SyncBN buffer");
   const dim3 grid = reduce2_grid(M, C);
-  launch_pdl((relu && !out) ? bn_bwd_reduce_kernel<true> : bn_bwd_reduce_kernel<false>, grid, dim3(256), 0, ST(stream), CBF(dout),
-             lddo, CBF(out), ldo, CBF(x), ldx, save, M, C, relu, drop_p, acc, reinterpret_cast<unsigned*>(ticket), sums, dgamma, dbeta,
-             accumulate, gamma, beta, to_sync(sync));
+  launch_pdl(by_mask_src(ms, bn_bwd_reduce_kernel<MaskSrc::ACT>, bn_bwd_reduce_kernel<MaskSrc::RECOMPUTE>,
+                         bn_bwd_reduce_kernel<MaskSrc::BITS>),
+             grid, dim3(256), 0, ST(stream), CBF(dout), lddo, CBF(out), ldo, mask, CBF(x), ldx, save, M, C, relu, drop_p, acc,
+             reinterpret_cast<unsigned*>(ticket), sums, dgamma, dbeta, accumulate, gamma, beta, to_sync(sync));
   return check_launch("bn_bwd_reduce");
 }
-int seg_bn_bwd_apply(const void* dout, int lddo, const void* out, int ldo, const void* x, int ldx, const float* save,
-                     const float* gamma, const float* sums, double count, int64_t M, int C, int relu, float drop_p,
-                     void* dx, int lddx, void* dres, int lddres, float beta_res, const float* beta, void* stream) {
+int seg_bn_bwd_apply(const void* dout, int lddo, const void* out, int ldo, const uint8_t* mask, const void* x, int ldx,
+                     const float* save, const float* gamma, const float* sums, double count, int64_t M, int C, int relu,
+                     float drop_p, void* dx, int lddx, void* dres, int lddres, float beta_res, const float* beta, void* stream) {
+  const MaskSrc ms = mask_src(relu, out, mask);
   SEG_REQUIRE(C % 8 == 0 && lddo % 8 == 0 && ldx % 8 == 0 && lddx % 8 == 0, "bn_bwd_apply: alignment");
-  SEG_REQUIRE(!(relu && !out) || (beta && drop_p == 0.f), "bn_bwd_apply: out == NULL (mask recomputed from x) needs beta and no dropout");
+  SEG_REQUIRE(ms != MaskSrc::RECOMPUTE || (beta && drop_p == 0.f), "bn_bwd_apply: out == NULL (mask recomputed from x) needs beta and no dropout");
   SEG_REQUIRE(relu || drop_p == 0.f, "bn_bwd_apply: dropout (drop_p > 0) needs relu: the keep mask is read from out > 0");
-  launch_pdl((relu && !out) ? bn_bwd_apply_kernel<true> : bn_bwd_apply_kernel<false>, rowmap_grid(M, C), dim3(256), 0, ST(stream),
-             CBF(dout), lddo, CBF(out), ldo, CBF(x), ldx, save,
+  launch_pdl(by_mask_src(ms, bn_bwd_apply_kernel<MaskSrc::ACT>, bn_bwd_apply_kernel<MaskSrc::RECOMPUTE>,
+                         bn_bwd_apply_kernel<MaskSrc::BITS>),
+             rowmap_grid(M, C), dim3(256), 0, ST(stream), CBF(dout), lddo, CBF(out), ldo, mask, CBF(x), ldx, save,
              gamma, sums, (float)(1.0 / count), M, C, relu, drop_p, BF(dx), lddx, BF(dres), lddres, beta_res, beta);
   return check_launch("bn_bwd_apply");
 }
 }  // extern "C"
 // co-resident grid of the cooperative kernel: blocks per SM from the occupancy of the instantiation actually launched
-template <bool REMASK>
+template <MaskSrc MS>
 static int fused_blocks_per_sm() {
   static int v = 0;
   if (v == 0) {
     int n = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, bn_bwd_fused_kernel<REMASK>, 256, 0) != cudaSuccess || n < 1) n = 1;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, bn_bwd_fused_kernel<MS>, 256, 0) != cudaSuccess || n < 1) n = 1;
     v = n;
   }
   return v;
+}
+// The grid fixes which rows each block sums, and so the rounding of the fp32 partial sums: the BITS variant runs on the
+// ACT variant's grid (when it fits), so that its sums and dx are bit-identical to those read from the activation
+static int fused_bps(MaskSrc ms) {
+  if (ms == MaskSrc::RECOMPUTE) return fused_blocks_per_sm<MaskSrc::RECOMPUTE>();
+  const int act = fused_blocks_per_sm<MaskSrc::ACT>();
+  if (ms == MaskSrc::ACT) return act;
+  const int bits = fused_blocks_per_sm<MaskSrc::BITS>();
+  return bits < act ? bits : act;
 }
 extern "C" {
 static dim3 fused_grid(int64_t M, int C, int blocks_per_sm) {
@@ -1638,26 +1696,27 @@ static dim3 fused_grid(int64_t M, int C, int blocks_per_sm) {
 }
 int seg_bn_bwd_fused_workspace(int64_t M, int C, int64_t* rows_floats, int64_t* tickets) {
   SEG_REQUIRE(C % 8 == 0 && rows_floats && tickets, "seg_bn_bwd_fused_workspace: bad arguments");
-  const int bps = fused_blocks_per_sm<true>() > fused_blocks_per_sm<false>() ? fused_blocks_per_sm<true>() : fused_blocks_per_sm<false>();
+  const int b0 = fused_bps(MaskSrc::ACT), b1 = fused_bps(MaskSrc::RECOMPUTE), b2 = fused_bps(MaskSrc::BITS);
+  const int bps = b0 > b1 ? (b0 > b2 ? b0 : b2) : (b1 > b2 ? b1 : b2);
   const dim3 g = fused_grid(M, C, bps);
   const int G = C / 8, GB = G < 256 ? G : 256;
   *rows_floats = (int64_t)g.y * g.x * 2 * GB * 8;
   *tickets = 1;
   return 0;
 }
-int seg_bn_bwd_fused(const void* dout, int lddo, const void* out, int ldo, const void* x, int ldx, const float* save,
-                     const float* gamma, const float* beta, double count_total, int64_t M, int C, int relu, float drop_p,
-                     float* sums, float* rows, void* tickets, float* dgamma, float* dbeta, int accumulate, void* dx, int lddx,
-                     void* dres, int lddres, float beta_res, int zero_sums, const seg_sync_desc* sync, void* stream) {
+int seg_bn_bwd_fused(const void* dout, int lddo, const void* out, int ldo, const uint8_t* mask, const void* x, int ldx,
+                     const float* save, const float* gamma, const float* beta, double count_total, int64_t M, int C, int relu,
+                     float drop_p, float* sums, float* rows, void* tickets, float* dgamma, float* dbeta, int accumulate, void* dx,
+                     int lddx, void* dres, int lddres, float beta_res, int zero_sums, const seg_sync_desc* sync, void* stream) {
+  const MaskSrc ms = mask_src(relu, out, mask);
   SEG_REQUIRE(C % 8 == 0 && lddo % 8 == 0 && ldx % 8 == 0 && lddx % 8 == 0 && (!out || ldo % 8 == 0) && (!dres || lddres % 8 == 0),
               "bn_bwd_fused: alignment");
-  SEG_REQUIRE(!(relu && !out) || (beta && drop_p == 0.f), "bn_bwd_fused: out == NULL (mask recomputed from x) needs beta and no dropout");
+  SEG_REQUIRE(ms != MaskSrc::RECOMPUTE || (beta && drop_p == 0.f), "bn_bwd_fused: out == NULL (mask recomputed from x) needs beta and no dropout");
   SEG_REQUIRE(relu || drop_p == 0.f, "bn_bwd_fused: dropout (drop_p > 0) needs relu: the keep mask is read from out > 0");
   SEG_REQUIRE(sums && rows && tickets && gamma && save && dx && count_total > 0, "bn_bwd_fused: missing buffer");
-  const bool remask = relu && !out;
   BnBwdFused p;
   memset(&p, 0, sizeof(p));
-  p.dout = CBF(dout); p.out = CBF(out); p.x = CBF(x);
+  p.dout = CBF(dout); p.out = CBF(out); p.x = CBF(x); p.mask = mask;
   p.lddo = lddo; p.ldo = ldo; p.ldx = ldx;
   p.save = save; p.gamma = gamma; p.beta = beta;
   p.M = M; p.C = C; p.relu = relu; p.drop_p = drop_p; p.inv_count = (float)(1.0 / count_total);
@@ -1670,13 +1729,11 @@ int seg_bn_bwd_fused(const void* dout, int lddo, const void* out, int ldo, const
   }
   // multi-GPU: leave one block slot per SM free — a concurrently running NCCL kernel (bucketed gradient all-reduce on the side
   // stream) must not keep part of this grid from becoming resident, or every block would sit at the barrier until it finishes
-  int bps = remask ? fused_blocks_per_sm<true>() : fused_blocks_per_sm<false>();
+  int bps = fused_bps(ms);
   if (sync && bps > 1) bps -= 1;
   const dim3 grid = fused_grid(M, C, bps);
-  if (remask)
-    bn_bwd_fused_kernel<true><<<grid, 256, 0, ST(stream)>>>(p);
-  else
-    bn_bwd_fused_kernel<false><<<grid, 256, 0, ST(stream)>>>(p);
+  by_mask_src(ms, bn_bwd_fused_kernel<MaskSrc::ACT>, bn_bwd_fused_kernel<MaskSrc::RECOMPUTE>,
+              bn_bwd_fused_kernel<MaskSrc::BITS>)<<<grid, 256, 0, ST(stream)>>>(p);
   return check_launch("bn_bwd_fused");
 }
 int seg_bn_param_grad(const float* sums, int C, float* dgamma, float* dbeta, int accumulate, void* stream) {

@@ -370,6 +370,10 @@ class Tape:
         if drop_p > 0.0:
             self._drop_ctr += 1
             seed = (self.seed * 1000003 + self._drop_ctr * 7919) & 0x7FFFFFFFFFFFFFFF  # + step counter on the device
+        # conv -> BN(batch statistics) -> ReLU with nothing in between: the ReLU mask can be recomputed from the conv output
+        # with the forward's own coefficients instead of being read (the one-launch backward of the small maps does so)
+        remask = bool(use_batch_stats and relu and res is None and drop_p == 0.0)
+        mask_kw = {}
         if use_batch_stats:
             if stats is None:
                 sync0 = self.sync if self.sync_fused() else None
@@ -383,13 +387,20 @@ class Tape:
                     # exchange object without the in-kernel protocol (the gloo stand-in of the CPU tests): sums over ranks
                     self.sync.allreduce_(stats)
                 count = count_local * self.sync.world
+            # the ReLU mask of the backward passes as bits, written by the forward apply: 1/16 of the bytes of re-reading
+            # the activation, and on the large maps faster than recomputing it too (the reduce's recomputing variant
+            # needs 74 registers: 3 blocks/SM instead of 4).  Not written where the one-launch backward recomputes it
+            # (remask on a small map).  A kernel layer without the bit mask (the ATen stand-in of the host-logic tests)
+            # reads the activation.
+            if relu and hasattr(ops, "relu_mask") and not (remask and count_local * C * 2 <= FUSED_BWD_MAX_BYTES):
+                mask_kw = {"mask": ops.relu_mask(y.t)}
             # finalize (coefficients, saved mean / 1/std, running statistics) happens inside the apply kernel
             a, save = ops.bn_apply_train(y.t, stats, count, bn.weight.detach(), bn.bias.detach(), bn.eps,
                                          bn.momentum if bn.momentum is not None else BN_MOM,
                                          1 if (self.clamp_eps and self.sync is not None and self.sync.world > 1) else 0,
                                          bn.running_mean, bn.running_var, res=res.t if res is not None else None, out=out,
                                          relu=relu, drop_p=drop_p, seed=seed, step_ctr=self.step_ctr if drop_p > 0.0 else None,
-                                         drop_hw=drop_hw)
+                                         drop_hw=drop_hw, **mask_kw)
             self.bn_modules.append(bn)
         else:
             ss, save = ops.bn_eval_scale_shift(bn.weight.detach(), bn.bias.detach(), bn.running_mean, bn.running_var, bn.eps,
@@ -398,11 +409,6 @@ class Tape:
             a = ops.bn_apply(y.t, ss, res=res.t if res is not None else None, out=out, relu=relu, drop_p=drop_p, seed=seed,
                              step_ctr=self.step_ctr if drop_p > 0.0 else None, drop_hw=drop_hw)
         aa = Act(a)
-        # conv -> BN(batch statistics) -> ReLU with nothing in between: the backward APPLY pass recomputes the ReLU mask
-        # from the conv output with the forward's own coefficients instead of re-reading the activation (one stream less).
-        # The reduce pass keeps reading the activation: its mask-recomputing variant needs 74 registers (3 blocks/SM
-        # instead of 4) and measured slower.
-        remask = bool(use_batch_stats and relu and res is None and drop_p == 0.0)
         if self.record:
             def bwd():
                 da = aa.grad
@@ -415,7 +421,7 @@ class Tape:
                 if want_pg and not acc_pg:
                     self.grads[bn.weight] = torch.empty(C, dtype=torch.float32, device=a.device)
                     self.grads[bn.bias] = torch.empty(C, dtype=torch.float32, device=a.device)
-                a_mask = None if remask else a
+                a_mask = None if remask else a  # the bit mask in mask_kw takes precedence
                 dy = torch.empty(y.t.shape, dtype=ACT_DTYPE, device=a.device)
                 dres, beta_res = (None, 0.0)
                 if res is not None and res.needs_grad:
@@ -426,11 +432,11 @@ class Tape:
                 if sync is not None and not getattr(sync, "fused", False):
                     # exchange object without the in-kernel protocol (the gloo stand-in of the CPU tests)
                     sums = ops.bn_bwd_reduce(da, a, y.t, save, relu=relu, drop_p=drop_p, dgamma=dg, dbeta=db, accumulate=acc_pg,
-                                             acc=self.zalloc64(ops.bn_bwd_reduce_acc_words(C), a.device))
+                                             acc=self.zalloc64(ops.bn_bwd_reduce_acc_words(C), a.device), **mask_kw)
                     gsums = sums.clone()
                     sync.allreduce_(gsums)
                     ops.bn_bwd_apply(da, a_mask, y.t, save, bn.weight.detach(), gsums, count, relu=relu, drop_p=drop_p, dx=dy,
-                                     dres=dres, beta_res=beta_res, beta=bn.bias.detach())
+                                     dres=dres, beta_res=beta_res, beta=bn.bias.detach(), **mask_kw)
                 elif count_local * C * 2 <= FUSED_BWD_MAX_BYTES:
                     # small maps (the operands stay in L2 between the phases): reduce -> grid barrier -> fixed-order cross-block
                     # sum (-> SyncBN exchange) -> apply in ONE cooperative launch.  Frozen BN (freeze_bn): dx = gamma*inv_std*dz,
@@ -438,15 +444,15 @@ class Tape:
                     # grid-barrier counter
                     ops.bn_bwd_fused(da, a_mask, y.t, save, bn.weight.detach(), count, relu=relu, drop_p=drop_p, dgamma=dg, dbeta=db,
                                      accumulate=acc_pg, dx=dy, dres=dres, beta_res=beta_res, beta=bn.bias.detach(),
-                                     zero_sums=not use_batch_stats, tickets=self.zalloc(1, a.device), sync=sync)
+                                     zero_sums=not use_batch_stats, tickets=self.zalloc(1, a.device), sync=sync, **mask_kw)
                 else:
                     # large maps stream from HBM in both passes anyway: two launches at full occupancy; under SyncBN the
                     # reduction's last block exchanges the sums, so the apply pass gets the world's
                     sums = ops.bn_bwd_reduce(da, a, y.t, save, relu=relu, drop_p=drop_p, dgamma=dg, dbeta=db, accumulate=acc_pg,
-                                             acc=self.zalloc64(ops.bn_bwd_reduce_acc_words(C), a.device), sync=sync)
+                                             acc=self.zalloc64(ops.bn_bwd_reduce_acc_words(C), a.device), sync=sync, **mask_kw)
                     gsums = sums if use_batch_stats else torch.zeros_like(sums)
                     ops.bn_bwd_apply(da, a_mask, y.t, save, bn.weight.detach(), gsums, count, relu=relu, drop_p=drop_p, dx=dy,
-                                     dres=dres, beta_res=beta_res, beta=bn.bias.detach())
+                                     dres=dres, beta_res=beta_res, beta=bn.bias.detach(), **mask_kw)
                 y.grad = dy
                 aa.grad = None
             self._push_back(bwd, (bn.weight, bn.bias))

@@ -68,12 +68,12 @@ _SIGS = {
     "seg_bn_apply": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int64, c_int, c_int, c_float, c_uint64, c_void_p, c_int, c_void_p]),
     "seg_counter_add": (c_int, [c_void_p, c_uint64, c_void_p]),
     "seg_bn_bwd_reduce_slots": (c_int, []),
-    "seg_bn_bwd_reduce": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int64, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
-    "seg_bn_apply_train": (c_int, [c_void_p, c_int, c_void_p, c_double, c_void_p, c_void_p, c_float, c_float, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int64, c_int, c_int, c_float, c_uint64, c_void_p, c_int, c_void_p]),
+    "seg_bn_bwd_reduce": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int64, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "seg_bn_apply_train": (c_int, [c_void_p, c_int, c_void_p, c_double, c_void_p, c_void_p, c_float, c_float, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int64, c_int, c_int, c_float, c_uint64, c_void_p, c_int, c_void_p]),
     "seg_bn_bwd_fused_workspace": (c_int, [c_int64, c_int, POINTER(c_int64), POINTER(c_int64)]),
-    "seg_bn_bwd_fused": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_double, c_int64, c_int, c_int, c_float,
+    "seg_bn_bwd_fused": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_double, c_int64, c_int, c_int, c_float,
                                  c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_float, c_int, c_void_p, c_void_p]),
-    "seg_bn_bwd_apply": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_double, c_int64, c_int, c_int, c_float, c_void_p, c_int, c_void_p, c_int, c_float, c_void_p, c_void_p]),
+    "seg_bn_bwd_apply": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_double, c_int64, c_int, c_int, c_float, c_void_p, c_int, c_void_p, c_int, c_float, c_void_p, c_void_p]),
     "seg_bn_param_grad": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p]),
     "seg_maxpool3x3s2_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "seg_maxpool3x3s2_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),

@@ -271,18 +271,42 @@ def counter_add(ctr, inc=1):
     call("seg_counter_add", ptr(ctr), int(inc))
 
 
+MASK_PASS = 1.0 / 16  # the ReLU bit mask: 1 bit per element, in bf16 passes over M x C
+
+
+def relu_mask(x):
+    """Uninitialised ReLU bit-mask buffer for the activation of BN over x (bn_apply_train(mask=) fills it, the backward
+    passes read it): uint8 [M][C/8], bit j of [m][g] = activation[m][8g+j] > 0; its own pitch C/8, whatever the
+    activation's channel pitch."""
+    return torch.empty((rows(x), x.shape[-1] // 8), dtype=torch.uint8, device=x.device)
+
+
+def _check_mask(mask, x):
+    if mask is not None:
+        assert mask.dtype == torch.uint8 and mask.is_contiguous() and tuple(mask.shape) == (rows(x), x.shape[-1] // 8), \
+            "mask: uint8 [M][C/8] from relu_mask()"
+
+
+def _mask_passes(relu, out, mask):
+    """bf16 passes over M x C the backward spends on the ReLU mask: the bits, the activation, or none (recomputed)."""
+    if not relu:
+        return 0
+    return MASK_PASS if mask is not None else (1 if out is not None else 0)
+
+
 def bn_bwd_reduce_acc_words(C):
     """fp64 words of the zeroed accumulator block of bn_bwd_reduce: [slots][2C] sums + one ticket word."""
     return int(lib.load().seg_bn_bwd_reduce_slots()) * 2 * C + 1
 
 
 def bn_bwd_reduce(dout, out, x, save, relu=True, drop_p=0.0, dgamma=None, dbeta=None, accumulate=False, acc=None,
-                  gamma=None, beta=None, sync=None):
+                  gamma=None, beta=None, sync=None, mask=None):
     """Returns sums fp32 [2C] = (sum dz, sum dz*xhat); optionally writes the parameter gradients from them.  One launch: fp64
     atomics into `acc` (exact, bit-reproducible), the last block rounds / writes.  acc: zeroed fp64 [bn_bwd_reduce_acc_words(C)]
     (accumulator copies + ticket) from the caller's arena, allocated here if None.  sync: SyncBN — the last block exchanges the sums with the
     peers and the returned sums are the world's.
-    out=None (with relu, gamma, beta): the ReLU mask is recomputed from x instead of read from the stored activation."""
+    out=None (with relu, gamma, beta): the ReLU mask is recomputed from x instead of read from the stored activation.
+    mask: the ReLU bit mask bn_apply_train wrote for this activation (read instead of out)."""
     C = x.shape[-1]
     M = rows(x)
     sums = torch.empty(2 * C, dtype=torch.float32, device=x.device)
@@ -290,37 +314,42 @@ def bn_bwd_reduce(dout, out, x, save, relu=True, drop_p=0.0, dgamma=None, dbeta=
     if acc is None:
         acc = torch.zeros(nw, dtype=torch.float64, device=x.device)
     assert acc.dtype == torch.float64 and acc.numel() >= nw
-    call("seg_bn_bwd_reduce", ptr(dout), ld(dout), ptr(out), ld(out) if out is not None else 0, ptr(x), ld(x), ptr(save),
+    _check_mask(mask, x)
+    call("seg_bn_bwd_reduce", ptr(dout), ld(dout), ptr(out), ld(out) if out is not None else 0, ptr(mask), ptr(x), ld(x), ptr(save),
          M, C, int(relu), float(drop_p), ptr(sums), ptr(acc), acc.data_ptr() + 8 * (nw - 1), ptr(dgamma), ptr(dbeta), int(accumulate),
          ptr(gamma), ptr(beta), ctypes.addressof(sync.desc) if sync is not None else None,
-         meta=_meta_rows(M, C, 3 if (relu and out is not None) else 2))
+         meta=_meta_rows(M, C, 2 + _mask_passes(relu, out, mask)))
     return sums
 
 
 def bn_apply_train(x, stats, count, gamma, beta, eps, momentum, clamp_eps, running_mean, running_var, res=None, out=None,
-                   relu=True, drop_p=0.0, seed=0, step_ctr=None, drop_hw=0):
+                   relu=True, drop_p=0.0, seed=0, step_ctr=None, drop_hw=0, mask=None):
     """Training-mode BN (+residual, ReLU, dropout) straight from the batch sums.  Returns (out, save[2C]).
-    Under SyncBN the producer called with sync= has left the world's sums in `stats`; `count` is then the world's."""
+    Under SyncBN the producer called with sync= has left the world's sums in `stats`; `count` is then the world's.
+    mask (with relu): relu_mask(x) buffer, filled with the ReLU bit mask of out for the backward passes."""
     C = x.shape[-1]
     if out is None:
         out = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
     save = torch.empty(2 * C, dtype=torch.float32, device=x.device)
     assert stats.dtype == torch.float64
+    _check_mask(mask, x)
     call("seg_bn_apply_train", ptr(x), ld(x), ptr(stats), float(count), ptr(gamma), ptr(beta), float(eps), float(momentum),
          int(clamp_eps), ptr(running_mean), ptr(running_var), ptr(save), ptr(res), ld(res) if res is not None else 0,
-         ptr(out), ld(out), rows(x), C, int(relu), float(drop_p), int(seed), ptr(step_ctr), int(drop_hw),
-         meta=_meta_rows(rows(x), C, 3 if res is not None else 2, res is not None))
+         ptr(out), ld(out), ptr(mask), rows(x), C, int(relu), float(drop_p), int(seed), ptr(step_ctr), int(drop_hw),
+         meta=_meta_rows(rows(x), C, (3 if res is not None else 2) + (MASK_PASS if mask is not None else 0), res is not None))
     return out, save
 
 
-def bn_bwd_apply(dout, out, x, save, gamma, sums, count, relu=True, drop_p=0.0, dx=None, dres=None, beta_res=0.0, beta=None):
+def bn_bwd_apply(dout, out, x, save, gamma, sums, count, relu=True, drop_p=0.0, dx=None, dres=None, beta_res=0.0, beta=None,
+                 mask=None):
     C = x.shape[-1]
     if dx is None:
         dx = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
-    call("seg_bn_bwd_apply", ptr(dout), ld(dout), ptr(out), ld(out) if out is not None else 0, ptr(x), ld(x), ptr(save),
+    _check_mask(mask, x)
+    call("seg_bn_bwd_apply", ptr(dout), ld(dout), ptr(out), ld(out) if out is not None else 0, ptr(mask), ptr(x), ld(x), ptr(save),
          ptr(gamma), ptr(sums), float(count), rows(x), C, int(relu), float(drop_p), ptr(dx), ld(dx), ptr(dres),
          ld(dres) if dres is not None else 0, float(beta_res), ptr(beta),
-         meta=_meta_rows(rows(x), C, (3 if (relu and out is not None) else 2) + 1 + (0 if dres is None else (2 if beta_res != 0.0 else 1)), dres is not None))
+         meta=_meta_rows(rows(x), C, 2 + _mask_passes(relu, out, mask) + 1 + (0 if dres is None else (2 if beta_res != 0.0 else 1)), dres is not None))
     return dx
 
 
@@ -336,10 +365,10 @@ def bn_bwd_fused_workspace(M, C):
 
 
 def bn_bwd_fused(dout, out, x, save, gamma, count_total, relu=True, drop_p=0.0, dgamma=None, dbeta=None, accumulate=False,
-                 dx=None, dres=None, beta_res=0.0, beta=None, zero_sums=False, tickets=None, sync=None):
+                 dx=None, dres=None, beta_res=0.0, beta=None, zero_sums=False, tickets=None, sync=None, mask=None):
     """BatchNorm backward in ONE cooperative launch (reduce -> grid barrier -> fixed-order cross-block sum [-> SyncBN exchange]
     -> apply).  Returns (dx, sums [2C]: the world's under sync).  out=None: ReLU mask recomputed from x (needs beta).  tickets:
-    bn_bwd_fused_workspace(M, C)[1] zeroed words."""
+    bn_bwd_fused_workspace(M, C)[1] zeroed words.  mask: ReLU bit mask from bn_apply_train (read instead of out)."""
     C = x.shape[-1]
     M = rows(x)
     if dx is None:
@@ -349,11 +378,12 @@ def bn_bwd_fused(dout, out, x, save, gamma, count_total, relu=True, drop_p=0.0, 
     fr = torch.empty(max(nr, 1), dtype=torch.float32, device=x.device)
     if tickets is None:
         tickets = torch.zeros(max(nt, 1), dtype=torch.float32, device=x.device)
-    call("seg_bn_bwd_fused", ptr(dout), ld(dout), ptr(out), ld(out) if out is not None else 0, ptr(x), ld(x), ptr(save), ptr(gamma),
+    _check_mask(mask, x)
+    call("seg_bn_bwd_fused", ptr(dout), ld(dout), ptr(out), ld(out) if out is not None else 0, ptr(mask), ptr(x), ld(x), ptr(save), ptr(gamma),
          ptr(beta), float(count_total), M, C, int(relu), float(drop_p), ptr(sums), ptr(fr), ptr(tickets), ptr(dgamma), ptr(dbeta),
          int(accumulate), ptr(dx), ld(dx), ptr(dres), ld(dres) if dres is not None else 0, float(beta_res), int(zero_sums),
          ctypes.addressof(sync.desc) if sync is not None else None,
-         meta=_meta_rows(M, C, (3 if (relu and out is not None) else 2) * 2 + 1 + (0 if dres is None else (2 if beta_res != 0.0 else 1)), dres is not None))
+         meta=_meta_rows(M, C, (2 + _mask_passes(relu, out, mask)) * 2 + 1 + (0 if dres is None else (2 if beta_res != 0.0 else 1)), dres is not None))
     return dx, sums
 
 
