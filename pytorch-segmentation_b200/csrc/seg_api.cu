@@ -2,6 +2,7 @@
 // (wgmma path where the shape allows it, CUDA-core implicit GEMM otherwise).  No CPU fallback anywhere.
 #include <stdarg.h>
 #include "seg_common.cuh"
+#include "seg_sync.cuh"
 
 namespace seg {
 
@@ -78,6 +79,7 @@ int seg_conv2d_fwd(const seg_conv_desc* d, const void* x, const void* w_packed, 
                    float beta, double* stats, const seg_sync_desc* sync, void* sync_ticket, int impl, void* stream) {
   if (check_desc(d)) return 1;
   SEG_REQUIRE(!sync || (stats && sync_ticket), "seg_conv2d_fwd: SyncBN needs stats and a zeroed ticket word");
+  if (sync && sync_check_desc(sync, 4ll * d->K, "seg_conv2d_fwd")) return 1;  // 2K fp64 statistics
   SEG_REQUIRE(!stats || beta == 0.f, "seg_conv2d_fwd: BatchNorm statistics need beta = 0 (got beta = %g)", (double)beta);
   const bool tc_ok = tc::supported(d) && tma_base_ok(x) && tma_base_ok(w_packed);
   unsigned* tk = reinterpret_cast<unsigned*>(sync_ticket);

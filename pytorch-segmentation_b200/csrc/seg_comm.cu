@@ -61,14 +61,7 @@ int seg_comm_ipc_close(void* ptr) {
 }
 
 int seg_syncbn_exchange(const seg_sync_desc* sync, float* vals, int n, void* stream) {
-  // the handle is read on the host: a device address (such as the peer-pointer array itself) is refused, not dereferenced
-  cudaPointerAttributes attr;
-  const bool host_handle = sync != nullptr && cudaPointerGetAttributes(&attr, sync) == cudaSuccess && attr.type != cudaMemoryTypeDevice;
-  if (!host_handle) cudaGetLastError();  // a failed query must not surface at the next launch check
-  SEG_REQUIRE(host_handle, "syncbn exchange: `sync` must point to a seg_sync_desc in host memory");
-  SEG_REQUIRE(sync->world >= 1 && sync->world <= 64 && sync->rank >= 0 && sync->rank < sync->world, "bad rank/world %d/%d",
-              sync->rank, sync->world);
-  SEG_REQUIRE(n > 0 && n <= sync->n_max, "syncbn exchange: n=%d exceeds n_max=%d", n, sync->n_max);
+  if (sync_check_desc(sync, n, "syncbn exchange")) return 1;
   // >= 64 threads: thread p < world raises this rank's flag on peer p and waits for peer p's
   const int threads = n >= 1024 ? 1024 : ((n + 31) / 32 * 32 < 64 ? 64 : (n + 31) / 32 * 32);
   syncbn_exchange_kernel<<<1, threads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(*sync, vals, n);

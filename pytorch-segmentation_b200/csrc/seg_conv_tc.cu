@@ -786,8 +786,7 @@ int conv_fwd(const seg_conv_desc* d, const void* x, const void* w, void* y, int 
   p.stat_ticket = stat_ticket;
   if (sync && stats) {
     SEG_REQUIRE(stat_ticket != nullptr, "conv fwd: SyncBN needs a zeroed ticket word");
-    SEG_REQUIRE(4 * d->K <= sync->n_max, "conv fwd: 2*K = %d fp64 statistics exceed the SyncBN buffer (%d floats)", 2 * d->K, sync->n_max);
-    p.sync = *sync;
+    p.sync = *sync;  // checked by seg_conv2d_fwd (sync_check_desc)
   }
   const int bn = pick_bn(d->K, y_dtype != SEG_DT_BF16);
   p.stat_rows = stat_rows_for(d->K);

@@ -269,7 +269,8 @@ static int dw_check(const seg_conv_desc* d, const void* xs, const void* ys) {
 int seg_dwconv3x3_fwd(const seg_conv_desc* d, const void* x, const float* w9, void* y, double* stats,
                       const seg_sync_desc* sync, void* sync_ticket, void* stream) {
   if (dw_check(d, x, y)) return 1;
-  SEG_REQUIRE(!sync || (stats && sync_ticket && 4 * d->C <= sync->n_max), "dwconv fwd: SyncBN needs stats, a zeroed ticket and 4*C <= n_max");
+  SEG_REQUIRE(!sync || (stats && sync_ticket), "dwconv fwd: SyncBN needs stats and a zeroed ticket word");
+  if (sync && sync_check_desc(sync, 4ll * d->C, "dwconv fwd")) return 1;  // 2C fp64 statistics
   const int64_t M = (int64_t)d->N * d->P * d->Q;
   dwconv_fwd_kernel<<<dw_grid(M, d->C), 256, 0, ST(stream)>>>(CBF(x), d->ldx, w9, BF(y), d->ldy, d->N, d->H, d->W, d->C, d->P, d->Q,
                                                               d->stride, d->pad, d->dil, stats, sync ? *sync : SyncDesc{},

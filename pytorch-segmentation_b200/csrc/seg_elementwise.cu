@@ -1590,7 +1590,8 @@ namespace seg {
 int bn_stats_launch(const void* x, int64_t M, int C, int ldx, double* stats, const seg_sync_desc* sync, unsigned* ticket,
                     cudaStream_t stream) {
   SEG_REQUIRE(C % 8 == 0 && ldx % 8 == 0, "bn_stats: C/ldx must be multiples of 8 (C=%d ldx=%d)", C, ldx);
-  SEG_REQUIRE(!sync || (ticket && 4 * C <= sync->n_max), "bn_stats: SyncBN needs a zeroed ticket and 4*C <= n_max (fp64 totals)");
+  SEG_REQUIRE(!sync || ticket, "bn_stats: SyncBN needs a zeroed ticket word");
+  if (sync && sync_check_desc(sync, 4ll * C, "bn_stats")) return 1;  // 2C fp64 totals
   bn_stats_kernel<<<colreduce_grid(M, C), 256, 0, stream>>>(CBF(x), M, C, ldx, stats, to_sync(sync), ticket);
   return check_launch("bn_stats");
 }
@@ -1645,7 +1646,7 @@ int seg_bn_bwd_reduce(const void* dout, int lddo, const void* out, int ldo, cons
   SEG_REQUIRE(ms != MaskSrc::RECOMPUTE || (gamma && beta && drop_p == 0.f), "bn_bwd_reduce: out == NULL (mask recomputed from x) needs gamma, beta and no dropout");
   SEG_REQUIRE(relu || drop_p == 0.f, "bn_bwd_reduce: dropout (drop_p > 0) needs relu: the keep mask is read from out > 0");
   SEG_REQUIRE(acc && ticket, "bn_bwd_reduce: zeroed fp64 accumulators [seg_bn_bwd_reduce_slots()][2C] and ticket word required");
-  SEG_REQUIRE(!sync || 2 * C <= sync->n_max, "bn_bwd_reduce: 2*C exceeds the SyncBN buffer");
+  if (sync && sync_check_desc(sync, 2ll * C, "bn_bwd_reduce")) return 1;
   const dim3 grid = reduce2_grid(M, C);
   launch_pdl(by_mask_src(ms, bn_bwd_reduce_kernel<MaskSrc::ACT>, bn_bwd_reduce_kernel<MaskSrc::RECOMPUTE>,
                          bn_bwd_reduce_kernel<MaskSrc::BITS>),
@@ -1724,7 +1725,7 @@ int seg_bn_bwd_fused(const void* dout, int lddo, const void* out, int ldo, const
   p.dgamma = dgamma; p.dbeta = dbeta; p.accumulate = accumulate; p.zero_sums = zero_sums;
   p.dx = BF(dx); p.dres = BF(dres); p.lddx = lddx; p.lddres = lddres; p.beta_res = beta_res;
   if (sync) {
-    SEG_REQUIRE(2 * C <= sync->n_max, "bn_bwd_fused: 2*C = %d sums exceed the SyncBN buffer (%d floats)", 2 * C, sync->n_max);
+    if (sync_check_desc(sync, 2ll * C, "bn_bwd_fused")) return 1;
     p.sync = *sync;
   }
   // multi-GPU: leave one block slot per SM free — a concurrently running NCCL kernel (bucketed gradient all-reduce on the side

@@ -23,7 +23,7 @@
 #pragma once
 #include <stdint.h>
 #include <stdio.h>
-#include "../../include/seg_b200.h"
+#include "seg_common.cuh"
 
 namespace seg {
 
@@ -37,6 +37,26 @@ __host__ __device__ inline size_t sync_flags_offset(int world, int n_max) {
 __host__ __device__ inline size_t sync_seq_offset(int world, int n_max) {
   size_t b = sync_flags_offset(world, n_max) + (size_t)2 * world * sizeof(uint32_t);
   return (b + 127) & ~(size_t)127;
+}
+
+// Host check of the descriptor every entry point that runs the exchange makes before it launches anything (the kernels
+// copy it by value and trust it).  The handle is read on the host: a device address (such as the peer-pointer array
+// itself) is refused, not dereferenced.  n_max must be even: the fp64 forward statistics address slot
+// (parity * world + p) * n_max FLOATS as doubles, so an odd n_max misaligns every other rank's slot and the second parity.
+// `need`: floats of one rank's vector in its slot (4C for the fp64 statistics, 2C for the fp32 backward sums).
+inline int sync_check_desc(const seg_sync_desc* s, int64_t need, const char* who) {
+  cudaPointerAttributes attr;
+  const bool host_handle = s != nullptr && cudaPointerGetAttributes(&attr, s) == cudaSuccess && attr.type != cudaMemoryTypeDevice;
+  if (!host_handle) cudaGetLastError();  // a failed query must not surface at the next launch check
+  SEG_REQUIRE(host_handle, "%s: `sync` must point to a seg_sync_desc in host memory", who);
+  SEG_REQUIRE(s->peers != nullptr, "%s: SyncBN descriptor: peers is NULL", who);
+  SEG_REQUIRE(s->world >= 1 && s->world <= 64, "%s: SyncBN descriptor: world = %d outside [1, 64]", who, s->world);
+  SEG_REQUIRE(s->rank >= 0 && s->rank < s->world, "%s: SyncBN descriptor: rank = %d outside [0, world = %d)", who, s->rank,
+              s->world);
+  SEG_REQUIRE(s->n_max > 0 && s->n_max % 2 == 0, "%s: SyncBN descriptor: n_max = %d must be positive and even", who, s->n_max);
+  SEG_REQUIRE(need > 0 && need <= s->n_max, "%s: SyncBN descriptor: n_max = %d floats cannot hold the %lld of this exchange",
+              who, s->n_max, (long long)need);
+  return 0;
 }
 
 __device__ __forceinline__ void sync_st_release_sys(uint32_t* p, uint32_t v) {

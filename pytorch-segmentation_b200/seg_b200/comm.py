@@ -24,6 +24,13 @@ def _sync_timeout_clocks():
     return int(float(os.environ.get("SEG_SYNC_TIMEOUT_S", "120")) * 2e9)
 
 
+def _check_n_max(n_max):
+    """The fp64 forward statistics address each rank's slot of n_max floats as doubles: n_max must be even for every
+    slot to be 8-byte aligned (the kernels' entry points refuse an odd one too)."""
+    if not (isinstance(n_max, int) and n_max > 0 and n_max % 2 == 0):
+        raise ValueError(f"SyncBN: n_max must be a positive even number of floats, got {n_max!r}")
+
+
 def _make_desc(peers, rank, world, n_max):
     return lib.SyncDesc(peers.data_ptr(), rank, world, n_max, _sync_timeout_clocks())
 
@@ -33,6 +40,7 @@ class SyncBNGroup:
     (<= n_max floats) over all ranks in place, bit-identically on every rank."""
 
     def __init__(self, n_max=8192, group=None):
+        _check_n_max(n_max)
         self.rank = dist.get_rank(group)
         self.world = dist.get_world_size(group)
         self.n_max = n_max
@@ -82,6 +90,7 @@ class LocalLoopbackGroup:
     """world == 1 stand-in with the same interface (used by single-GPU tests of the exchange kernel)."""
 
     def __init__(self, n_max=8192):
+        _check_n_max(n_max)
         self.rank, self.world, self.n_max = 0, 1, n_max
         L = lib.load()
         mine = ctypes.c_void_p()

@@ -129,6 +129,12 @@ def _worker(rank, world, port, out_path, graph=False, nsteps=1):
         loss = st.step(x[half].cuda(), y[half].cuda())
     lt = loss.detach().clone()
     dist.all_reduce(lt)
+    # the replicas must stay bit-equal: identical world statistics and one all-reduced gradient on every rank
+    mine = torch.cat([p.detach().float().reshape(-1) for p in m.parameters()]
+                     + [b.detach().float().reshape(-1) for n, b in m.named_buffers() if "running_" in n])
+    every = [torch.empty_like(mine) for _ in range(world)]
+    dist.all_gather(every, mine)
+    replicas_equal = all(torch.equal(every[0].view(torch.int32), e.view(torch.int32)) for e in every[1:])
     if rank == 0:
         m1 = seg_b200.DeepLab(7, backbone="resnet14")
         m1.load_state_dict(sd)
@@ -141,7 +147,7 @@ def _worker(rank, world, port, out_path, graph=False, nsteps=1):
         upd1 = torch.cat([(p.detach().cpu() - sd[n]).reshape(-1) for n, p in m1.named_parameters()])
         rs2 = torch.cat([b.detach().cpu().float().reshape(-1) for n, b in m.named_buffers() if "running_" in n])
         rs1 = torch.cat([b.detach().cpu().float().reshape(-1) for n, b in m1.named_buffers() if "running_" in n])
-        torch.save({"loss2": (lt / world).item(), "loss1": loss1.item(),
+        torch.save({"loss2": (lt / world).item(), "loss1": loss1.item(), "replicas_equal": replicas_equal,
                     "cos": torch.nn.functional.cosine_similarity(upd2.double(), upd1.double(), dim=0).item(),
                     "stats_rel": ((rs2 - rs1).abs().max() / rs1.abs().max()).item()}, out_path)
     st.release_graph()
@@ -156,6 +162,7 @@ def test_two_gpu_syncbn_train_step_equals_single_gpu_on_concatenated_batch(tmp_p
     mp.spawn(_worker, args=(2, 29600 + os.getpid() % 1000, out), nprocs=2, join=True)
     r = torch.load(out)
     print(r)
+    assert r["replicas_equal"], "rank 1's parameters / running statistics differ from rank 0's"
     assert abs(r["loss2"] - r["loss1"]) < 2e-2 * abs(r["loss1"])
     assert r["stats_rel"] < 2e-2
     assert r["cos"] > 0.95
@@ -171,6 +178,7 @@ def test_two_gpu_graph_captured_steps_equal_single_gpu_eager_steps(tmp_path):
     mp.spawn(_worker, args=(2, 29600 + (os.getpid() + 7) % 1000, out, True, 3), nprocs=2, join=True)
     r = torch.load(out)
     print(r)
+    assert r["replicas_equal"], "rank 1's parameters / running statistics differ from rank 0's"
     assert abs(r["loss2"] - r["loss1"]) < 3e-2 * abs(r["loss1"])
     assert r["stats_rel"] < 3e-2
     assert r["cos"] > 0.9
