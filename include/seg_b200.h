@@ -223,6 +223,13 @@ int seg_maxpool2x2_bwd(const void* dy, const uint8_t* code, void* dx, int N, int
 int seg_maxunpool2x2_fwd(const void* x, const uint8_t* code, void* y, int N, int H, int W, int C, void* stream);
 /* dx[N,P,Q,C] = dy[N,H,W,C] gathered at the coded positions */
 int seg_maxunpool2x2_bwd(const void* dy, const uint8_t* code, void* dx, int N, int H, int W, int C, void* stream);
+/* F.relu followed by nn.MaxPool2d(2, 2, ceil_mode=True) (FCN8's VGG trunk, fcn.py:20-22), over the raw conv output x[N,H,W,C]
+ * (H, W >= 1): y[N,P,Q,C] = relu(window max), P = ceil(H/2), Q = ceil(W/2); the last windows of an odd H / W hold 1 or 2
+ * elements.  code (uint8, y's shape) = 2r + s by ATen's rule where the window max is > 0 or NaN (there it equals the index
+ * ATen's pool of relu(x) picks); a window whose max is <= 0 gets 4 + (2r + s).  C % 8 == 0, dense NHWC. */
+int seg_relu_maxpool2x2_ceil_fwd(const void* x, void* y, uint8_t* code, int N, int H, int W, int C, void* stream);
+/* dx[N,H,W,C] = dy at the coded position of windows whose max was > 0 or NaN, 0 everywhere else (relu + pool autograd) */
+int seg_relu_maxpool2x2_ceil_bwd(const void* dy, const uint8_t* code, void* dx, int N, int H, int W, int C, void* stream);
 /* nn.AdaptiveAvgPool2d(bins) (deeplabv3_plus.py:274 bins=1; pspnet.py:26 bins 1,2,3,6): y[N,b,b,C] bf16 */
 int seg_adaptive_avgpool_fwd(const void* x, int ldx, void* y, int N, int H, int W, int C, int bins, void* stream);
 /* dx = beta*dx + scatter(dy) */
@@ -360,6 +367,33 @@ int seg_eval_metrics_nchw(const float* logits, const int64_t* target, int N, int
 int seg_relu_fwd(const void* x, int ldx, void* y, int ldy, int64_t M, int C, void* stream);
 int seg_relu_bwd(const void* dy, int lddy, const void* y, int ldy, void* dx, int lddx, int64_t M, int C, float beta,
                  void* stream);
+/* F.relu + nn.Dropout(drop_p) in training (FCN8's conv6 / conv7, fcn.py:49-51): y = relu(x) * keep / (1 - drop_p) with keep =
+ * hash_uniform(seed + step_ctr * golden, row * C + c) >= drop_p (bn_apply's stream; step_ctr: device counter or NULL).
+ * drop_p = 0 is F.relu.  Backward: dx = beta*dx + (y > 0 ? dy / (1 - drop_p) : 0).  C and pitches % 8 == 0. */
+int seg_relu_dropout_fwd(const void* x, int ldx, void* y, int ldy, int64_t M, int C, float drop_p, uint64_t seed,
+                         const uint64_t* step_ctr, void* stream);
+int seg_relu_dropout_bwd(const void* dy, int lddy, const void* y, int ldy, void* dx, int lddx, int64_t M, int C, float drop_p,
+                         float beta, void* stream);
+/* ---- class-map transposed convolution (FCN8's frozen score upsamplers, fcn.py:57-97) ----
+ * ConvTranspose2d(C, C, k = 2s, stride s, padding 0, no bias) of x[N,h,w,C] (bf16, pitch ldx) -> a [N,(h+1)s,(w+1)s,C] map of
+ * which only the window rows [y0, y0+Ho) x cols [x0, x0+Wo) are computed.  1 <= C <= 160, 1 <= s <= 8.  Tensor cores
+ * (mma.sync bf16, fp32 accumulation); no atomics: every output element is one thread's fixed-order sum.  Only the C class
+ * lanes of pitched operands are read or written.  bf16 operand pitches must be even and their base addresses 4-byte aligned.
+ * seg_score_pack: weight w[C][C][k][k] (fp32, any dense values) -> the kernels' bf16 operand (packed_elems bf16 elements);
+ * bwd = 0 packs the forward's four-tap parity-class GEMMs, 1 the data gradient's. */
+int64_t seg_score_packed_elems(int C, int s);
+int seg_score_pack(const float* w, void* packed, int C, int s, int bwd, void* stream);
+/* y[n,i,j,c] = convT(x)[n, y0+i, x0+j, c] (+ alpha * skip[n, sy0+i, sx0+j, c] + bias[c] when skip is non-NULL; bias may be
+ * NULL).  y_dtype SEG_DT_BF16 / SEG_DT_F32, pitch ldy. */
+int seg_score_upsample_fwd(const void* x, int ldx, int N, int h, int w, int C, int s, const void* packed, void* y, int ldy,
+                           int y_dtype, int y0, int x0, int Ho, int Wo, const void* skip, int lds, int Hs, int Ws, int sy0, int sx0,
+                           float alpha, const float* bias, void* stream);
+/* dx[N,h,w,C] (bf16, pitch ldx, written) = the data gradient of the windowed forward for dy[N,Ho,Wo,C] (bf16, pitch lddy) */
+int seg_score_upsample_bwd(const void* dy, int lddy, int N, int h, int w, int C, int s, const void* packed_bwd, void* dx, int ldx,
+                           int y0, int x0, int Ho, int Wo, void* stream);
+/* dskip[N,Hs,Ws,C] (bf16, pitch ldd) = alpha * dy[n, a-sy0, b-sx0, c] inside the window, 0 elsewhere (the skip's gradient) */
+int seg_score_skip_bwd(const void* dy, int lddy, int Ho, int Wo, void* dskip, int ldd, int N, int Hs, int Ws, int C, int sy0,
+                       int sx0, float alpha, void* stream);
 int seg_nhwc_to_nchw_f32(const void* x, int ldx, int x_dtype, float* y, int N, int H, int W, int C, void* stream);
 /* y[M][ldy] (bf16) = beta*y + x[M][ldx] (bf16) */
 int seg_axpby_bf16(const void* x, int ldx, void* y, int ldy, int64_t M, int C, float beta, void* stream);

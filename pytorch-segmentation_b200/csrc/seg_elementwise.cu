@@ -903,6 +903,12 @@ __device__ __forceinline__ float bf16_bits_to_float(unsigned short b) { return _
 
 // ATen's rule (max_pool2d_with_indices): scan the window in row-major order from -inf, take v > best || isnan(v); the
 // index starts at the window's first element.  Starting from that element instead gives the same value and index.
+// CEIL_RELU (FCN8's VGG trunk: conv -> ReLU -> MaxPool2d(2, 2, ceil_mode=True), fcn.py:20-22): P = ceil(H/2), Q = ceil(W/2),
+// the last row / column windows of an odd H / W hold only their in-range elements, and the output is relu(window max).  The
+// window max is > 0 or NaN exactly when the pool of the ReLU'd map picks a positive / NaN element, and then both rules pick
+// the same element, so the code is ATen's on relu(x) there.  A window whose max is <= 0 pools to 0 and gets code bit 2 (4 +
+// its raw 2r + s): the ReLU's backward zeroes its gradient, and the scatter, which matches codes 0-3 only, writes 0 for it.
+template <bool CEIL_RELU>
 __global__ void __launch_bounds__(256) maxpool2x2_fwd_kernel(const uint4* __restrict__ x, uint4* __restrict__ y,
                                                              uint2* __restrict__ code, int N, int H, int W, int G, int P, int Q) {
   const int64_t total = (int64_t)N * P * Q * G;
@@ -914,11 +920,13 @@ __global__ void __launch_bounds__(256) maxpool2x2_fwd_kernel(const uint4* __rest
     const int p = (int)(t % P);
     const int n = (int)(t / P);
     const int64_t b = (((int64_t)n * H + 2 * p) * W + 2 * q) * G + g;
+    const bool s1 = !CEIL_RELU || 2 * q + 1 < W, r1 = !CEIL_RELU || 2 * p + 1 < H;
+    const bool valid[4] = {true, s1, r1, r1 && s1};
     Raw8 v[4], o;
     v[0].u = x[b];
-    v[1].u = x[b + G];
-    v[2].u = x[b + (int64_t)W * G];
-    v[3].u = x[b + (int64_t)W * G + G];
+    v[1].u = s1 ? x[b + G] : v[0].u;
+    v[2].u = r1 ? x[b + (int64_t)W * G] : v[0].u;
+    v[3].u = (r1 && s1) ? x[b + (int64_t)W * G + G] : v[0].u;
     uint32_t lo = 0, hi = 0;
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
@@ -928,11 +936,15 @@ __global__ void __launch_bounds__(256) maxpool2x2_fwd_kernel(const uint4* __rest
 #pragma unroll
       for (int k = 1; k < 4; ++k) {
         const float f = bf16_bits_to_float(v[k].h[j]);
-        if (f > best || isnan(f)) {
+        if (valid[k] && (f > best || isnan(f))) {
           best = f;
           bits = v[k].h[j];
           c = k;
         }
+      }
+      if (CEIL_RELU && !(best > 0.f) && !isnan(best)) {
+        bits = 0;
+        c |= 4u;
       }
       o.h[j] = bits;
       if (j < 4) lo |= c << (8 * j);
@@ -1437,6 +1449,51 @@ __global__ void axpby_kernel(const __nv_bfloat16* __restrict__ x, int ldx, __nv_
   }
 }
 
+// ReLU + nn.Dropout(p) (FCN8's conv6 / conv7, fcn.py:49-51): the element index r * C + c and the seed (+ the device step
+// counter) feed hash_uniform exactly as in bn_apply's dropout, so graph replays draw fresh masks.  The backward reads the
+// keep mask from out > 0 (a kept element of a positive input is positive, a dropped or ReLU'd one is 0).
+__global__ void relu_dropout_fwd_kernel(const __nv_bfloat16* __restrict__ x, int ldx, __nv_bfloat16* __restrict__ y, int ldy,
+                                        int64_t M, int C, float drop_p, uint64_t seed, const uint64_t* __restrict__ step_ctr) {
+  if (step_ctr) seed += (*step_ctr) * 0x9E3779B97F4A7C15ull;
+  const float keep_scale = drop_p > 0.f ? 1.f / (1.f - drop_p) : 1.f;
+  const int G = C >> 3;
+  const int64_t total = M * G;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int g = (int)(i % G);
+    const int64_t row = i / G;
+    float a[8];
+    unpack8(*reinterpret_cast<const bf16x8*>(x + row * ldx + g * 8), a);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      a[k] = fmaxf(a[k], 0.f);
+      if (drop_p > 0.f) a[k] = hash_uniform(seed, (uint64_t)(row * C + g * 8 + k)) >= drop_p ? a[k] * keep_scale : 0.f;
+    }
+    *reinterpret_cast<bf16x8*>(y + row * ldy + g * 8) = pack8(a);
+  }
+}
+__global__ void relu_dropout_bwd_kernel(const __nv_bfloat16* __restrict__ dy, int lddy, const __nv_bfloat16* __restrict__ y, int ldy,
+                                        __nv_bfloat16* __restrict__ dx, int lddx, int64_t M, int C, float drop_p, float beta) {
+  const float keep_scale = drop_p > 0.f ? 1.f / (1.f - drop_p) : 1.f;
+  const int G = C >> 3;
+  const int64_t total = M * G;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int g = (int)(i % G);
+    const int64_t row = i / G;
+    float d[8], o[8];
+    unpack8(*reinterpret_cast<const bf16x8*>(dy + row * lddy + g * 8), d);
+    unpack8(*reinterpret_cast<const bf16x8*>(y + row * ldy + g * 8), o);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) d[k] = o[k] > 0.f ? d[k] * keep_scale : 0.f;
+    if (beta != 0.f) {
+      float b[8];
+      unpack8(*reinterpret_cast<const bf16x8*>(dx + row * lddx + g * 8), b);
+#pragma unroll
+      for (int k = 0; k < 8; ++k) d[k] += beta * b[k];
+    }
+    *reinterpret_cast<bf16x8*>(dx + row * lddx + g * 8) = pack8(d);
+  }
+}
+
 __global__ void counter_add_kernel(uint64_t* ctr, uint64_t inc) {
   if (threadIdx.x == 0 && blockIdx.x == 0) *ctr += inc;
 }
@@ -1754,8 +1811,9 @@ int seg_maxpool3x3s2_bwd(const void* dy, const uint8_t* idx, void* dx, int N, in
   return check_launch("maxpool_bwd");
 }
 
-static int check_pool2x2(const char* what, const void* a, const void* b, const void* code, int N, int H, int W, int C) {
-  SEG_REQUIRE(N > 0 && H >= 2 && W >= 2, "%s: needs N >= 1 and H, W >= 2 (got %d x %d x %d)", what, N, H, W);
+static int check_pool2x2(const char* what, const void* a, const void* b, const void* code, int N, int H, int W, int C,
+                         int min_hw = 2) {
+  SEG_REQUIRE(N > 0 && H >= min_hw && W >= min_hw, "%s: needs N >= 1 and H, W >= %d (got %d x %d x %d)", what, min_hw, N, H, W);
   SEG_REQUIRE(C > 0 && C % 8 == 0, "%s: C = %d is not a positive multiple of 8", what, C);
   SEG_REQUIRE(((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b)) & 15) == 0 &&
                   (reinterpret_cast<uintptr_t>(code) & 7) == 0,
@@ -1765,7 +1823,7 @@ static int check_pool2x2(const char* what, const void* a, const void* b, const v
 int seg_maxpool2x2_fwd(const void* x, void* y, uint8_t* code, int N, int H, int W, int C, void* stream) {
   if (check_pool2x2("maxpool2x2_fwd", x, y, code, N, H, W, C)) return 1;
   const int P = H / 2, Q = W / 2;
-  maxpool2x2_fwd_kernel<<<grid_for((int64_t)N * P * Q * (C / 8), 256), 256, 0, ST(stream)>>>(
+  maxpool2x2_fwd_kernel<false><<<grid_for((int64_t)N * P * Q * (C / 8), 256), 256, 0, ST(stream)>>>(
       reinterpret_cast<const uint4*>(x), reinterpret_cast<uint4*>(y), reinterpret_cast<uint2*>(code), N, H, W, C / 8, P, Q);
   return check_launch("maxpool2x2_fwd");
 }
@@ -1789,6 +1847,21 @@ int seg_maxunpool2x2_bwd(const void* dy, const uint8_t* code, void* dx, int N, i
   unpool2x2_gather_kernel<<<grid_for((int64_t)N * P * Q * (C / 8), 256), 256, 0, ST(stream)>>>(
       reinterpret_cast<const uint4*>(dy), reinterpret_cast<const uint2*>(code), reinterpret_cast<uint4*>(dx), N, H, W, C / 8, P, Q);
   return check_launch("maxunpool2x2_bwd");
+}
+int seg_relu_maxpool2x2_ceil_fwd(const void* x, void* y, uint8_t* code, int N, int H, int W, int C, void* stream) {
+  if (check_pool2x2("relu_maxpool2x2_ceil_fwd", x, y, code, N, H, W, C, 1)) return 1;
+  const int P = (H + 1) / 2, Q = (W + 1) / 2;
+  maxpool2x2_fwd_kernel<true><<<grid_for((int64_t)N * P * Q * (C / 8), 256), 256, 0, ST(stream)>>>(
+      reinterpret_cast<const uint4*>(x), reinterpret_cast<uint4*>(y), reinterpret_cast<uint2*>(code), N, H, W, C / 8, P, Q);
+  return check_launch("relu_maxpool2x2_ceil_fwd");
+}
+int seg_relu_maxpool2x2_ceil_bwd(const void* dy, const uint8_t* code, void* dx, int N, int H, int W, int C, void* stream) {
+  if (check_pool2x2("relu_maxpool2x2_ceil_bwd", dy, dx, code, N, H, W, C, 1)) return 1;
+  // the floor-mode scatter with every window read: codes 4-7 (max <= 0) match no position, so the whole window gets 0
+  unpool2x2_scatter_kernel<<<grid_for((int64_t)N * ((H + 1) / 2) * ((W + 1) / 2) * (C / 8), 256), 256, 0, ST(stream)>>>(
+      reinterpret_cast<const uint4*>(dy), reinterpret_cast<const uint2*>(code), reinterpret_cast<uint4*>(dx), N, H, W, C / 8,
+      (H + 1) / 2, (W + 1) / 2);
+  return check_launch("relu_maxpool2x2_ceil_bwd");
 }
 int seg_adaptive_avgpool_fwd(const void* x, int ldx, void* y, int N, int H, int W, int C, int bins, void* stream) {
   SEG_REQUIRE(C % 8 == 0 && ldx % 8 == 0, "avgpool: alignment");
@@ -1878,6 +1951,21 @@ int seg_relu_fwd(const void* x, int ldx, void* y, int ldy, int64_t M, int C, voi
   SEG_REQUIRE(C % 8 == 0 && ldx % 8 == 0 && ldy % 8 == 0, "relu: alignment");
   relu_fwd_kernel<<<grid_for(M * (C / 8), 256), 256, 0, ST(stream)>>>(CBF(x), ldx, BF(y), ldy, M, C);
   return check_launch("relu_fwd");
+}
+int seg_relu_dropout_fwd(const void* x, int ldx, void* y, int ldy, int64_t M, int C, float drop_p, uint64_t seed,
+                         const uint64_t* step_ctr, void* stream) {
+  SEG_REQUIRE(C % 8 == 0 && ldx % 8 == 0 && ldy % 8 == 0, "relu_dropout_fwd: C and pitches must be multiples of 8");
+  SEG_REQUIRE(drop_p >= 0.f && drop_p < 1.f, "relu_dropout_fwd: drop_p = %g is not in [0, 1)", (double)drop_p);
+  relu_dropout_fwd_kernel<<<grid_for(M * (C / 8), 256), 256, 0, ST(stream)>>>(CBF(x), ldx, BF(y), ldy, M, C, drop_p, seed, step_ctr);
+  return check_launch("relu_dropout_fwd");
+}
+int seg_relu_dropout_bwd(const void* dy, int lddy, const void* y, int ldy, void* dx, int lddx, int64_t M, int C, float drop_p,
+                         float beta, void* stream) {
+  SEG_REQUIRE(C % 8 == 0 && lddy % 8 == 0 && ldy % 8 == 0 && lddx % 8 == 0, "relu_dropout_bwd: C and pitches must be multiples of 8");
+  SEG_REQUIRE(drop_p >= 0.f && drop_p < 1.f, "relu_dropout_bwd: drop_p = %g is not in [0, 1)", (double)drop_p);
+  relu_dropout_bwd_kernel<<<grid_for(M * (C / 8), 256), 256, 0, ST(stream)>>>(CBF(dy), lddy, CBF(y), ldy, BF(dx), lddx, M, C, drop_p,
+                                                                           beta);
+  return check_launch("relu_dropout_bwd");
 }
 int seg_relu_bwd(const void* dy, int lddy, const void* y, int ldy, void* dx, int lddx, int64_t M, int C, float beta,
                  void* stream) {

@@ -13,6 +13,7 @@ _LAZY = {
     "DeepLab_DUC_HDC": ("nets", "DeepLab_DUC_HDC"),
     "UNetResnet": ("nets", "UNetResnet"),
     "SegNet": ("nets", "SegNet"),
+    "FCN8": ("nets", "FCN8"),
     "CrossEntropyLoss2d": ("losses", "CrossEntropyLoss2d"),
     "DiceLoss": ("losses", "DiceLoss"),
     "FocalLoss": ("losses", "FocalLoss"),

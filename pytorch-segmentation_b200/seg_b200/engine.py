@@ -208,12 +208,13 @@ class Tape:
         self.back = []
 
     # ------------------------------------------------------------------ conv
-    def conv(self, x, spec, out=None, out_dtype=None, want_stats=False):
-        """x: Act (NHWC bf16) — or, for an explicit-im2col conv, a raw NCHW fp32 tensor (the network input)."""
+    def conv(self, x, spec, out=None, out_dtype=None, want_stats=False, use_bias=True):
+        """x: Act (NHWC bf16) — or, for an explicit-im2col conv, a raw NCHW fp32 tensor (the network input).  use_bias=False
+        leaves the module's bias out of the epilogue and its gradient (a consumer applies it: `score_upsample`)."""
         wp = self.packed_override.get(spec)
         if wp is None:
             wp = spec.packed()
-        bias = spec.m.bias
+        bias = spec.m.bias if use_bias else None
         stats = None
         if out_dtype is None:
             out_dtype = ACT_DTYPE
@@ -505,6 +506,80 @@ class Tape:
             self.back.append(bwd)
         return ya
 
+    def relu_maxpool_ceil(self, x):
+        """F.relu then nn.MaxPool2d(2, 2, ceil_mode=True) of the raw conv output x (FCN8's VGG stages, fcn.py:20-22), one
+        kernel each way; the backward writes every element of x's gradient.  x must be the pool's only consumer."""
+        y, code = ops.relu_maxpool2x2_ceil_fwd(x.t)
+        ya = Act(y)
+        if self.record:
+            def bwd():
+                if ya.grad is None or not x.needs_grad:
+                    return
+                assert x.grad is None, "relu_maxpool_ceil input must have a single consumer"
+                x.grad = ops.relu_maxpool2x2_ceil_bwd(ya.grad, code, tuple(x.t.shape))
+                x._written = True
+                ya.grad = None
+            self.back.append(bwd)
+        return ya
+
+    def relu_dropout(self, x, drop_p):
+        """F.relu then nn.Dropout(drop_p) (FCN8's conv6 / conv7, fcn.py:49-51); a plain ReLU outside training or with the
+        engine's dropout off.  Masks: bn_act's seed sequence and the device step counter."""
+        if not (self.training and self.dropout):
+            drop_p = 0.0
+        seed = 0
+        if drop_p > 0.0:
+            self._drop_ctr += 1
+            seed = (self.seed * 1000003 + self._drop_ctr * 7919) & 0x7FFFFFFFFFFFFFFF
+        y = ops.relu_dropout_fwd(x.t, drop_p, seed, self.step_ctr if drop_p > 0.0 else None)
+        ya = Act(y)
+        if self.record:
+            def bwd():
+                if ya.grad is None or not x.needs_grad:
+                    return
+                gx, beta = x.grad_target()
+                ops.relu_dropout_bwd(ya.grad, y, drop_p, gx, beta)
+                ya.grad = None
+            self.back.append(bwd)
+        return ya
+
+    def score_upsample(self, x, up, window, skip=None, skip_off=(0, 0), alpha=0.0, bias=None, out_dtype=None):
+        """Window (y0, x0, Ho, Wo) of the frozen nn.ConvTranspose2d `up` (C -> C, k = 2s, stride s, no padding) over the class
+        map x, plus alpha * skip[window at skip_off] + bias when a skip is given — FCN8's `adj_poolN(alpha * poolN)[crop] +
+        up(...)` (fcn.py:86-97) with the adj conv run by `conv(..., use_bias=False)` into `skip`.  One launch each way; the
+        backward writes x's gradient, the skip's (alpha * dY in the window, 0 elsewhere) and adds the bias gradient (column
+        sums of dY).  x and skip must have no other consumer.  `up` gets no gradient: a trainable weight raises."""
+        if up.weight.requires_grad:
+            raise NotImplementedError("score_upsample: the engine computes no gradient for the upsampling weight; keep it frozen "
+                                      "(requires_grad=False), as models/fcn.py does")
+        k = up.kernel_size[0]
+        wf = ops.score_pack(up.weight, bwd=False)
+        wb = ops.score_pack(up.weight, bwd=True) if self.record else None
+        y = ops.score_upsample_fwd(x.t, wf, k, window, skip=skip.t if skip is not None else None, skip_off=skip_off, alpha=alpha,
+                                   bias=bias.detach() if bias is not None else None, out_dtype=out_dtype or ACT_DTYPE)
+        ya = Act(y)
+        if self.record:
+            def bwd():
+                dy = ya.grad
+                if dy is None:
+                    return
+                if bias is not None and bias.requires_grad:
+                    C = dy.shape[-1]
+                    wide = dy if C % 8 == 0 else dy.as_strided(dy.shape[:-1] + (ops.ld(dy),), dy.stride(), dy.storage_offset())
+                    s = ops.bn_stats(wide)[:C].float()  # column sums of dY (fp64 accumulation), as Tape.conv's bias gradient
+                    self._param_grad(bias, lambda g, beta: g.add_(s) if beta else g.copy_(s))
+                if skip is not None and skip.needs_grad:
+                    assert skip.grad is None, "score_upsample skip must have a single consumer"
+                    skip.grad = ops.score_skip_bwd(dy, tuple(skip.t.shape), skip_off, alpha)
+                    skip._written = True
+                if x.needs_grad:
+                    assert x.grad is None, "score_upsample input must have a single consumer"
+                    x.grad = ops.score_upsample_bwd(dy, wb, tuple(x.t.shape), k, window)
+                    x._written = True
+                ya.grad = None
+            self._push_back(bwd, (bias,))
+        return ya
+
     def avgpool(self, x, bins):
         y = ops.adaptive_avgpool_fwd(x.t, bins)
         ya = Act(y)
@@ -593,6 +668,11 @@ class Tape:
             slices.append(buf[..., off:off + c])
             off += c
         return whole, slices
+
+    def pitched(self, N, H, W, C, device):
+        """Activation buffer [N,H,W,C] with channel pitch ceil8(C), for class maps (C = the class count): the kernels that
+        produce and consume them touch the C class lanes only."""
+        return torch.empty((N, H, W, (C + 7) // 8 * 8), dtype=ACT_DTYPE, device=device)[..., :C]
 
     def bind_slices(self, whole, acts):
         """After the producers ran: make each producer Act's gradient a view of the concat gradient buffer."""

@@ -81,6 +81,8 @@ _SIGS = {
     "seg_maxpool2x2_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "seg_maxunpool2x2_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "seg_maxunpool2x2_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "seg_relu_maxpool2x2_ceil_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "seg_relu_maxpool2x2_ceil_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "seg_adaptive_avgpool_fwd": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "seg_adaptive_avgpool_bwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "seg_bilinear_fwd": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
@@ -108,6 +110,16 @@ _SIGS = {
     "seg_upsample_loss_bwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int64, c_void_p, c_int, c_float, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
     "seg_relu_fwd": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int64, c_int, c_void_p]),
     "seg_relu_bwd": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int64, c_int, c_float, c_void_p]),
+    "seg_relu_dropout_fwd": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int64, c_int, c_float, c_uint64, c_void_p, c_void_p]),
+    "seg_relu_dropout_bwd": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int64, c_int, c_float, c_float, c_void_p]),
+    "seg_score_packed_elems": (c_int64, [c_int, c_int]),
+    "seg_score_pack": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "seg_score_upsample_fwd": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
+                                       c_int, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p]),
+    "seg_score_upsample_bwd": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
+                                       c_int, c_void_p]),
+    "seg_score_skip_bwd": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float,
+                                   c_void_p]),
     "seg_nhwc_to_nchw_f32": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "seg_axpby_bf16": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int64, c_int, c_float, c_void_p]),
     "seg_comm_buffer_bytes": (ctypes.c_size_t, [c_int, c_int]),

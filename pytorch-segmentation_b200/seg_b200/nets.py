@@ -6,6 +6,7 @@
     DeepLab_DUC_HDC(num_classes, in_channels=3, pretrained=None, output_stride=8, freeze_bn=False, **_)
     UNetResnet(num_classes, in_channels=3, backbone='resnet50', pretrained=None, freeze_bn=False, **_)
     SegNet(num_classes, in_channels=3, pretrained=None, freeze_bn=False, freeze_backbone=False, **_)
+    FCN8(num_classes, pretrained=None, freeze_bn=False, freeze_backbone=False, **_)
 
 (default backbones are the reference's; `pretrained`: the reference defaults to True and downloads ImageNet weights — there is
 no network here, so an explicit True raises and the default (None) initialises randomly with a logged warning)
@@ -1274,3 +1275,132 @@ class SegNet(_EngineModel):
 
     def get_decoder_params(self):
         return self.parameters()
+
+
+# ----------------------------------------------------------------------------------------------- FCN8
+def upsampling_weight(in_channels, out_channels, kernel_size):
+    """The bilinear ConvTranspose2d init of utils/helpers.py:get_upsampling_weight: the separable tent filter on the channel
+    diagonal, zeros elsewhere."""
+    factor = (kernel_size + 1) // 2
+    center = factor - 1 if kernel_size % 2 == 1 else factor - 0.5
+    og = np.ogrid[:kernel_size, :kernel_size]
+    filt = (1 - abs(og[0] - center) / factor) * (1 - abs(og[1] - center) / factor)
+    weight = np.zeros((in_channels, out_channels, kernel_size, kernel_size), dtype=np.float64)
+    weight[list(range(in_channels)), list(range(out_channels)), :, :] = filt
+    return torch.from_numpy(weight).float()
+
+
+class FCN8(_EngineModel):
+    """FCN-8s on a VGG16 trunk — replaces models/fcn.py:9-103 (which cannot be constructed: it reads an undefined
+    `freeze_backbone`).  pool3 / pool4 / pool5 = torchvision vgg16().features[:17] / [17:24] / [24:] with the first conv padded
+    by 100 and every MaxPool2d in ceil mode; output = conv6 (7x7, 512 -> 4096) ReLU Dropout conv7 (1x1) ReLU Dropout
+    Conv2d(4096, C, 1); adj_pool3 / adj_pool4 = 1x1 convs to C; up_output / up_pool4_out = ConvTranspose2d(C, C, 4, 2) and
+    up_final = ConvTranspose2d(C, C, 16, 8), bias-free, bilinear-initialised and frozen.
+    Forward: each conv runs on the wgmma kernels with its bias in the epilogue, the ReLU standalone or fused with the stage's
+    ceil-mode pool (`Tape.relu_maxpool_ceil`), conv6 / conv7's ReLU + Dropout in one pass.  The adj convs write W·pool
+    without their bias; each upsampler is one `Tape.score_upsample` launch over only its cropped window, adding
+    alpha * skip + bias (alpha = 0.01, 1e-4) in the same pass, so s2, s4 (bf16) and the cropped fp32 logits come out of one
+    launch each.
+    Init as the reference: torchvision's VGG init for the features (kaiming-normal fan_out, bias 0), conv6 / conv7 from
+    N(0, 0.01) Linear weights with bias 0, default init for the score and adj convs.  Parameter groups as the reference's.
+    freeze_backbone freezes pool3 / pool4 / pool5.  An input with other than 3 channels raises ValueError."""
+
+    VGG = (64, 64, "M", 128, 128, "M", 256, 256, 256, "M", 512, 512, 512, "M", 512, 512, 512, "M")
+
+    def __init__(self, num_classes, pretrained=None, freeze_bn=False, freeze_backbone=False, **_):
+        super().__init__()
+        _check_pretrained(self, pretrained)
+        self.num_classes = num_classes
+        features, cin = [], 3
+        for v in self.VGG:
+            if v == "M":
+                features.append(nn.MaxPool2d(kernel_size=2, stride=2, ceil_mode=True))
+            else:
+                features += [nn.Conv2d(cin, v, kernel_size=3, padding=1), nn.ReLU(inplace=True)]
+                cin = v
+        features[0].padding = (100, 100)
+        for m in features:  # torchvision VGG._initialize_weights
+            if isinstance(m, nn.Conv2d):
+                nn.init.kaiming_normal_(m.weight, mode="fan_out", nonlinearity="relu")
+                nn.init.constant_(m.bias, 0)
+        self.pool3 = nn.Sequential(*features[:17])
+        self.pool4 = nn.Sequential(*features[17:24])
+        self.pool5 = nn.Sequential(*features[24:])
+        self.adj_pool3 = nn.Conv2d(256, num_classes, kernel_size=1)
+        self.adj_pool4 = nn.Conv2d(512, num_classes, kernel_size=1)
+        conv6 = nn.Conv2d(512, 4096, kernel_size=7)
+        conv7 = nn.Conv2d(4096, 4096, kernel_size=1)
+        for c in (conv6, conv7):  # vgg.classifier[0] / [3]: nn.Linear with torchvision's N(0, 0.01), bias 0, reshaped
+            nn.init.normal_(c.weight, 0, 0.01)
+            nn.init.constant_(c.bias, 0)
+        self.output = nn.Sequential(conv6, nn.ReLU(inplace=True), nn.Dropout(), conv7, nn.ReLU(inplace=True), nn.Dropout(),
+                                    nn.Conv2d(4096, num_classes, kernel_size=1))
+        self.up_output = nn.ConvTranspose2d(num_classes, num_classes, kernel_size=4, stride=2, bias=False)
+        self.up_pool4_out = nn.ConvTranspose2d(num_classes, num_classes, kernel_size=4, stride=2, bias=False)
+        self.up_final = nn.ConvTranspose2d(num_classes, num_classes, kernel_size=16, stride=8, bias=False)
+        for up, k in ((self.up_output, 4), (self.up_pool4_out, 4), (self.up_final, 16)):
+            up.weight.data.copy_(upsampling_weight(num_classes, num_classes, k))
+            up.weight.requires_grad = False
+        if freeze_bn:
+            self.freeze_bn()
+        if freeze_backbone:
+            for p in chain(self.pool3.parameters(), self.pool4.parameters(), self.pool5.parameters()):
+                p.requires_grad = False
+
+    def all_conv_specs(self):
+        # the frozen upsamplers run on the score kernels, not the conv path: no packed weight or weight gradient
+        return [self._spec(n, m) for n, m in self.named_modules() if isinstance(m, nn.Conv2d)]
+
+    def _check(self, x):
+        """Before any launch: a 3-channel NCHW input, and frozen upsamplers (the engine computes no gradient for them)."""
+        if x.dim() != 4 or x.shape[1] != 3:
+            raise ValueError(f"FCN8 takes a 3-channel NCHW input (VGG16's first conv); got shape {tuple(x.shape)}")
+        for name in ("up_output", "up_pool4_out", "up_final"):
+            if getattr(self, name).weight.requires_grad:
+                raise NotImplementedError(f"FCN8.{name}: the engine computes no gradient for the upsampling weight; keep it "
+                                          "frozen (requires_grad=False), as models/fcn.py does")
+
+    def forward(self, x):
+        self._check(x)
+        return super().forward(x)
+
+    def _forward_heads(self, tape, x):
+        self._check(x)
+        N, _, H, W = x.shape
+        a, taps = x, []
+        for name in ("pool3", "pool4", "pool5"):
+            seq = getattr(self, name)
+            for j, m in enumerate(seq):
+                if isinstance(m, nn.Conv2d):
+                    y, _ = tape.conv(a, self._spec(f"{name}.{j}", m))
+                    pool_next = j + 2 < len(seq) and isinstance(seq[j + 2], nn.MaxPool2d)
+                    a = tape.relu_maxpool_ceil(y) if pool_next else tape.relu(y)
+            taps.append(a)
+        pool3, pool4, pool5 = taps
+        out, C, dev = self.output, self.num_classes, x.device
+        a = tape.relu_dropout(tape.conv(pool5, self._spec("output.0", out[0]))[0], out[2].p)
+        a = tape.relu_dropout(tape.conv(a, self._spec("output.3", out[3]))[0], out[5].p)
+        _, h, w, _ = a.t.shape
+        score, _ = tape.conv(a, self._spec("output.6", out[6]), out=tape.pitched(N, h, w, C, dev))
+        # s2 = adj_pool4(0.01 * pool4)[5:5+h2, 5:5+w2] + up_output(score)  (fcn.py:85-88)
+        skip4, _ = tape.conv(pool4, self._spec("adj_pool4", self.adj_pool4), out=tape.pitched(N, *pool4.shape[1:3], C, dev),
+                             use_bias=False)
+        h2, w2 = 2 * h + 2, 2 * w + 2
+        s2 = tape.score_upsample(score, self.up_output, (0, 0, h2, w2), skip=skip4, skip_off=(5, 5), alpha=0.01,
+                                 bias=self.adj_pool4.bias)
+        # s4 = adj_pool3(0.0001 * pool3)[9:9+h4, 9:9+w4] + up_pool4_out(s2)  (fcn.py:91-92)
+        skip3, _ = tape.conv(pool3, self._spec("adj_pool3", self.adj_pool3), out=tape.pitched(N, *pool3.shape[1:3], C, dev),
+                             use_bias=False)
+        h4, w4 = 2 * h2 + 2, 2 * w2 + 2
+        s4 = tape.score_upsample(s2, self.up_pool4_out, (0, 0, h4, w4), skip=skip3, skip_off=(9, 9), alpha=1e-4,
+                                 bias=self.adj_pool3.bias)
+        # logits = up_final(s4)[31:31+H, 31:31+W]  (fcn.py:95-96)
+        lo = tape.score_upsample(s4, self.up_final, (31, 31, H, W), out_dtype=torch.float32)
+        return [FullResHead(lo)]
+
+    def get_backbone_params(self):
+        return chain(self.pool3.parameters(), self.pool4.parameters(), self.pool5.parameters(), self.output.parameters())
+
+    def get_decoder_params(self):
+        return chain(self.up_output.parameters(), self.adj_pool4.parameters(), self.up_pool4_out.parameters(),
+                     self.adj_pool3.parameters(), self.up_final.parameters())

@@ -448,6 +448,25 @@ def maxunpool2x2_bwd(dy, code):
     return dx
 
 
+def relu_maxpool2x2_ceil_fwd(x):
+    """F.relu then nn.MaxPool2d(2, 2, ceil_mode=True) of the raw conv output x: (y [N,ceil(H/2),ceil(W/2),C] bf16, codes uint8
+    of y's shape: 2r + s, plus 4 where the window max is <= 0 and the gradient is dropped)."""
+    N, H, W, C = x.shape
+    assert x.is_contiguous()
+    y = torch.empty((N, (H + 1) // 2, (W + 1) // 2, C), dtype=torch.bfloat16, device=x.device)
+    code = torch.empty(y.shape, dtype=torch.uint8, device=x.device)
+    call("seg_relu_maxpool2x2_ceil_fwd", ptr(x), ptr(y), ptr(code), N, H, W, C)
+    return y, code
+
+
+def relu_maxpool2x2_ceil_bwd(dy, code, x_shape):
+    N, H, W, C = x_shape
+    assert dy.is_contiguous() and tuple(dy.shape) == (N, (H + 1) // 2, (W + 1) // 2, C) and code.shape == dy.shape
+    dx = torch.empty(x_shape, dtype=torch.bfloat16, device=dy.device)
+    call("seg_relu_maxpool2x2_ceil_bwd", ptr(dy), ptr(code), ptr(dx), N, H, W, C)
+    return dx
+
+
 def adaptive_avgpool_fwd(x, bins):
     N, H, W, C = x.shape
     y = torch.empty((N, bins, bins, C), dtype=torch.bfloat16, device=x.device)
@@ -746,6 +765,64 @@ def relu_fwd(x):
 def relu_bwd(dy, y, dx, beta):
     call("seg_relu_bwd", ptr(dy), ld(dy), ptr(y), ld(y), ptr(dx), ld(dx), rows(y), y.shape[-1], float(beta))
     return dx
+
+
+def relu_dropout_fwd(x, drop_p, seed=0, step_ctr=None):
+    """relu(x) then nn.Dropout(drop_p) in training (drop_p = 0: F.relu); masks from bn_apply's hash stream."""
+    y = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
+    call("seg_relu_dropout_fwd", ptr(x), ld(x), ptr(y), ld(y), rows(x), x.shape[-1], float(drop_p), int(seed), ptr(step_ctr))
+    return y
+
+
+def relu_dropout_bwd(dy, y, drop_p, dx, beta):
+    call("seg_relu_dropout_bwd", ptr(dy), ld(dy), ptr(y), ld(y), ptr(dx), ld(dx), rows(y), y.shape[-1], float(drop_p), float(beta))
+    return dx
+
+
+# ---------------------------------------------------------------- class-map transposed conv (FCN8's score upsamplers)
+def score_pack(w, bwd):
+    """ConvTranspose2d weight [C][C][k][k] (k = 2s) -> the score kernels' packed bf16 operand (forward or data gradient)."""
+    C, _, k, _ = w.shape
+    n = int(lib.load().seg_score_packed_elems(C, k // 2))
+    if n < 0:
+        raise RuntimeError(f"score kernels: C = {C}, k = {k} unsupported (1 <= C <= 160, k = 2s, s <= 8)")
+    out = torch.empty(n, dtype=torch.bfloat16, device=w.device)
+    call("seg_score_pack", ptr(w.detach().float().contiguous()), ptr(out), C, k // 2, int(bool(bwd)))
+    return out
+
+
+def score_upsample_fwd(x, packed, k, window, skip=None, skip_off=(0, 0), alpha=0.0, bias=None, out_dtype=torch.bfloat16):
+    """Window (y0, x0, Ho, Wo) of ConvTranspose2d(C, C, k, k // 2)(x), + alpha * skip[window at skip_off] + bias if skip is
+    given.  Returns [N,Ho,Wo,C] of out_dtype; a bf16 result has channel pitch ceil8(C) (pad lanes never written)."""
+    N, h, w, C = x.shape
+    y0, x0, Ho, Wo = window
+    cp = (C + 7) // 8 * 8 if out_dtype == torch.bfloat16 else C
+    y = torch.empty((N, Ho, Wo, cp), dtype=out_dtype, device=x.device)[..., :C]
+    Hs, Ws = (skip.shape[1], skip.shape[2]) if skip is not None else (0, 0)
+    call("seg_score_upsample_fwd", ptr(x), ld(x), N, h, w, C, k // 2, ptr(packed), ptr(y), ld(y),
+         DT_BF16 if out_dtype == torch.bfloat16 else DT_F32, y0, x0, Ho, Wo, ptr(skip), ld(skip) if skip is not None else 0, Hs, Ws,
+         skip_off[0], skip_off[1], float(alpha), ptr(bias))
+    return y
+
+
+def score_upsample_bwd(dy, packed_bwd, x_shape, k, window):
+    """Data gradient [N,h,w,C] bf16 (pitch ceil8(C)) of score_upsample_fwd's transposed conv for the window gradient dy."""
+    N, h, w, C = x_shape
+    y0, x0, Ho, Wo = window
+    assert tuple(dy.shape) == (N, Ho, Wo, C)
+    dx = torch.empty((N, h, w, (C + 7) // 8 * 8), dtype=torch.bfloat16, device=dy.device)[..., :C]
+    call("seg_score_upsample_bwd", ptr(dy), ld(dy), N, h, w, C, k // 2, ptr(packed_bwd), ptr(dx), ld(dx), y0, x0, Ho, Wo)
+    return dx
+
+
+def score_skip_bwd(dy, skip_shape, skip_off, alpha, out=None):
+    """Gradient of the skip map: alpha * dy placed at skip_off, 0 elsewhere (bf16 [N,Hs,Ws,C], pitch ceil8(C) unless `out`)."""
+    N, Hs, Ws, C = skip_shape
+    if out is None:
+        out = torch.empty((N, Hs, Ws, (C + 7) // 8 * 8), dtype=torch.bfloat16, device=dy.device)[..., :C]
+    call("seg_score_skip_bwd", ptr(dy), ld(dy), dy.shape[1], dy.shape[2], ptr(out), ld(out), N, Hs, Ws, C, skip_off[0], skip_off[1],
+         float(alpha))
+    return out
 
 
 def axpby(x, y, beta):
