@@ -155,11 +155,15 @@ int seg_bn_apply(const void* x, int ldx, const float* scale_shift, const void* r
  * seg_bn_finalize + seg_bn_apply in ONE launch (training mode): coefficients are derived from the batch sums inside the
  * kernel; save[2C] = (mean, 1/std) for the backward pass and the running statistics are written by one block row.
  * mask (optional, needs relu): the ReLU bit mask for the backward passes, uint8 [M][C/8] with its own pitch C/8 (independent
- * of ldo): bit j of mask[m][g] = (stored out[m][8g+j] > 0). */
+ * of ldo): bit j of mask[m][g] = (stored out[m][8g+j] > 0).
+ * growth > 0: `stats` is a dense block's statistics table and x its channel prefix [0, C): fp64 records [sum(w), sum^2(w)]
+ * back to back in channel order, the block input's (w = c0) first, then one per layer (w = growth), each written once by
+ * its producer (and, under SyncBN, exchanged there).  Channel c's sums are read from its record.  growth == 0: stats is
+ * [2C] (the launch without a table). */
 int seg_bn_apply_train(const void* x, int ldx, const double* stats, double count, const float* gamma, const float* beta,
                        float eps, float momentum, int clamp_eps, float* running_mean, float* running_var, float* save,
                        const void* res, int ldr, void* out, int ldo, uint8_t* mask, int64_t M, int C, int relu, float drop_p,
-                       uint64_t seed, const uint64_t* step_ctr, int drop_hw, void* stream);
+                       uint64_t seed, const uint64_t* step_ctr, int drop_hw, int c0, int growth, void* stream);
 /* device-side step counter (*ctr += inc): mixed into dropout seeds and SyncBN epochs so a captured CUDA graph of the
  * train step stays correct on every replay */
 int seg_counter_add(uint64_t* ctr, uint64_t inc, void* stream);
@@ -183,25 +187,26 @@ int seg_bn_bwd_reduce(const void* dout, int lddo, const void* out, int ldo, cons
                       const float* save_mean_istd, int64_t M, int C, int relu, float drop_p, float* sums, double* acc,
                       void* ticket, float* dgamma, float* dbeta, int accumulate, const float* gamma, const float* beta,
                       const seg_sync_desc* sync, void* stream);
-/* backward, pass 2: dx = gamma*istd*(dz - sums0/count - xhat*sums1/count); dres = beta_res*dres + dz (optional).
- * `sums` are the sums over `count` elements (under SyncBN the world's, from seg_bn_bwd_reduce). */
+/* backward, pass 2: dx = beta_dx*dx + gamma*istd*(dz - sums0/count - xhat*sums1/count); dres = beta_res*dres + dz (optional).
+ * `sums` are the sums over `count` elements (under SyncBN the world's, from seg_bn_bwd_reduce).  beta_dx is 0 or 1; with 1
+ * the sum is taken in fp32 and rounded to bf16 once (a pre-activation BN adding into its concat's gradient). */
 int seg_bn_bwd_apply(const void* dout, int lddo, const void* out, int ldo, const uint8_t* mask, const void* x, int ldx,
                      const float* save_mean_istd, const float* gamma, const float* sums, double count, int64_t M,
                      int C, int relu, float drop_p, void* dx, int lddx, void* dres, int lddres, float beta_res,
-                     const float* beta, void* stream);
+                     const float* beta, float beta_dx, void* stream);
 /* BatchNorm backward in ONE cooperative launch = seg_bn_bwd_reduce + (SyncBN exchange) + seg_bn_bwd_apply: partial sums per
  * block -> grid barrier -> the cross-block sum spread over all blocks in fixed order (bit-reproducible) -> grid barrier ->
  * dx / dres.  dgamma / dbeta (optional) receive the parameter gradients from the LOCAL totals.  count_total = rows summed
  * over the world.  zero_sums != 0: frozen BatchNorm (BaseModel.freeze_bn): dx = gamma*istd*dz.  sync != NULL: one block
  * exchanges the totals with the SyncBN peers inside the kernel.  sums[2C] receives the totals dx is computed from (the WORLD's
  * under SyncBN).  Workspace from seg_bn_bwd_fused_workspace: rows (uninitialised floats) and tickets (uint32, ZERO at launch).
- * The grid is sized to be co-resident. */
+ * The grid is sized to be co-resident.  beta_dx (0 or 1): as seg_bn_bwd_apply's. */
 int seg_bn_bwd_fused_workspace(int64_t M, int C, int64_t* rows_floats, int64_t* tickets);
 int seg_bn_bwd_fused(const void* dout, int lddo, const void* out, int ldo, const uint8_t* mask, const void* x, int ldx,
                      const float* save_mean_istd, const float* gamma, const float* beta, double count_total, int64_t M,
                      int C, int relu, float drop_p, float* sums, float* rows, void* tickets, float* dgamma, float* dbeta,
                      int accumulate, void* dx, int lddx, void* dres, int lddres, float beta_res, int zero_sums,
-                     const seg_sync_desc* sync, void* stream);
+                     const seg_sync_desc* sync, float beta_dx, void* stream);
 /* parameter grads from the LOCAL sums: dbeta (=|+=) sums[0:C], dgamma (=|+=) sums[C:2C] */
 int seg_bn_param_grad(const float* sums, int C, float* dgamma, float* dbeta, int accumulate, void* stream);
 
@@ -230,6 +235,11 @@ int seg_maxunpool2x2_bwd(const void* dy, const uint8_t* code, void* dx, int N, i
 int seg_relu_maxpool2x2_ceil_fwd(const void* x, void* y, uint8_t* code, int N, int H, int W, int C, void* stream);
 /* dx[N,H,W,C] = dy at the coded position of windows whose max was > 0 or NaN, 0 everywhere else (relu + pool autograd) */
 int seg_relu_maxpool2x2_ceil_bwd(const void* dy, const uint8_t* code, void* dx, int N, int H, int W, int C, void* stream);
+/* nn.AvgPool2d(2, 2), floor mode (DenseNet's transition1): y [N][H/2][W/2][C] (channel pitch ldy: may be a concat slice)
+ * = the mean of each 2x2 window, summed in fp32 and rounded once; a trailing odd row / column is dropped.  Backward:
+ * dx = beta*dx + dy/4 over every element of dx (0 for the dropped row / column). */
+int seg_avgpool2x2_fwd(const void* x, int ldx, void* y, int ldy, int N, int H, int W, int C, void* stream);
+int seg_avgpool2x2_bwd(const void* dy, int lddy, void* dx, int lddx, int N, int H, int W, int C, float beta, void* stream);
 /* nn.AdaptiveAvgPool2d(bins) (deeplabv3_plus.py:274 bins=1; pspnet.py:26 bins 1,2,3,6): y[N,b,b,C] bf16 */
 int seg_adaptive_avgpool_fwd(const void* x, int ldx, void* y, int N, int H, int W, int C, int bins, void* stream);
 /* dx = beta*dx + scatter(dy) */

@@ -293,8 +293,13 @@ struct BnTrain {
   float eps, momentum;
   int clamp_eps;
   float *running_mean, *running_var, *save;
+  // growth > 0: `stats` is a dense block's statistics table — records [sum(w), sum^2(w)] back to back in channel order,
+  // the block input's (w = c0) first, then one per layer (w = growth); channel c's sums are read from its record
+  int c0, growth;
 };
 
+// TABLE: tr.stats is a dense block's statistics table (BnTrain::c0 / growth); the launch without it compiles as before
+template <bool TABLE = false>
 __global__ void __launch_bounds__(256, 4) bn_apply_kernel(const __nv_bfloat16* __restrict__ x, int ldx,
                                                        const float* __restrict__ ss, const __nv_bfloat16* __restrict__ res,
                                                        int ldr, __nv_bfloat16* __restrict__ out, int ldo, int64_t M, int C,
@@ -318,8 +323,19 @@ __global__ void __launch_bounds__(256, 4) bn_apply_kernel(const __nv_bfloat16* _
         // fp64 totals, one channel at a time (no register arrays of doubles); under SyncBN the producer's exchange has
         // already turned them into the world's
         const int cj = rm.g * 8 + j;
-        const double s1 = __ldg(tr.stats + cj);
-        const double s2 = __ldg(tr.stats + C + cj);
+        int rec = 0, w = C, k = cj;
+        if constexpr (TABLE) {
+          if (cj < tr.c0) {
+            w = tr.c0;
+          } else {
+            const int l = (cj - tr.c0) / tr.growth;
+            w = tr.growth;
+            k = cj - tr.c0 - l * tr.growth;
+            rec = 2 * tr.c0 + 2 * l * tr.growth;
+          }
+        }
+        const double s1 = __ldg(tr.stats + rec + k);
+        const double s2 = __ldg(tr.stats + rec + w + k);
         const double mean = s1 * inv_count;
         double var = fma(s2, inv_count, -mean * mean);
         if (var < 0) var = 0;
@@ -497,7 +513,8 @@ __global__ void __launch_bounds__(256, 4)
 }
 
 // dx = A*dz + B*x + Cc with A = gamma*istd, B = -gamma*istd^2*s1/count, Cc = -gamma*istd*s0/count + gamma*istd^2*mean*s1/count
-template <MaskSrc MS>
+// ACC: dx += (the same), summed in fp32 and rounded to bf16 once (pre-activation BN adding into a concat's gradient)
+template <MaskSrc MS, bool ACC = false>
 __global__ void __launch_bounds__(256, 4)
     bn_bwd_apply_kernel(const __nv_bfloat16* __restrict__ dout, int lddo, const __nv_bfloat16* __restrict__ out, int ldo,
                         const uint8_t* __restrict__ mask, const __nv_bfloat16* __restrict__ x, int ldx,
@@ -566,6 +583,12 @@ __global__ void __launch_bounds__(256, 4)
     float o8[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) o8[j] = fmaf(cA[j], dz[j], fmaf(cB[j], xv[j], cC[j]));
+    if constexpr (ACC) {
+      float old[8];
+      unpack8(*reinterpret_cast<const bf16x8*>(dx + row * lddx + co), old);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) o8[j] += old[j];
+    }
     *reinterpret_cast<bf16x8*>(dx + row * lddx + co) = pack8(o8);
   }
   pdl_trigger();
@@ -623,7 +646,7 @@ struct BnBwdFused {
   SyncDesc sync;
 };
 
-template <MaskSrc MS>
+template <MaskSrc MS, bool ACC = false>
 __global__ void __launch_bounds__(256, 3) bn_bwd_fused_kernel(const BnBwdFused p) {
   constexpr bool REMASK = MS == MaskSrc::RECOMPUTE;
   const RowMap rm = row_map(p.C);
@@ -789,6 +812,12 @@ __global__ void __launch_bounds__(256, 3) bn_bwd_fused_kernel(const BnBwdFused p
       float o8[8];
 #pragma unroll
       for (int j = 0; j < 8; ++j) o8[j] = fmaf(cA[j], dz[j], fmaf(cB[j], xv[j], cC[j]));
+      if constexpr (ACC) {  // as bn_bwd_apply_kernel<MS, true>
+        float old[8];
+        unpack8(*reinterpret_cast<const bf16x8*>(p.dx + row * p.lddx + co), old);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) o8[j] += old[j];
+      }
       *reinterpret_cast<bf16x8*>(p.dx + row * p.lddx + co) = pack8(o8);
     }
   }
@@ -1062,6 +1091,64 @@ __global__ void __launch_bounds__(256) adaptive_avgpool_fwd_kernel(const __nv_bf
       s[k] /= (float)cnt;
     }
     *reinterpret_cast<bf16x8*>(y + (((int64_t)n * bins + i) * bins + j) * C + g * 8) = pack8(s);
+  }
+}
+
+// nn.AvgPool2d(2, 2), floor mode (DenseNet's transition1): y[n][p][q] = mean of the 2x2 window at (2p, 2q); a trailing odd
+// row / column is dropped.  The fp32 sum of the four bf16 values is rounded to bf16 once.  ldx / ldy: channel pitches (y may
+// be a channel slice of a concat buffer).
+__global__ void __launch_bounds__(256) avgpool2x2_fwd_kernel(const __nv_bfloat16* __restrict__ x, int ldx,
+                                                             __nv_bfloat16* __restrict__ y, int ldy, int N, int H, int W, int C) {
+  const int G = C >> 3, P = H >> 1, Q = W >> 1;
+  const int64_t total = (int64_t)N * P * Q * G;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int g = (int)(i % G);
+    int64_t t = i / G;
+    const int q = (int)(t % Q);
+    t /= Q;
+    const int pp = (int)(t % P);
+    const int n = (int)(t / P);
+    const int64_t r0 = ((int64_t)n * H + 2 * pp) * W + 2 * q;
+    float a[8], b[8], c[8], d[8], o[8];
+    unpack8(*reinterpret_cast<const bf16x8*>(x + r0 * ldx + g * 8), a);
+    unpack8(*reinterpret_cast<const bf16x8*>(x + (r0 + 1) * ldx + g * 8), b);
+    unpack8(*reinterpret_cast<const bf16x8*>(x + (r0 + W) * ldx + g * 8), c);
+    unpack8(*reinterpret_cast<const bf16x8*>(x + (r0 + W + 1) * ldx + g * 8), d);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) o[j] = ((a[j] + b[j]) + (c[j] + d[j])) * 0.25f;
+    *reinterpret_cast<bf16x8*>(y + (((int64_t)n * P + pp) * Q + q) * ldy + g * 8) = pack8(o);
+  }
+}
+
+// its backward: dx = beta * dx + dy / 4 over every element of dx (0 for a dropped row / column), in fp32, rounded once
+__global__ void __launch_bounds__(256) avgpool2x2_bwd_kernel(const __nv_bfloat16* __restrict__ dy, int lddy,
+                                                             __nv_bfloat16* __restrict__ dx, int lddx, int N, int H, int W, int C,
+                                                             float beta) {
+  const int G = C >> 3, P = H >> 1, Q = W >> 1;
+  const int64_t total = (int64_t)N * H * W * G;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int g = (int)(i % G);
+    const int64_t r = i / G;
+    const int w = (int)(r % W);
+    const int h = (int)((r / W) % H);
+    const int n = (int)(r / ((int64_t)W * H));
+    float v[8];
+    if (h < 2 * P && w < 2 * Q) {
+      unpack8(*reinterpret_cast<const bf16x8*>(dy + (((int64_t)n * P + (h >> 1)) * Q + (w >> 1)) * lddy + g * 8), v);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) v[j] *= 0.25f;
+    } else {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) v[j] = 0.f;
+    }
+    __nv_bfloat16* o = dx + r * lddx + g * 8;
+    if (beta != 0.f) {
+      float old[8];
+      unpack8(*reinterpret_cast<const bf16x8*>(o), old);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) v[j] = fmaf(beta, old[j], v[j]);
+    }
+    *reinterpret_cast<bf16x8*>(o) = pack8(v);
   }
 }
 
@@ -1674,19 +1761,22 @@ int seg_bn_apply(const void* x, int ldx, const float* ss, const void* res, int l
   SEG_REQUIRE(C % 8 == 0 && ldx % 8 == 0 && ldo % 8 == 0 && (!res || ldr % 8 == 0), "bn_apply: alignment");
   BnTrain tr;
   memset(&tr, 0, sizeof(tr));
-  launch_pdl(bn_apply_kernel, rowmap_grid(M, C), dim3(256), 0, ST(stream), CBF(x), ldx, ss, CBF(res), ldr, BF(out), ldo, M, C, relu,
+  launch_pdl(bn_apply_kernel<false>, rowmap_grid(M, C), dim3(256), 0, ST(stream), CBF(x), ldx, ss, CBF(res), ldr, BF(out), ldo, M, C, relu,
              drop_p, seed, step_ctr, drop_hw, tr, (uint8_t*)nullptr);
   return check_launch("bn_apply");
 }
 int seg_bn_apply_train(const void* x, int ldx, const double* stats, double count, const float* gamma, const float* beta,
                        float eps, float momentum, int clamp_eps, float* running_mean, float* running_var, float* save,
                        const void* res, int ldr, void* out, int ldo, uint8_t* mask, int64_t M, int C, int relu, float drop_p,
-                       uint64_t seed, const uint64_t* step_ctr, int drop_hw, void* stream) {
+                       uint64_t seed, const uint64_t* step_ctr, int drop_hw, int c0, int growth, void* stream) {
   SEG_REQUIRE(C % 8 == 0 && ldx % 8 == 0 && ldo % 8 == 0 && (!res || ldr % 8 == 0), "bn_apply_train: alignment");
   SEG_REQUIRE(stats && gamma && beta && save && count > 0, "bn_apply_train: stats, gamma, beta, save required");
   SEG_REQUIRE(!mask || relu, "bn_apply_train: the ReLU bit mask needs relu");
-  BnTrain tr = {stats, count, gamma, beta, eps, momentum, clamp_eps, running_mean, running_var, save};
-  launch_pdl(bn_apply_kernel, rowmap_grid(M, C), dim3(256), 0, ST(stream), CBF(x), ldx, (const float*)nullptr, CBF(res), ldr, BF(out),
+  SEG_REQUIRE(growth >= 0 && (growth == 0 || (c0 > 0 && c0 <= C)),
+              "bn_apply_train: statistics table needs 0 < c0 <= C and growth > 0 (c0=%d growth=%d C=%d)", c0, growth, C);
+  BnTrain tr = {stats, count, gamma, beta, eps, momentum, clamp_eps, running_mean, running_var, save, c0, growth};
+  launch_pdl(growth > 0 ? bn_apply_kernel<true> : bn_apply_kernel<false>, rowmap_grid(M, C), dim3(256), 0, ST(stream), CBF(x), ldx,
+             (const float*)nullptr, CBF(res), ldr, BF(out),
              ldo, M, C, relu, drop_p, seed, step_ctr, drop_hw, tr, mask);
   return check_launch("bn_apply_train");
 }
@@ -1713,25 +1803,29 @@ int seg_bn_bwd_reduce(const void* dout, int lddo, const void* out, int ldo, cons
 }
 int seg_bn_bwd_apply(const void* dout, int lddo, const void* out, int ldo, const uint8_t* mask, const void* x, int ldx,
                      const float* save, const float* gamma, const float* sums, double count, int64_t M, int C, int relu,
-                     float drop_p, void* dx, int lddx, void* dres, int lddres, float beta_res, const float* beta, void* stream) {
+                     float drop_p, void* dx, int lddx, void* dres, int lddres, float beta_res, const float* beta, float beta_dx,
+                     void* stream) {
   const MaskSrc ms = mask_src(relu, out, mask);
   SEG_REQUIRE(C % 8 == 0 && lddo % 8 == 0 && ldx % 8 == 0 && lddx % 8 == 0, "bn_bwd_apply: alignment");
   SEG_REQUIRE(ms != MaskSrc::RECOMPUTE || (beta && drop_p == 0.f), "bn_bwd_apply: out == NULL (mask recomputed from x) needs beta and no dropout");
   SEG_REQUIRE(relu || drop_p == 0.f, "bn_bwd_apply: dropout (drop_p > 0) needs relu: the keep mask is read from out > 0");
-  launch_pdl(by_mask_src(ms, bn_bwd_apply_kernel<MaskSrc::ACT>, bn_bwd_apply_kernel<MaskSrc::RECOMPUTE>,
-                         bn_bwd_apply_kernel<MaskSrc::BITS>),
+  SEG_REQUIRE(beta_dx == 0.f || beta_dx == 1.f, "bn_bwd_apply: beta_dx must be 0 or 1 (got %g)", (double)beta_dx);
+  launch_pdl(beta_dx != 0.f ? by_mask_src(ms, bn_bwd_apply_kernel<MaskSrc::ACT, true>, bn_bwd_apply_kernel<MaskSrc::RECOMPUTE, true>,
+                                          bn_bwd_apply_kernel<MaskSrc::BITS, true>)
+                            : by_mask_src(ms, bn_bwd_apply_kernel<MaskSrc::ACT>, bn_bwd_apply_kernel<MaskSrc::RECOMPUTE>,
+                                          bn_bwd_apply_kernel<MaskSrc::BITS>),
              rowmap_grid(M, C), dim3(256), 0, ST(stream), CBF(dout), lddo, CBF(out), ldo, mask, CBF(x), ldx, save,
              gamma, sums, (float)(1.0 / count), M, C, relu, drop_p, BF(dx), lddx, BF(dres), lddres, beta_res, beta);
   return check_launch("bn_bwd_apply");
 }
 }  // extern "C"
 // co-resident grid of the cooperative kernel: blocks per SM from the occupancy of the instantiation actually launched
-template <MaskSrc MS>
+template <MaskSrc MS, bool ACC = false>
 static int fused_blocks_per_sm() {
   static int v = 0;
   if (v == 0) {
     int n = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, bn_bwd_fused_kernel<MS>, 256, 0) != cudaSuccess || n < 1) n = 1;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, bn_bwd_fused_kernel<MS, ACC>, 256, 0) != cudaSuccess || n < 1) n = 1;
     v = n;
   }
   return v;
@@ -1744,6 +1838,15 @@ static int fused_bps(MaskSrc ms) {
   if (ms == MaskSrc::ACT) return act;
   const int bits = fused_blocks_per_sm<MaskSrc::BITS>();
   return bits < act ? bits : act;
+}
+// the accumulating variant: never more blocks than it can keep co-resident (the grid barrier needs every block resident)
+static int fused_bps(MaskSrc ms, bool acc) {
+  const int b = fused_bps(ms);
+  if (!acc) return b;
+  const int a = ms == MaskSrc::RECOMPUTE ? fused_blocks_per_sm<MaskSrc::RECOMPUTE, true>()
+                : ms == MaskSrc::BITS   ? fused_blocks_per_sm<MaskSrc::BITS, true>()
+                                        : fused_blocks_per_sm<MaskSrc::ACT, true>();
+  return a < b ? a : b;
 }
 extern "C" {
 static dim3 fused_grid(int64_t M, int C, int blocks_per_sm) {
@@ -1765,8 +1868,11 @@ int seg_bn_bwd_fused_workspace(int64_t M, int C, int64_t* rows_floats, int64_t* 
 int seg_bn_bwd_fused(const void* dout, int lddo, const void* out, int ldo, const uint8_t* mask, const void* x, int ldx,
                      const float* save, const float* gamma, const float* beta, double count_total, int64_t M, int C, int relu,
                      float drop_p, float* sums, float* rows, void* tickets, float* dgamma, float* dbeta, int accumulate, void* dx,
-                     int lddx, void* dres, int lddres, float beta_res, int zero_sums, const seg_sync_desc* sync, void* stream) {
+                     int lddx, void* dres, int lddres, float beta_res, int zero_sums, const seg_sync_desc* sync, float beta_dx,
+                     void* stream) {
   const MaskSrc ms = mask_src(relu, out, mask);
+  SEG_REQUIRE(beta_dx == 0.f || beta_dx == 1.f, "bn_bwd_fused: beta_dx must be 0 or 1 (got %g)", (double)beta_dx);
+  const bool acc = beta_dx != 0.f;
   SEG_REQUIRE(C % 8 == 0 && lddo % 8 == 0 && ldx % 8 == 0 && lddx % 8 == 0 && (!out || ldo % 8 == 0) && (!dres || lddres % 8 == 0),
               "bn_bwd_fused: alignment");
   SEG_REQUIRE(ms != MaskSrc::RECOMPUTE || (beta && drop_p == 0.f), "bn_bwd_fused: out == NULL (mask recomputed from x) needs beta and no dropout");
@@ -1787,11 +1893,13 @@ int seg_bn_bwd_fused(const void* dout, int lddo, const void* out, int ldo, const
   }
   // multi-GPU: leave one block slot per SM free — a concurrently running NCCL kernel (bucketed gradient all-reduce on the side
   // stream) must not keep part of this grid from becoming resident, or every block would sit at the barrier until it finishes
-  int bps = fused_bps(ms);
+  int bps = fused_bps(ms, acc);
   if (sync && bps > 1) bps -= 1;
   const dim3 grid = fused_grid(M, C, bps);
-  by_mask_src(ms, bn_bwd_fused_kernel<MaskSrc::ACT>, bn_bwd_fused_kernel<MaskSrc::RECOMPUTE>,
-              bn_bwd_fused_kernel<MaskSrc::BITS>)<<<grid, 256, 0, ST(stream)>>>(p);
+  (acc ? by_mask_src(ms, bn_bwd_fused_kernel<MaskSrc::ACT, true>, bn_bwd_fused_kernel<MaskSrc::RECOMPUTE, true>,
+                     bn_bwd_fused_kernel<MaskSrc::BITS, true>)
+       : by_mask_src(ms, bn_bwd_fused_kernel<MaskSrc::ACT>, bn_bwd_fused_kernel<MaskSrc::RECOMPUTE>,
+                     bn_bwd_fused_kernel<MaskSrc::BITS>))<<<grid, 256, 0, ST(stream)>>>(p);
   return check_launch("bn_bwd_fused");
 }
 int seg_bn_param_grad(const float* sums, int C, float* dgamma, float* dbeta, int accumulate, void* stream) {
@@ -1875,6 +1983,21 @@ int seg_adaptive_avgpool_bwd(const void* dy, void* dx, int lddx, int N, int H, i
   adaptive_avgpool_bwd_kernel<<<grid_for((int64_t)N * H * W * (C / 8), 256), 256, 0, ST(stream)>>>(CBF(dy), BF(dx), lddx, N, H,
                                                                                                    W, C, bins, beta);
   return check_launch("adaptive_avgpool_bwd");
+}
+
+int seg_avgpool2x2_fwd(const void* x, int ldx, void* y, int ldy, int N, int H, int W, int C, void* stream) {
+  SEG_REQUIRE(C % 8 == 0 && ldx % 8 == 0 && ldy % 8 == 0 && ldx >= C && ldy >= C, "avgpool2x2: alignment");
+  SEG_REQUIRE(N > 0 && H >= 2 && W >= 2, "avgpool2x2: needs H, W >= 2 (got %dx%d)", H, W);
+  avgpool2x2_fwd_kernel<<<grid_for((int64_t)N * (H / 2) * (W / 2) * (C / 8), 256), 256, 0, ST(stream)>>>(CBF(x), ldx, BF(y), ldy, N,
+                                                                                                         H, W, C);
+  return check_launch("avgpool2x2_fwd");
+}
+int seg_avgpool2x2_bwd(const void* dy, int lddy, void* dx, int lddx, int N, int H, int W, int C, float beta, void* stream) {
+  SEG_REQUIRE(C % 8 == 0 && lddy % 8 == 0 && lddx % 8 == 0 && lddy >= C && lddx >= C, "avgpool2x2_bwd: alignment");
+  SEG_REQUIRE(N > 0 && H >= 2 && W >= 2, "avgpool2x2_bwd: needs H, W >= 2 (got %dx%d)", H, W);
+  avgpool2x2_bwd_kernel<<<grid_for((int64_t)N * H * W * (C / 8), 256), 256, 0, ST(stream)>>>(CBF(dy), lddy, BF(dx), lddx, N, H, W,
+                                                                                             C, beta);
+  return check_launch("avgpool2x2_bwd");
 }
 
 int seg_bilinear_fwd(const void* x, int ldx, void* y, int ldy, int N, int Hi, int Wi, int Ho, int Wo, int C,

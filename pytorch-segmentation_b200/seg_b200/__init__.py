@@ -14,6 +14,7 @@ _LAZY = {
     "UNetResnet": ("nets", "UNetResnet"),
     "SegNet": ("nets", "SegNet"),
     "FCN8": ("nets", "FCN8"),
+    "PSPDenseNet": ("nets", "PSPDenseNet"),
     "CrossEntropyLoss2d": ("losses", "CrossEntropyLoss2d"),
     "DiceLoss": ("losses", "DiceLoss"),
     "FocalLoss": ("losses", "FocalLoss"),

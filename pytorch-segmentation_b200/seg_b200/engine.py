@@ -208,9 +208,10 @@ class Tape:
         self.back = []
 
     # ------------------------------------------------------------------ conv
-    def conv(self, x, spec, out=None, out_dtype=None, want_stats=False, use_bias=True):
+    def conv(self, x, spec, out=None, out_dtype=None, want_stats=False, use_bias=True, stats_out=None):
         """x: Act (NHWC bf16) — or, for an explicit-im2col conv, a raw NCHW fp32 tensor (the network input).  use_bias=False
-        leaves the module's bias out of the epilogue and its gradient (a consumer applies it: `score_upsample`)."""
+        leaves the module's bias out of the epilogue and its gradient (a consumer applies it: `score_upsample`).
+        stats_out: zeroed fp64 [2K] record (a slice of a dense block's statistics table) the epilogue's statistics go to."""
         wp = self.packed_override.get(spec)
         if wp is None:
             wp = spec.packed()
@@ -221,7 +222,8 @@ class Tape:
         want = want_stats and self.training
         sync = tk = None
         if want:
-            stats = self.zalloc64(2 * spec.K, wp.device)  # fp64 accumulators: the conv epilogue adds its column sums
+            # fp64 accumulators: the conv epilogue adds its column sums
+            stats = self.zalloc64(2 * spec.K, wp.device) if stats_out is None else stats_out
             if self.sync_fused():  # SyncBN: the last CTA pushes the totals to the peers (no exchange launch)
                 sync, tk = self.sync, self.zalloc(1, wp.device)
         if spec.explicit:
@@ -240,6 +242,8 @@ class Tape:
         ya = Act(y)
         if sync is not None:
             self._pushed.add(stats.data_ptr())
+        elif want and stats_out is not None:
+            self.exchange_record(stats)
         if self.record:
             def bwd():
                 dy = ya.grad
@@ -355,10 +359,32 @@ class Tape:
             self.back.append(bwd)
         return ya
 
+    # ------------------------------------------------------------------ dense-block statistics table
+    def exchange_record(self, stats):
+        """A statistics record a producer wrote into a dense block's table: with an exchange object that has no in-kernel
+        protocol (the gloo stand-in), sum it over the ranks here, once — its consumers (every later layer's norm1) never
+        exchange a prefix."""
+        if self.sync_active() and stats.data_ptr() not in self._pushed:
+            self.sync.allreduce_(stats)
+            self._pushed.add(stats.data_ptr())
+
+    def record_stats(self, x, stats):
+        """bn_stats of x (a slice of a dense block's buffer) into its zeroed table record, exchanged once."""
+        if not self.training:
+            return
+        sync0 = self.sync if self.sync_fused() else None
+        ops.bn_stats(x.t, stats=stats, sync=sync0)
+        if sync0 is not None:
+            self._pushed.add(stats.data_ptr())
+        self.exchange_record(stats)
+
     # ------------------------------------------------------------------ batch norm (+ residual, ReLU, dropout)
-    def bn_act(self, y, bn, stats=None, relu=True, res=None, out=None, drop_p=0.0, drop_channelwise=False):
+    def bn_act(self, y, bn, stats=None, relu=True, res=None, out=None, drop_p=0.0, drop_channelwise=False, table=None):
         """y: Act holding the raw conv output.  Returns the activated Act.  drop_channelwise: nn.Dropout2d semantics (one
-        draw per image and channel, models/pspnet.py:22,68) instead of nn.Dropout's per-element draws."""
+        draw per image and channel, models/pspnet.py:22,68) instead of nn.Dropout's per-element draws.
+        table = (stats table, c0, growth): pre-activation BN over a dense block's channel prefix y (`prefix`): the batch
+        statistics come from the block's table (records exchanged by their producers), and the backward ADDS the data
+        gradient into y's gradient (a view of the block's) as its first writer's beta dictates."""
         drop_hw = y.t.shape[1] * y.t.shape[2] if drop_channelwise else 0
         C = y.t.shape[-1]
         count_local = ops.rows(y.t)
@@ -375,6 +401,12 @@ class Tape:
         # with the forward's own coefficients instead of being read (the one-launch backward of the small maps does so)
         remask = bool(use_batch_stats and relu and res is None and drop_p == 0.0)
         mask_kw = {}
+        table_kw, acc_kw = {}, {}
+        if table is not None:
+            if use_batch_stats:
+                stats, table_kw = table[0], {"table": (table[1], table[2])}
+            else:
+                stats = None
         if use_batch_stats:
             if stats is None:
                 sync0 = self.sync if self.sync_fused() else None
@@ -384,7 +416,7 @@ class Tape:
             count = count_local
             if self.sync_active():
                 # a producer called with sync= has already exchanged: `stats` holds the world's totals
-                if stats.data_ptr() not in self._pushed:
+                if stats.data_ptr() not in self._pushed and table is None:
                     # exchange object without the in-kernel protocol (the gloo stand-in of the CPU tests): sums over ranks
                     self.sync.allreduce_(stats)
                 count = count_local * self.sync.world
@@ -401,7 +433,7 @@ class Tape:
                                          1 if (self.clamp_eps and self.sync is not None and self.sync.world > 1) else 0,
                                          bn.running_mean, bn.running_var, res=res.t if res is not None else None, out=out,
                                          relu=relu, drop_p=drop_p, seed=seed, step_ctr=self.step_ctr if drop_p > 0.0 else None,
-                                         drop_hw=drop_hw, **mask_kw)
+                                         drop_hw=drop_hw, **mask_kw, **table_kw)
             self.bn_modules.append(bn)
         else:
             ss, save = ops.bn_eval_scale_shift(bn.weight.detach(), bn.bias.detach(), bn.running_mean, bn.running_var, bn.eps,
@@ -423,7 +455,13 @@ class Tape:
                     self.grads[bn.weight] = torch.empty(C, dtype=torch.float32, device=a.device)
                     self.grads[bn.bias] = torch.empty(C, dtype=torch.float32, device=a.device)
                 a_mask = None if remask else a  # the bit mask in mask_kw takes precedence
-                dy = torch.empty(y.t.shape, dtype=ACT_DTYPE, device=a.device)
+                acc_kw = {}
+                if table is not None:
+                    dy, beta_dx = y.grad_target()
+                    if beta_dx:
+                        acc_kw = {"beta_dx": beta_dx}
+                else:
+                    dy = torch.empty(y.t.shape, dtype=ACT_DTYPE, device=a.device)
                 dres, beta_res = (None, 0.0)
                 if res is not None and res.needs_grad:
                     dres, beta_res = res.grad_target()
@@ -437,7 +475,7 @@ class Tape:
                     gsums = sums.clone()
                     sync.allreduce_(gsums)
                     ops.bn_bwd_apply(da, a_mask, y.t, save, bn.weight.detach(), gsums, count, relu=relu, drop_p=drop_p, dx=dy,
-                                     dres=dres, beta_res=beta_res, beta=bn.bias.detach(), **mask_kw)
+                                     dres=dres, beta_res=beta_res, beta=bn.bias.detach(), **mask_kw, **acc_kw)
                 elif count_local * C * 2 <= FUSED_BWD_MAX_BYTES:
                     # small maps (the operands stay in L2 between the phases): reduce -> grid barrier -> fixed-order cross-block
                     # sum (-> SyncBN exchange) -> apply in ONE cooperative launch.  Frozen BN (freeze_bn): dx = gamma*inv_std*dz,
@@ -445,7 +483,7 @@ class Tape:
                     # grid-barrier counter
                     ops.bn_bwd_fused(da, a_mask, y.t, save, bn.weight.detach(), count, relu=relu, drop_p=drop_p, dgamma=dg, dbeta=db,
                                      accumulate=acc_pg, dx=dy, dres=dres, beta_res=beta_res, beta=bn.bias.detach(),
-                                     zero_sums=not use_batch_stats, tickets=self.zalloc(1, a.device), sync=sync, **mask_kw)
+                                     zero_sums=not use_batch_stats, tickets=self.zalloc(1, a.device), sync=sync, **mask_kw, **acc_kw)
                 else:
                     # large maps stream from HBM in both passes anyway: two launches at full occupancy; under SyncBN the
                     # reduction's last block exchanges the sums, so the apply pass gets the world's
@@ -453,7 +491,7 @@ class Tape:
                                              acc=self.zalloc64(ops.bn_bwd_reduce_acc_words(C), a.device), sync=sync, **mask_kw)
                     gsums = sums if use_batch_stats else torch.zeros_like(sums)
                     ops.bn_bwd_apply(da, a_mask, y.t, save, bn.weight.detach(), gsums, count, relu=relu, drop_p=drop_p, dx=dy,
-                                     dres=dres, beta_res=beta_res, beta=bn.bias.detach(), **mask_kw)
+                                     dres=dres, beta_res=beta_res, beta=bn.bias.detach(), **mask_kw, **acc_kw)
                 y.grad = dy
                 aa.grad = None
             self._push_back(bwd, (bn.weight, bn.bias))
@@ -580,6 +618,20 @@ class Tape:
             self._push_back(bwd, (bias,))
         return ya
 
+    def avgpool2x2(self, x, out=None):
+        """nn.AvgPool2d(2, 2), floor mode (DenseNet's transition1), into `out` (a channel slice of the next block's buffer)."""
+        y = ops.avgpool2x2_fwd(x.t, out=out)
+        ya = Act(y)
+        if self.record:
+            def bwd():
+                if ya.grad is None or not x.needs_grad:
+                    return
+                gx, beta = x.grad_target()
+                ops.avgpool2x2_bwd(ya.grad, tuple(x.t.shape), dx=gx, beta=beta)
+                ya.grad = None
+            self.back.append(bwd)
+        return ya
+
     def avgpool(self, x, bins):
         y = ops.adaptive_avgpool_fwd(x.t, bins)
         ya = Act(y)
@@ -678,7 +730,9 @@ class Tape:
         """After the producers ran: make each producer Act's gradient a view of the concat gradient buffer."""
         if not self.record:
             return
-        g = torch.empty(whole.t.shape, dtype=ACT_DTYPE, device=whole.t.device)
+        g = whole.grad  # pre-allocated by `dense_buffer`
+        if g is None:
+            g = torch.empty(whole.t.shape, dtype=ACT_DTYPE, device=whole.t.device)
         whole.grad = g
         off = 0
         for a in acts:
@@ -686,6 +740,26 @@ class Tape:
             a.grad = g[..., off:off + c]
             off += c
         whole._written = False  # the consumer's dgrad overwrites (beta = 0) the pre-allocated buffer
+
+    def dense_buffer(self, N, H, W, C, device):
+        """A dense block's NHWC buffer: its producers write channel slices in place and its layers read prefixes (`prefix`).
+        Its gradient buffer exists from the start, so the prefix views can be bound before the backward runs; the block's
+        downstream consumer writes it first (beta = 0), every later writer adds."""
+        whole = Act(torch.empty((N, H, W, C), dtype=ACT_DTYPE, device=device))
+        if self.record:
+            whole.grad = torch.empty((N, H, W, C), dtype=ACT_DTYPE, device=device)
+        return whole
+
+    def prefix(self, whole, c0, c1=None, act=None):
+        """Channels [c0, c1) of a `dense_buffer` as an Act whose gradient is the matching view of the block's gradient,
+        written before any consumer of the view runs its backward (so every writer accumulates).  act: the Act of the
+        producer that wrote those channels in place, bound instead of a new one."""
+        c1 = whole.t.shape[-1] if c1 is None else c1
+        a = Act(whole.t[..., c0:c1]) if act is None else act
+        if whole.grad is not None:
+            a.grad = whole.grad[..., c0:c1]
+            a._written = True
+        return a
 
     def shared_slice(self, act):
         """`act` was produced into a concat slice (and bound by `bind_slices`) and has consumers of its own besides the

@@ -69,11 +69,11 @@ _SIGS = {
     "seg_counter_add": (c_int, [c_void_p, c_uint64, c_void_p]),
     "seg_bn_bwd_reduce_slots": (c_int, []),
     "seg_bn_bwd_reduce": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int64, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
-    "seg_bn_apply_train": (c_int, [c_void_p, c_int, c_void_p, c_double, c_void_p, c_void_p, c_float, c_float, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int64, c_int, c_int, c_float, c_uint64, c_void_p, c_int, c_void_p]),
+    "seg_bn_apply_train": (c_int, [c_void_p, c_int, c_void_p, c_double, c_void_p, c_void_p, c_float, c_float, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int64, c_int, c_int, c_float, c_uint64, c_void_p, c_int, c_int, c_int, c_void_p]),
     "seg_bn_bwd_fused_workspace": (c_int, [c_int64, c_int, POINTER(c_int64), POINTER(c_int64)]),
     "seg_bn_bwd_fused": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_double, c_int64, c_int, c_int, c_float,
-                                 c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_float, c_int, c_void_p, c_void_p]),
-    "seg_bn_bwd_apply": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_double, c_int64, c_int, c_int, c_float, c_void_p, c_int, c_void_p, c_int, c_float, c_void_p, c_void_p]),
+                                 c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_float, c_int, c_void_p, c_float, c_void_p]),
+    "seg_bn_bwd_apply": (c_int, [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_double, c_int64, c_int, c_int, c_float, c_void_p, c_int, c_void_p, c_int, c_float, c_void_p, c_float, c_void_p]),
     "seg_bn_param_grad": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p]),
     "seg_maxpool3x3s2_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "seg_maxpool3x3s2_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
@@ -83,6 +83,8 @@ _SIGS = {
     "seg_maxunpool2x2_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "seg_relu_maxpool2x2_ceil_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "seg_relu_maxpool2x2_ceil_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "seg_avgpool2x2_fwd": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "seg_avgpool2x2_bwd": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "seg_adaptive_avgpool_fwd": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
     "seg_adaptive_avgpool_bwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "seg_bilinear_fwd": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),

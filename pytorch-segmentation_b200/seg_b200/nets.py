@@ -7,6 +7,7 @@
     UNetResnet(num_classes, in_channels=3, backbone='resnet50', pretrained=None, freeze_bn=False, **_)
     SegNet(num_classes, in_channels=3, pretrained=None, freeze_bn=False, freeze_backbone=False, **_)
     FCN8(num_classes, pretrained=None, freeze_bn=False, freeze_backbone=False, **_)
+    PSPDenseNet(num_classes, in_channels=3, backbone='densenet201', pretrained=None, use_aux=True, freeze_bn=False, **_)
 
 (default backbones are the reference's; `pretrained`: the reference defaults to True and downloads ImageNet weights — there is
 no network here, so an explicit True raises and the default (None) initialises randomly with a logged warning)
@@ -818,14 +819,21 @@ class PSPNet(_EngineModel):
             heads.append(BilinearHead(la, False, H, W))
         return heads
 
-    def _psp_head(self, tape, a):
-        """_PSPModule.forward + the classifier (pspnet.py:31-38, :66-70): returns the fp32 stride-8 logits Act."""
-        N, Hf, Wf = a.t.shape[0], a.t.shape[1], a.t.shape[2]
+    def _psp_head(self, tape, a, cat=None):
+        """_PSPModule.forward + the classifier (pspnet.py:31-38, :66-70): returns the fp32 stride-8 logits Act.  a: the trunk
+        output (m channels; stages of m // 4).  cat: a `dense_buffer` of 2m channels whose first m the trunk wrote in place
+        (PSPDenseNet's block4); otherwise the concat is allocated here."""
+        N, Hf, Wf, m = a.t.shape
+        q = m // 4
         psp = self.master_branch[0]
-        # pspnet.py:31-38: cat([features, stage1..4]) -> 3x3 bottleneck.  The trunk output is copied into slice 0
+        # pspnet.py:31-38: cat([features, stage1..4]) -> 3x3 bottleneck.  A ResNet trunk's output is copied into slice 0
         # (it is also the residual-stream tensor, so it cannot simply be produced in place there).
-        cat, sl = tape.concat(N, Hf, Wf, [2048, 512, 512, 512, 512], a.t.device)
-        feats = tape.copy_into(a, sl[0])
+        if cat is None:
+            cat, sl = tape.concat(N, Hf, Wf, [m, q, q, q, q], a.t.device)
+            feats = tape.copy_into(a, sl[0])
+        else:
+            sl = [cat.t[..., :m]] + [cat.t[..., m + i * q:m + (i + 1) * q] for i in range(4)]
+            feats = a
         br = [feats]
         for i, b in enumerate(self.bins):
             st = psp.stages[i]
@@ -1404,3 +1412,188 @@ class FCN8(_EngineModel):
     def get_decoder_params(self):
         return chain(self.up_output.parameters(), self.adj_pool4.parameters(), self.up_pool4_out.parameters(),
                      self.adj_pool3.parameters(), self.up_final.parameters())
+
+
+# ----------------------------------------------------------------------------------------------- PSPDenseNet
+DENSENET_BLOCKS = {"densenet121": (6, 12, 24, 16), "densenet169": (6, 12, 32, 32), "densenet201": (6, 12, 48, 32)}
+GROWTH, BN_SIZE = 32, 4  # torchvision densenet121/169/201: growth_rate 32, bn_size 4, num_init_features 64
+
+
+def _dense_block(cin, n, dil):
+    """torchvision _DenseBlock holder: denselayerK = norm1, relu1, conv1 (1x1 -> 4 * growth), norm2, relu2, conv2 (3x3 ->
+    growth, dilation / padding `dil`), reading the concat of the block input and every earlier layer's output."""
+    blk = _Holder()
+    for k in range(n):
+        lay = _Holder()
+        lay.norm1, lay.relu1 = nn.BatchNorm2d(cin + k * GROWTH), nn.ReLU(inplace=True)
+        lay.conv1 = nn.Conv2d(cin + k * GROWTH, BN_SIZE * GROWTH, 1, bias=False)
+        lay.norm2, lay.relu2 = nn.BatchNorm2d(BN_SIZE * GROWTH), nn.ReLU(inplace=True)
+        lay.conv2 = nn.Conv2d(BN_SIZE * GROWTH, GROWTH, 3, padding=dil, dilation=dil, bias=False)
+        setattr(blk, f"denselayer{k + 1}", lay)
+    return blk
+
+
+class PSPDenseNet(_EngineModel):
+    """PSPNet over a dilated DenseNet-121/169/201 — replaces models/pspnet.py:117-205 (trained from scratch: the custom
+    block0).  block0 = Conv2d(in, 64, 3, s2) BN ReLU, then [Conv2d(64, 64, 3) BN ReLU] * 2 — ONE conv and ONE BN applied
+    twice (block0.3 is block0.6, block0.4 is block0.7; every conv unpadded), MaxPool2d(3, 2, 1); the dense blocks; transition1
+    = norm relu 1x1 conv AvgPool2d(2, 2); transition2 / 3 without the pool; block3 / block4's conv2 dilated 2 / 4; no norm5:
+    block4's concat feeds the PSP module (bins 1, 2, 3, 6), whose bottleneck, dropout and classifier are PSPNet's; the aux
+    branch reads transition3's output.  Logits: bilinear, align_corners=False.
+    Each dense block is ONE buffer of its final width (`Tape.dense_buffer`): the block input and every conv2 write their
+    channel slice in place, and each norm1 is a pre-activation BN over the prefix, whose batch statistics come from the
+    block's table of per-slice records (`Tape.bn_act(table=)`) and whose backward adds into the prefix of the block's
+    gradient.  block4's buffer is the PSP concat, so the trunk output is never copied.
+    Init as the reference: torchvision's DenseNet init for the trunk (kaiming-normal convs, BN 1 / 0), initialize_weights for
+    block0 and the heads.  Parameter groups as the reference's (block4 is in neither).  freeze_backbone is ignored, as
+    there.  densenet161 raises NotImplementedError: its block1 expects 96 channels and the reference cannot train it from
+    scratch."""
+
+    def __init__(self, num_classes, in_channels=3, backbone="densenet201", pretrained=None, use_aux=True, freeze_bn=False, **_):
+        super().__init__()
+        if backbone == "densenet161":
+            raise NotImplementedError("PSPDenseNet(densenet161) cannot train from scratch in the reference either: its block1 "
+                                      "expects 96 input channels but block0 gives 64 (RuntimeError: running_mean should "
+                                      "contain 64 elements not 96)")
+        if backbone not in DENSENET_BLOCKS:
+            raise NotImplementedError(f"seg_b200.PSPDenseNet: backbone {backbone!r} not built")
+        _check_pretrained(self, pretrained)
+        self.num_classes, self.use_aux = num_classes, use_aux
+        self.layers = DENSENET_BLOCKS[backbone]
+        c3 = nn.Conv2d(64, 64, 3, bias=False)
+        n3 = nn.BatchNorm2d(64)
+        r3 = nn.ReLU(inplace=True)
+        self.block0 = nn.Sequential(nn.Conv2d(in_channels, 64, 3, stride=2, bias=False), nn.BatchNorm2d(64), nn.ReLU(inplace=True),
+                                    c3, n3, r3, c3, n3, r3, nn.MaxPool2d(kernel_size=3, stride=2, padding=1))
+        widths, c = [], 64
+        for bi, n in enumerate(self.layers):
+            widths.append((c, c + n * GROWTH))
+            c = (c + n * GROWTH) // 2
+        self.widths = widths  # (input, output) channels of each dense block
+        for bi, ((cin, _), n, dil) in enumerate(zip(widths, self.layers, (1, 1, 2, 4))):
+            setattr(self, f"block{bi + 1}", _dense_block(cin, n, dil))
+        t1 = _Holder()
+        t1.norm, t1.relu = nn.BatchNorm2d(widths[0][1]), nn.ReLU(inplace=True)
+        t1.conv = nn.Conv2d(widths[0][1], widths[1][0], 1, bias=False)
+        t1.pool = nn.AvgPool2d(kernel_size=2, stride=2)
+        self.transition1 = t1
+        for k in (2, 3):
+            cin, cout = widths[k - 1][1], widths[k][0]
+            setattr(self, f"transition{k}", nn.Sequential(nn.BatchNorm2d(cin), nn.ReLU(inplace=True), nn.Conv2d(cin, cout, 1, bias=False)))
+        m_out, aux_in = widths[3][1], widths[3][0]
+        psp = _Holder()
+        stages = []
+        for b in (1, 2, 3, 6):
+            cv, bn = _cbn(m_out, m_out // 4, 1)
+            stages.append(nn.Sequential(nn.AdaptiveAvgPool2d(output_size=b), cv, bn, nn.ReLU(inplace=True)))
+        psp.stages = nn.ModuleList(stages)
+        cv, bn = _cbn(m_out * 2, m_out // 4, 3)
+        psp.bottleneck = nn.Sequential(cv, bn, nn.ReLU(inplace=True), nn.Dropout2d(0.1))
+        self.master_branch = nn.Sequential(psp, nn.Conv2d(m_out // 4, num_classes, kernel_size=1))
+        cv, bn = _cbn(aux_in, m_out // 4, 3)
+        self.auxiliary_branch = nn.Sequential(cv, bn, nn.ReLU(inplace=True), nn.Dropout2d(0.1),
+                                              nn.Conv2d(m_out // 4, num_classes, kernel_size=1))
+        self.bins = (1, 2, 3, 6)
+        for mod in (self.block1, self.block2, self.block3, self.block4, self.transition1, self.transition2, self.transition3):
+            for m in mod.modules():  # torchvision DenseNet.__init__
+                if isinstance(m, nn.Conv2d):
+                    nn.init.kaiming_normal_(m.weight)
+                elif isinstance(m, nn.BatchNorm2d):
+                    nn.init.constant_(m.weight, 1)
+                    nn.init.constant_(m.bias, 0)
+        _init_like_reference_head(self.block0)
+        _init_like_reference_head(self.master_branch, self.auxiliary_branch)
+        if freeze_bn:
+            self.freeze_bn()
+
+    _psp_head = PSPNet._psp_head
+
+    def _spec(self, name, module):
+        # the network input (NCHW fp32, any channel count) always goes through the explicit im2col conv
+        s = self._specs.get(name)
+        if s is None or s.m is not module:
+            s = ConvSpec(name, module, explicit_im2col=(name == "block0.0"))
+            self._specs[name] = s
+        return s
+
+    def _finish(self, tape):
+        # block0.4 normalises twice per step: its num_batches_tracked rises by 2, as the reference's
+        counts = {}
+        for m in tape.bn_modules:
+            counts[m] = counts.get(m, 0) + 1
+        for k in sorted(set(counts.values())):
+            torch._foreach_add_([m.num_batches_tracked for m, c in counts.items() if c == k], k)
+
+    def _dense(self, tape, buf, table, bi, c0, dil):
+        """Block bi's layers over its buffer (slice [0, c0) already written, its record in table[:2 c0])."""
+        blk = getattr(self, f"block{bi}")
+        for k in range(self.layers[bi - 1]):
+            lay = getattr(blk, f"denselayer{k + 1}")
+            cin, name = c0 + k * GROWTH, f"block{bi}.denselayer{k + 1}"
+            h = tape.bn_act(tape.prefix(buf, 0, cin), lay.norm1, table=(table, c0, GROWTH))
+            h = self._cbr(tape, h, name + ".conv1", lay.conv1, lay.norm2)
+            rec = table[2 * cin:2 * cin + 2 * GROWTH] if table is not None else None
+            y, _ = tape.conv(h, self._spec(name + ".conv2", lay.conv2), out=buf.t[..., cin:cin + GROWTH], want_stats=True,
+                             stats_out=rec)
+            tape.prefix(buf, cin, cin + GROWTH, act=y)
+
+    def _block_buffer(self, tape, N, H, W, bi, pitch=None):
+        c0, c1 = self.widths[bi - 1]
+        buf = tape.dense_buffer(N, H, W, pitch or c1, self.block0[0].weight.device)
+        table = tape.zalloc64(2 * c1, buf.t.device) if tape.training else None
+        return buf, table
+
+    def _forward_heads(self, tape, x):
+        N, _, H, W = x.shape
+        b0 = self.block0
+        a = self._cbr(tape, x, "block0.0", b0[0], b0[1])
+        a = self._cbr(tape, a, "block0.3", b0[3], b0[4])
+        a = self._cbr(tape, a, "block0.3", b0[6], b0[7])  # block0.6 / block0.7 are block0.3 / block0.4: one ConvSpec
+        a = tape.maxpool(a)
+        Hb, Wb = a.t.shape[1], a.t.shape[2]
+        # block1: the max-pooled stem is copied into slice 0
+        buf, table = self._block_buffer(tape, N, Hb, Wb, 1)
+        s0 = tape.prefix(buf, 0, 64, act=tape.copy_into(a, buf.t[..., :64]))
+        if table is not None:
+            tape.record_stats(s0, table[:128])
+        self._dense(tape, buf, table, 1, 64, 1)
+        # transition1: BN ReLU 1x1 conv, then the 2x2 average pool straight into block2's slice 0
+        t1 = self.transition1
+        h = tape.bn_act(buf, t1.norm, table=(table, 64, GROWTH))
+        y, _ = tape.conv(h, self._spec("transition1.conv", t1.conv))
+        c0 = self.widths[1][0]
+        buf, table = self._block_buffer(tape, N, y.t.shape[1] // 2, y.t.shape[2] // 2, 2)
+        s0 = tape.prefix(buf, 0, c0, act=tape.avgpool2x2(y, out=buf.t[..., :c0]))
+        if table is not None:
+            tape.record_stats(s0, table[:2 * c0])
+        self._dense(tape, buf, table, 2, c0, 1)
+        # transition2 / transition3: BN ReLU 1x1 conv straight into slice 0 of the next block (block4's is the PSP concat)
+        m_out = self.widths[3][1]
+        for bi, dil in ((3, 2), (4, 4)):
+            tr = getattr(self, f"transition{bi - 1}")
+            prev_c0 = self.widths[bi - 2][0]
+            h = tape.bn_act(buf, tr[0], table=(table, prev_c0, GROWTH))
+            c0 = self.widths[bi - 1][0]
+            nbuf, ntable = self._block_buffer(tape, N, buf.t.shape[1], buf.t.shape[2], bi, pitch=2 * m_out if bi == 4 else None)
+            y, _ = tape.conv(h, self._spec(f"transition{bi - 1}.2", tr[2]), out=nbuf.t[..., :c0], want_stats=True,
+                             stats_out=ntable[:2 * c0] if ntable is not None else None)
+            x_aux = tape.prefix(nbuf, 0, c0, act=y)
+            buf, table = nbuf, ntable
+            self._dense(tape, buf, table, bi, c0, dil)
+        heads = []
+        if self.training and self.use_aux:
+            # recorded before the PSP head: in the backward the bottleneck's dgrad writes block4's gradient first (beta = 0),
+            # then the aux conv adds into transition3's slice
+            ab = self.auxiliary_branch
+            ya = self._cbr(tape, x_aux, "auxiliary_branch.0", ab[0], ab[1], drop_p=ab[3].p, drop_channelwise=True)
+            la, _ = tape.conv(ya, self._spec("auxiliary_branch.4", ab[4]), out_dtype=torch.float32)
+            heads.append(BilinearHead(la, False, H, W))
+        lo = self._psp_head(tape, tape.prefix(buf, 0, m_out), cat=buf)
+        return [BilinearHead(lo, False, H, W)] + heads
+
+    def get_backbone_params(self):
+        return chain(self.block0.parameters(), self.block1.parameters(), self.block2.parameters(), self.block3.parameters(),
+                     self.transition1.parameters(), self.transition2.parameters(), self.transition3.parameters())
+
+    def get_decoder_params(self):
+        return chain(self.master_branch.parameters(), self.auxiliary_branch.parameters())

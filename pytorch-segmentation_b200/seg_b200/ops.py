@@ -323,33 +323,41 @@ def bn_bwd_reduce(dout, out, x, save, relu=True, drop_p=0.0, dgamma=None, dbeta=
 
 
 def bn_apply_train(x, stats, count, gamma, beta, eps, momentum, clamp_eps, running_mean, running_var, res=None, out=None,
-                   relu=True, drop_p=0.0, seed=0, step_ctr=None, drop_hw=0, mask=None):
+                   relu=True, drop_p=0.0, seed=0, step_ctr=None, drop_hw=0, mask=None, table=None):
     """Training-mode BN (+residual, ReLU, dropout) straight from the batch sums.  Returns (out, save[2C]).
     Under SyncBN the producer called with sync= has left the world's sums in `stats`; `count` is then the world's.
-    mask (with relu): relu_mask(x) buffer, filled with the ReLU bit mask of out for the backward passes."""
+    mask (with relu): relu_mask(x) buffer, filled with the ReLU bit mask of out for the backward passes.
+    table = (c0, growth): `stats` is a dense block's statistics table (records [sum, sum^2] of width c0, then growth, back to
+    back in channel order) and x the block buffer's channel prefix [0, C)."""
     C = x.shape[-1]
     if out is None:
         out = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
     save = torch.empty(2 * C, dtype=torch.float32, device=x.device)
     assert stats.dtype == torch.float64
+    c0, growth = table if table is not None else (0, 0)
+    if table is not None:
+        assert growth > 0 and 0 < c0 <= C and (C - c0) % growth == 0, f"table {table} does not tile {C} channels"
+        assert stats.is_contiguous() and stats.numel() >= 2 * C, "statistics table too short"
     _check_mask(mask, x)
     call("seg_bn_apply_train", ptr(x), ld(x), ptr(stats), float(count), ptr(gamma), ptr(beta), float(eps), float(momentum),
          int(clamp_eps), ptr(running_mean), ptr(running_var), ptr(save), ptr(res), ld(res) if res is not None else 0,
-         ptr(out), ld(out), ptr(mask), rows(x), C, int(relu), float(drop_p), int(seed), ptr(step_ctr), int(drop_hw),
-         meta=_meta_rows(rows(x), C, (3 if res is not None else 2) + (MASK_PASS if mask is not None else 0), res is not None))
+         ptr(out), ld(out), ptr(mask), rows(x), C, int(relu), float(drop_p), int(seed), ptr(step_ctr), int(drop_hw), int(c0),
+         int(growth), meta=_meta_rows(rows(x), C, (3 if res is not None else 2) + (MASK_PASS if mask is not None else 0), res is not None))
     return out, save
 
 
 def bn_bwd_apply(dout, out, x, save, gamma, sums, count, relu=True, drop_p=0.0, dx=None, dres=None, beta_res=0.0, beta=None,
-                 mask=None):
+                 mask=None, beta_dx=0.0):
+    """beta_dx = 1: dx += the BN data gradient (fp32 sum, one bf16 rounding) instead of dx = it."""
     C = x.shape[-1]
     if dx is None:
         dx = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
+        beta_dx = 0.0
     _check_mask(mask, x)
     call("seg_bn_bwd_apply", ptr(dout), ld(dout), ptr(out), ld(out) if out is not None else 0, ptr(mask), ptr(x), ld(x), ptr(save),
          ptr(gamma), ptr(sums), float(count), rows(x), C, int(relu), float(drop_p), ptr(dx), ld(dx), ptr(dres),
-         ld(dres) if dres is not None else 0, float(beta_res), ptr(beta),
-         meta=_meta_rows(rows(x), C, 2 + _mask_passes(relu, out, mask) + 1 + (0 if dres is None else (2 if beta_res != 0.0 else 1)), dres is not None))
+         ld(dres) if dres is not None else 0, float(beta_res), ptr(beta), float(beta_dx),
+         meta=_meta_rows(rows(x), C, 2 + _mask_passes(relu, out, mask) + (2 if beta_dx else 1) + (0 if dres is None else (2 if beta_res != 0.0 else 1)), dres is not None))
     return dx
 
 
@@ -365,14 +373,16 @@ def bn_bwd_fused_workspace(M, C):
 
 
 def bn_bwd_fused(dout, out, x, save, gamma, count_total, relu=True, drop_p=0.0, dgamma=None, dbeta=None, accumulate=False,
-                 dx=None, dres=None, beta_res=0.0, beta=None, zero_sums=False, tickets=None, sync=None, mask=None):
+                 dx=None, dres=None, beta_res=0.0, beta=None, zero_sums=False, tickets=None, sync=None, mask=None, beta_dx=0.0):
     """BatchNorm backward in ONE cooperative launch (reduce -> grid barrier -> fixed-order cross-block sum [-> SyncBN exchange]
     -> apply).  Returns (dx, sums [2C]: the world's under sync).  out=None: ReLU mask recomputed from x (needs beta).  tickets:
-    bn_bwd_fused_workspace(M, C)[1] zeroed words.  mask: ReLU bit mask from bn_apply_train (read instead of out)."""
+    bn_bwd_fused_workspace(M, C)[1] zeroed words.  mask: ReLU bit mask from bn_apply_train (read instead of out).
+    beta_dx = 1: dx += the BN data gradient (fp32 sum, one bf16 rounding)."""
     C = x.shape[-1]
     M = rows(x)
     if dx is None:
         dx = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
+        beta_dx = 0.0
     sums = torch.empty(2 * C, dtype=torch.float32, device=x.device)
     nr, nt = bn_bwd_fused_workspace(M, C)
     fr = torch.empty(max(nr, 1), dtype=torch.float32, device=x.device)
@@ -382,8 +392,8 @@ def bn_bwd_fused(dout, out, x, save, gamma, count_total, relu=True, drop_p=0.0, 
     call("seg_bn_bwd_fused", ptr(dout), ld(dout), ptr(out), ld(out) if out is not None else 0, ptr(mask), ptr(x), ld(x), ptr(save), ptr(gamma),
          ptr(beta), float(count_total), M, C, int(relu), float(drop_p), ptr(sums), ptr(fr), ptr(tickets), ptr(dgamma), ptr(dbeta),
          int(accumulate), ptr(dx), ld(dx), ptr(dres), ld(dres) if dres is not None else 0, float(beta_res), int(zero_sums),
-         ctypes.addressof(sync.desc) if sync is not None else None,
-         meta=_meta_rows(M, C, (2 + _mask_passes(relu, out, mask)) * 2 + 1 + (0 if dres is None else (2 if beta_res != 0.0 else 1)), dres is not None))
+         ctypes.addressof(sync.desc) if sync is not None else None, float(beta_dx),
+         meta=_meta_rows(M, C, (2 + _mask_passes(relu, out, mask)) * 2 + (2 if beta_dx else 1) + (0 if dres is None else (2 if beta_res != 0.0 else 1)), dres is not None))
     return dx, sums
 
 
@@ -464,6 +474,28 @@ def relu_maxpool2x2_ceil_bwd(dy, code, x_shape):
     assert dy.is_contiguous() and tuple(dy.shape) == (N, (H + 1) // 2, (W + 1) // 2, C) and code.shape == dy.shape
     dx = torch.empty(x_shape, dtype=torch.bfloat16, device=dy.device)
     call("seg_relu_maxpool2x2_ceil_bwd", ptr(dy), ptr(code), ptr(dx), N, H, W, C)
+    return dx
+
+
+def avgpool2x2_fwd(x, out=None):
+    """nn.AvgPool2d(2, 2) (floor mode) of x [N,H,W,C] -> [N,H//2,W//2,C]; `out` may be a channel slice of a concat buffer."""
+    N, H, W, C = x.shape
+    if out is None:
+        out = torch.empty((N, H // 2, W // 2, C), dtype=torch.bfloat16, device=x.device)
+    assert tuple(out.shape) == (N, H // 2, W // 2, C)
+    call("seg_avgpool2x2_fwd", ptr(x), ld(x), ptr(out), ld(out), N, H, W, C, meta=_meta_rows(N * H * W, C, 1.25))
+    return out
+
+
+def avgpool2x2_bwd(dy, x_shape, dx=None, beta=0.0):
+    """dx = beta * dx + the pool's data gradient over every element of dx (0 for a dropped odd row / column)."""
+    N, H, W, C = x_shape
+    assert tuple(dy.shape) == (N, H // 2, W // 2, C)
+    if dx is None:
+        dx = torch.empty(x_shape, dtype=torch.bfloat16, device=dy.device)
+        beta = 0.0
+    call("seg_avgpool2x2_bwd", ptr(dy), ld(dy), ptr(dx), ld(dx), N, H, W, C, float(beta),
+         meta=_meta_rows(N * H * W, C, 1.25 + (1 if beta else 0)))
     return dx
 
 
