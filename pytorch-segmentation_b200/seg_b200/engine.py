@@ -196,6 +196,70 @@ class Tape:
             self.back_params[len(self.back)] = tuple(p for p in params if p is not None)
         self.back.append(fn)
 
+    def _unary_back(self, x, ya, fn, sole=None):
+        """Record the backward of an op whose one input is x and whose output is ya (nothing when not recording), in one of
+        two forms.  Accumulating (sole None): fn(dy, gx, beta) writes (beta = 0) or adds (beta = 1) x's gradient into
+        x.grad_target().  Sole writer (sole = the op's name): x must have no other consumer; fn(dy) returns x's whole
+        gradient, and later writers accumulate into it."""
+        if not self.record:
+            return
+
+        def bwd():
+            if ya.grad is None or not x.needs_grad:
+                return
+            if sole is None:
+                gx, beta = x.grad_target()
+                fn(ya.grad, gx, beta)
+            else:
+                assert x.grad is None, f"{sole} input must have a single consumer"
+                x.grad = fn(ya.grad)
+                x._written = True
+            ya.grad = None
+        self.back.append(bwd)
+
+    def _drop_seed(self, drop_p):
+        """(drop_p, seed) of a dropout: none outside training or with the engine's dropout off; each dropout that draws takes
+        the next seed of the tape's sequence (the kernels mix in the device step counter)."""
+        if not (self.training and self.dropout):
+            drop_p = 0.0
+        if not drop_p > 0.0:
+            return drop_p, 0
+        self._drop_ctr += 1
+        return drop_p, (self.seed * 1000003 + self._drop_ctr * 7919) & 0x7FFFFFFFFFFFFFFF
+
+    def _bias_grad(self, bias, dy):
+        """Bias gradient = column sums of dY (fp64 accumulation); a channel count off the 8-lane pitch is read at its pitch."""
+        if bias is None or not bias.requires_grad:
+            return
+        C, cpad = dy.shape[-1], ops.ld(dy)
+        wide = dy if C % 8 == 0 else dy.as_strided(dy.shape[:-1] + (cpad,), dy.stride(), dy.storage_offset())
+        s = ops.bn_stats(wide)[:C].float()
+        self._param_grad(bias, lambda g, beta: g.add_(s) if beta else g.copy_(s))
+
+    def _weight_grad(self, spec, a, b, geo, impl):
+        """spec's weight gradient, conv2d_wgrad(a, b, *geo): into the trainer's persistent packed-gradient buffer (unpacked
+        once per step, batched) when it has one, else unpacked into the parameter's fp32 gradient."""
+        w = spec.m.weight
+        if not w.requires_grad:
+            return
+        if spec in self.dw_buffers:
+            ops.conv2d_wgrad(a, b, *geo, out=self.dw_buffers[spec], impl=impl)
+            self.touched.add(w)
+            return
+        dwp = ops.conv2d_wgrad(a, b, *geo, impl=impl)
+        if spec.explicit:
+            def fill(g, beta):
+                # packed [1][K][Kpad] -> [K][R,S,C] -> OIHW
+                full = dwp[0, :, : spec.R * spec.S * spec.C].reshape(spec.K, spec.R, spec.S, spec.C).permute(0, 3, 1, 2)
+                if beta:
+                    g.add_(full)
+                else:
+                    g.copy_(full)
+        else:
+            def fill(g, beta):
+                ops.unpack_wgrad(dwp, tuple(w.shape), beta=beta, out=g)
+        self._param_grad(w, fill)
+
     def backward(self, after=None):
         """Replay the recorded closures in reverse.  after(i): called when closure i (and everything recorded after it) has
         run — the fused train step uses it to launch a gradient bucket's all-reduce as soon as the bucket is complete."""
@@ -249,33 +313,11 @@ class Tape:
                 dy = ya.grad
                 if dy is None:
                     return
-                R, S, stride, pad, dil = geo
-                if spec.m.weight.requires_grad and spec in self.dw_buffers:
-                    # accumulate into the trainer's persistent packed-gradient buffer; unpacked once per step, batched
-                    ops.conv2d_wgrad(dy, xin, R, S, stride, pad, dil, out=self.dw_buffers[spec], impl=self.impl)
-                    self.touched.add(spec.m.weight)
-                elif spec.m.weight.requires_grad:
-                    dwp = ops.conv2d_wgrad(dy, xin, R, S, stride, pad, dil, impl=self.impl)
-                    if spec.explicit:
-                        def fill(g, beta):
-                            # packed [1][K][Kpad] -> [K][R,S,C] -> OIHW
-                            full = dwp[0, :, : spec.R * spec.S * spec.C].reshape(spec.K, spec.R, spec.S, spec.C).permute(0, 3, 1, 2)
-                            if beta:
-                                g.add_(full)
-                            else:
-                                g.copy_(full)
-                    else:
-                        def fill(g, beta):
-                            ops.unpack_wgrad(dwp, tuple(spec.m.weight.shape), beta=beta, out=g)
-                    self._param_grad(spec.m.weight, fill)
-                if bias is not None and bias.requires_grad:
-                    cpad = ops.ld(dy)
-                    wide = dy if dy.shape[-1] % 8 == 0 else dy.as_strided(dy.shape[:-1] + (cpad,), dy.stride(), dy.storage_offset())
-                    s = ops.bn_stats(wide)[: spec.K].float()  # column sums of dY (fp64 accumulation)
-                    self._param_grad(bias, lambda g, beta: g.add_(s) if beta else g.copy_(s))
+                self._weight_grad(spec, dy, xin, geo, self.impl)
+                self._bias_grad(bias, dy)
                 if (not spec.explicit) and isinstance(x, Act) and x.needs_grad:
                     gx, beta = x.grad_target()
-                    ops.conv2d_dgrad(dy, wp, tuple(x.t.shape), R, S, stride, pad, dil, out=gx, beta=beta, impl=self.impl)
+                    ops.conv2d_dgrad(dy, wp, tuple(x.t.shape), *geo, out=gx, beta=beta, impl=self.impl)
                 elif isinstance(x, Act) and x.needs_grad:
                     # 1x1 im2col conv (C % 8 != 0, e.g. DUC_out.conv over the class scores): the columns are the input padded
                     # to Kpad channels, so the dgrad over the columns is the data gradient; its pad lanes are zero because the
@@ -308,12 +350,7 @@ class Tape:
                 dy = ya.grad
                 if dy is None:
                     return
-                if spec.m.weight.requires_grad and spec in self.dw_buffers:
-                    ops.conv2d_wgrad(x.t, dy, k, k, s, p, 1, out=self.dw_buffers[spec], impl=impl)
-                    self.touched.add(spec.m.weight)
-                elif spec.m.weight.requires_grad:
-                    dwp = ops.conv2d_wgrad(x.t, dy, k, k, s, p, 1, impl=impl)
-                    self._param_grad(spec.m.weight, lambda g, beta: ops.unpack_wgrad(dwp, tuple(spec.m.weight.shape), beta=beta, out=g))
+                self._weight_grad(spec, x.t, dy, (k, k, s, p, 1), impl)
                 if x.needs_grad:
                     gx, beta = x.grad_target()
                     ops.conv2d_fwd(dy, wp, spec.K, k, k, s, p, 1, out=gx, beta=beta, impl=impl)
@@ -349,14 +386,7 @@ class Tape:
     def relu(self, x):
         y = ops.relu_fwd(x.t)
         ya = Act(y)
-        if self.record:
-            def bwd():
-                if ya.grad is None or not x.needs_grad:
-                    return
-                gx, beta = x.grad_target()
-                ops.relu_bwd(ya.grad, y, gx, beta)
-                ya.grad = None
-            self.back.append(bwd)
+        self._unary_back(x, ya, lambda dy, gx, beta: ops.relu_bwd(dy, y, gx, beta))
         return ya
 
     # ------------------------------------------------------------------ dense-block statistics table
@@ -389,14 +419,7 @@ class Tape:
         C = y.t.shape[-1]
         count_local = ops.rows(y.t)
         use_batch_stats = self.training and bn.training
-        if self.training and not (self.dropout):
-            drop_p = 0.0
-        if not self.training:
-            drop_p = 0.0
-        seed = 0
-        if drop_p > 0.0:
-            self._drop_ctr += 1
-            seed = (self.seed * 1000003 + self._drop_ctr * 7919) & 0x7FFFFFFFFFFFFFFF  # + step counter on the device
+        drop_p, seed = self._drop_seed(drop_p)
         # conv -> BN(batch statistics) -> ReLU with nothing in between: the ReLU mask can be recomputed from the conv output
         # with the forward's own coefficients instead of being read (the one-launch backward of the small maps does so)
         remask = bool(use_batch_stats and relu and res is None and drop_p == 0.0)
@@ -499,16 +522,10 @@ class Tape:
 
     # ------------------------------------------------------------------ pooling / resize / concat
     def maxpool(self, x):
+        """nn.MaxPool2d(3, 2, 1) of a ResNet stem.  x must be the pool's only consumer."""
         y, idx = ops.maxpool3x3s2_fwd(x.t)
         ya = Act(y)
-        if self.record:
-            def bwd():
-                if ya.grad is None or not x.needs_grad:
-                    return
-                assert x.grad is None, "maxpool input must have a single consumer"
-                x.grad = ops.maxpool3x3s2_bwd(ya.grad, idx, tuple(x.t.shape))
-                ya.grad = None
-            self.back.append(bwd)
+        self._unary_back(x, ya, lambda dy: ops.maxpool3x3s2_bwd(dy, idx, tuple(x.t.shape)), sole="maxpool")
         return ya
 
     def maxpool2x2(self, x):
@@ -516,15 +533,7 @@ class Tape:
         codes and the pre-pool shape, for `maxunpool2x2`.  x must be the pool's only consumer (as in SegNet)."""
         y, code = ops.maxpool2x2_fwd(x.t)
         ya = Act(y)
-        if self.record:
-            def bwd():
-                if ya.grad is None or not x.needs_grad:
-                    return
-                assert x.grad is None, "maxpool2x2 input must have a single consumer"
-                x.grad = ops.maxpool2x2_bwd(ya.grad, code, tuple(x.t.shape))
-                x._written = True
-                ya.grad = None
-            self.back.append(bwd)
+        self._unary_back(x, ya, lambda dy: ops.maxpool2x2_bwd(dy, code, tuple(x.t.shape)), sole="maxpool2x2")
         return ya, (code, tuple(x.t.shape))
 
     def maxunpool2x2(self, x, record):
@@ -533,15 +542,7 @@ class Tape:
         code, shape = record
         y = ops.maxunpool2x2_fwd(x.t, code, shape[1:3])
         ya = Act(y)
-        if self.record:
-            def bwd():
-                if ya.grad is None or not x.needs_grad:
-                    return
-                assert x.grad is None, "maxunpool2x2 input must have a single consumer"
-                x.grad = ops.maxunpool2x2_bwd(ya.grad, code)
-                x._written = True
-                ya.grad = None
-            self.back.append(bwd)
+        self._unary_back(x, ya, lambda dy: ops.maxunpool2x2_bwd(dy, code), sole="maxunpool2x2")
         return ya
 
     def relu_maxpool_ceil(self, x):
@@ -549,36 +550,16 @@ class Tape:
         kernel each way; the backward writes every element of x's gradient.  x must be the pool's only consumer."""
         y, code = ops.relu_maxpool2x2_ceil_fwd(x.t)
         ya = Act(y)
-        if self.record:
-            def bwd():
-                if ya.grad is None or not x.needs_grad:
-                    return
-                assert x.grad is None, "relu_maxpool_ceil input must have a single consumer"
-                x.grad = ops.relu_maxpool2x2_ceil_bwd(ya.grad, code, tuple(x.t.shape))
-                x._written = True
-                ya.grad = None
-            self.back.append(bwd)
+        self._unary_back(x, ya, lambda dy: ops.relu_maxpool2x2_ceil_bwd(dy, code, tuple(x.t.shape)), sole="relu_maxpool_ceil")
         return ya
 
     def relu_dropout(self, x, drop_p):
         """F.relu then nn.Dropout(drop_p) (FCN8's conv6 / conv7, fcn.py:49-51); a plain ReLU outside training or with the
         engine's dropout off.  Masks: bn_act's seed sequence and the device step counter."""
-        if not (self.training and self.dropout):
-            drop_p = 0.0
-        seed = 0
-        if drop_p > 0.0:
-            self._drop_ctr += 1
-            seed = (self.seed * 1000003 + self._drop_ctr * 7919) & 0x7FFFFFFFFFFFFFFF
+        drop_p, seed = self._drop_seed(drop_p)
         y = ops.relu_dropout_fwd(x.t, drop_p, seed, self.step_ctr if drop_p > 0.0 else None)
         ya = Act(y)
-        if self.record:
-            def bwd():
-                if ya.grad is None or not x.needs_grad:
-                    return
-                gx, beta = x.grad_target()
-                ops.relu_dropout_bwd(ya.grad, y, drop_p, gx, beta)
-                ya.grad = None
-            self.back.append(bwd)
+        self._unary_back(x, ya, lambda dy, gx, beta: ops.relu_dropout_bwd(dy, y, drop_p, gx, beta))
         return ya
 
     def score_upsample(self, x, up, window, skip=None, skip_off=(0, 0), alpha=0.0, bias=None, out_dtype=None):
@@ -601,11 +582,7 @@ class Tape:
                 dy = ya.grad
                 if dy is None:
                     return
-                if bias is not None and bias.requires_grad:
-                    C = dy.shape[-1]
-                    wide = dy if C % 8 == 0 else dy.as_strided(dy.shape[:-1] + (ops.ld(dy),), dy.stride(), dy.storage_offset())
-                    s = ops.bn_stats(wide)[:C].float()  # column sums of dY (fp64 accumulation), as Tape.conv's bias gradient
-                    self._param_grad(bias, lambda g, beta: g.add_(s) if beta else g.copy_(s))
+                self._bias_grad(bias, dy)
                 if skip is not None and skip.needs_grad:
                     assert skip.grad is None, "score_upsample skip must have a single consumer"
                     skip.grad = ops.score_skip_bwd(dy, tuple(skip.t.shape), skip_off, alpha)
@@ -622,40 +599,20 @@ class Tape:
         """nn.AvgPool2d(2, 2), floor mode (DenseNet's transition1), into `out` (a channel slice of the next block's buffer)."""
         y = ops.avgpool2x2_fwd(x.t, out=out)
         ya = Act(y)
-        if self.record:
-            def bwd():
-                if ya.grad is None or not x.needs_grad:
-                    return
-                gx, beta = x.grad_target()
-                ops.avgpool2x2_bwd(ya.grad, tuple(x.t.shape), dx=gx, beta=beta)
-                ya.grad = None
-            self.back.append(bwd)
+        self._unary_back(x, ya, lambda dy, gx, beta: ops.avgpool2x2_bwd(dy, tuple(x.t.shape), dx=gx, beta=beta))
         return ya
 
     def avgpool(self, x, bins):
         y = ops.adaptive_avgpool_fwd(x.t, bins)
         ya = Act(y)
-        if self.record:
-            def bwd():
-                if ya.grad is None or not x.needs_grad:
-                    return
-                gx, beta = x.grad_target()
-                ops.adaptive_avgpool_bwd(ya.grad, tuple(x.t.shape), bins, dx=gx, beta=beta)
-                ya.grad = None
-            self.back.append(bwd)
+        self._unary_back(x, ya, lambda dy, gx, beta: ops.adaptive_avgpool_bwd(dy, tuple(x.t.shape), bins, dx=gx, beta=beta))
         return ya
 
     def bilinear(self, x, Ho, Wo, align_corners, out=None):
         y = ops.bilinear_fwd(x.t, Ho, Wo, align_corners, out=out)
         ya = Act(y)
-        if self.record:
-            def bwd():
-                if ya.grad is None or not x.needs_grad:
-                    return
-                gx, beta = x.grad_target()
-                ops.bilinear_bwd(ya.grad, x.t.shape[1], x.t.shape[2], align_corners, dx=gx, beta=beta)
-                ya.grad = None
-            self.back.append(bwd)
+        self._unary_back(x, ya, lambda dy, gx, beta: ops.bilinear_bwd(dy, x.t.shape[1], x.t.shape[2], align_corners, dx=gx,
+                                                                      beta=beta))
         return ya
 
     def pixel_shuffle(self, x, r, out=None, crop=None):
@@ -664,14 +621,7 @@ class Tape:
         Ho, Wo = crop if crop is not None else (H * r, W * r)
         y = ops.pixel_shuffle_fwd(x.t, r, Ho, Wo, out=out)
         ya = Act(y)
-        if self.record:
-            def bwd():
-                if ya.grad is None or not x.needs_grad:
-                    return
-                gx, beta = x.grad_target()
-                ops.pixel_shuffle_bwd(ya.grad, r, H, W, dx=gx, beta=beta)
-                ya.grad = None
-            self.back.append(bwd)
+        self._unary_back(x, ya, lambda dy, gx, beta: ops.pixel_shuffle_bwd(dy, r, H, W, dx=gx, beta=beta))
         return ya
 
     def up_add(self, x, y):
@@ -699,14 +649,7 @@ class Tape:
         """Copy an activation into a concat slice (used when the producer's tensor is also consumed elsewhere)."""
         ops.axpby(x.t, out, 0.0)
         ya = Act(out)
-        if self.record:
-            def bwd():
-                if ya.grad is None or not x.needs_grad:
-                    return
-                gx, beta = x.grad_target()
-                ops.axpby(ya.grad, gx, beta)
-                ya.grad = None
-            self.back.append(bwd)
+        self._unary_back(x, ya, lambda dy, gx, beta: ops.axpby(dy, gx, beta))
         return ya
 
     def concat(self, N, H, W, channels, device):

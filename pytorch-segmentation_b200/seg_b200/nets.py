@@ -122,6 +122,67 @@ def _res_layers(blocks, inplanes, plan):
     return layers
 
 
+def _stem7(in_channels, stride=2):
+    """torchvision ResNet stem holder: 7x7 conv (64) - BN - ReLU - 3x3/2 max-pool."""
+    c, n = nn.Conv2d(in_channels, 64, 7, stride=stride, padding=3, bias=False), nn.BatchNorm2d(64)
+    return nn.Sequential(c, n, nn.ReLU(inplace=True), nn.MaxPool2d(kernel_size=3, stride=2, padding=1))
+
+
+def _deep_stem():
+    """Deep stem holder (resnet.py:137-151): [3x3/2 conv-BN-ReLU, 3x3 conv-BN-ReLU, 3x3 conv to 128], its BN, ReLU, 3x3/2
+    max-pool."""
+    s1, n1 = _cbn(3, 64, 3, 2, 1)
+    s2, n2 = _cbn(64, 64, 3, 1, 1)
+    s3 = nn.Conv2d(64, 128, 3, stride=1, padding=1, bias=False)
+    stem = nn.Sequential(s1, n1, nn.ReLU(inplace=True), s2, n2, nn.ReLU(inplace=True), s3)
+    return nn.Sequential(stem, nn.BatchNorm2d(128), nn.ReLU(inplace=True), nn.MaxPool2d(kernel_size=3, stride=2, padding=1))
+
+
+def _psp_module(m, bins, out):
+    """_PSPModule holder (pspnet.py:11-38, upernet.py:9-38): per bin an adaptive average pool and a 1x1 conv-BN-ReLU to m // 4
+    channels; the bottleneck, a 3x3 conv-BN-ReLU-Dropout2d(0.1) from the 2m-channel concat to `out` channels."""
+    psp = _Holder()
+    stages = []
+    for b in bins:
+        c, n = _cbn(m, m // 4, 1)
+        stages.append(nn.Sequential(nn.AdaptiveAvgPool2d(output_size=b), c, n, nn.ReLU(inplace=True)))
+    psp.stages = nn.ModuleList(stages)
+    c, n = _cbn(m * 2, out, 3)
+    psp.bottleneck = nn.Sequential(c, n, nn.ReLU(inplace=True), nn.Dropout2d(0.1))
+    return psp
+
+
+def _psp_branches(m, aux_in, num_classes):
+    """PSPNet's (master_branch, auxiliary_branch) (pspnet.py:59-70): the PSP module (bins 1, 2, 3, 6) over the m-channel
+    trunk output + a 1x1 classifier; a 3x3 conv-BN-ReLU-Dropout2d(0.1) over the aux_in-channel aux features + a 1x1
+    classifier."""
+    master = nn.Sequential(_psp_module(m, (1, 2, 3, 6), m // 4), nn.Conv2d(m // 4, num_classes, kernel_size=1))
+    c, n = _cbn(aux_in, m // 4, 3)
+    aux = nn.Sequential(c, n, nn.ReLU(inplace=True), nn.Dropout2d(0.1), nn.Conv2d(m // 4, num_classes, kernel_size=1))
+    return master, aux
+
+
+def _aspp_module(dilations):
+    """ASSP holder (deeplabv3_plus.py:260-284, duc_hdc.py:126-155) over the 2048-channel trunk output: per dilation a
+    256-channel conv-BN-ReLU branch (1x1 for the first, 3x3 dilated for the others), image pooling, and the 1x1
+    conv-BN-ReLU-Dropout(0.5) over the concat."""
+    a = _Holder()
+    for i, d in enumerate(dilations, 1):
+        c, n = _cbn(2048, 256, 1 if i == 1 else 3, 1, d)
+        setattr(a, f"aspp{i}", nn.Sequential(c, n, nn.ReLU(inplace=True)))
+    c, n = _cbn(2048, 256, 1)
+    a.avg_pool = nn.Sequential(nn.AdaptiveAvgPool2d((1, 1)), c, n, nn.ReLU(inplace=True))
+    a.conv1, a.bn1 = _cbn(256 * (len(dilations) + 1), 256, 1)
+    a.relu, a.dropout = nn.ReLU(inplace=True), nn.Dropout(0.5)
+    return a
+
+
+def _freeze(params):
+    """freeze_backbone: the parameters stop receiving gradients."""
+    for p in params:
+        p.requires_grad = False
+
+
 def _sepconv(cin, cout, stride, dil):
     """SeparableConv2d holder (deeplabv3_plus.py:70-86): depthwise 3x3 'same' conv -> BN -> pointwise 1x1."""
     s = _Holder()
@@ -322,6 +383,8 @@ class _GraphFn(torch.autograd.Function):
 class _EngineModel(BaseModel):
     """Shared plumbing: spec cache, engine options, forward entry."""
 
+    IM2COL_CONV = None  # the conv that reads the network input (NCHW fp32, any channel count) through the explicit im2col
+
     def __init__(self):
         super().__init__()
         self._specs = {}
@@ -483,7 +546,7 @@ class _EngineModel(BaseModel):
     def _spec(self, name, module):
         s = self._specs.get(name)
         if s is None or s.m is not module:
-            s = ConvSpec(name, module)
+            s = ConvSpec(name, module, explicit_im2col=(name == self.IM2COL_CONV))
             self._specs[name] = s
         return s
 
@@ -562,9 +625,71 @@ class _EngineModel(BaseModel):
             r = self._cbr(tape, x, prefix + "downsample.0", blk.downsample[0], blk.downsample[1], relu=False)
         return self._cbr(tape, a, prefix + "conv3", blk.conv3, blk.bn3, relu=True, res=r, out=out)
 
+    def _stem(self, tape, x, name, stem):
+        """A ResNet stem holder (`_stem7` or `_deep_stem`) at `name`: its conv-BN-ReLU units, then the 3x3/2 max-pool."""
+        if isinstance(stem[0], nn.Sequential):  # deep stem: the third conv's BN is the outer holder's
+            s = stem[0]
+            for i, bn in ((0, s[1]), (3, s[4]), (6, stem[1])):
+                x = self._cbr(tape, x, f"{name}.0.{i}", s[i], bn)
+        else:
+            x = self._cbr(tape, x, f"{name}.0", stem[0], stem[1])
+        return tape.maxpool(x)
+
+    def _trunk(self, tape, x, prefix, stem):
+        """ResNet trunk: the stem holder `stem` and layer1..4, attributes of the module at `prefix` ("" = the model); returns
+        the four layer outputs."""
+        owner = self.get_submodule(prefix.rstrip(".")) if prefix else self
+        a = self._stem(tape, x, prefix + stem, getattr(owner, stem))
+        feats = []
+        for li in (1, 2, 3, 4):
+            for bi, blk in enumerate(getattr(owner, f"layer{li}")):
+                a = self._block(tape, a, f"{prefix}layer{li}.{bi}.", blk)
+            feats.append(a)
+        return feats
+
+    def _ppm(self, tape, a, psp, prefix, cat=None):
+        """_PSPModule.forward (pspnet.py:31-38, upernet.py:31-38) of the `_psp_module` holder `psp` at `prefix`: cat([a, one
+        stage per bin]) -> bottleneck; returns the bottleneck's output.  a: the trunk output (m channels; stages of m // 4).
+        cat: a `dense_buffer` of 2m channels whose first m the trunk wrote in place (PSPDenseNet's block4); otherwise the
+        concat is allocated here and a, which is also the residual stream's tensor, is copied into slice 0."""
+        N, Hf, Wf, m = a.t.shape
+        q = m // 4
+        if cat is None:
+            cat, sl = tape.concat(N, Hf, Wf, [m, q, q, q, q], a.t.device)
+            feats = tape.copy_into(a, sl[0])
+        else:
+            sl = [cat.t[..., :m]] + [cat.t[..., m + i * q:m + (i + 1) * q] for i in range(4)]
+            feats = a
+        br = [feats]
+        for i, st in enumerate(psp.stages):
+            p = tape.avgpool(a, st[0].output_size)
+            p = self._cbr(tape, p, f"{prefix}.stages.{i}.1", st[1], st[2])
+            br.append(tape.bilinear(p, Hf, Wf, True, out=sl[i + 1]))
+        tape.bind_slices(cat, br)
+        b = psp.bottleneck
+        return self._cbr(tape, cat, f"{prefix}.bottleneck.0", b[0], b[1], drop_p=b[3].p, drop_channelwise=True)
+
+    def _aspp(self, tape, a):
+        """ASSP.forward (deeplabv3_plus.py:286-297, duc_hdc.py:157-174) of the `_aspp_module` holder `ASSP`: every dilated
+        branch and the image pooling written straight into one concat buffer, then the 1x1 fusion conv."""
+        N, Hf, Wf = a.t.shape[0], a.t.shape[1], a.t.shape[2]
+        A = self.ASSP
+        branches = [seq for name, seq in A.named_children() if name.startswith("aspp")]
+        cat, sl = tape.concat(N, Hf, Wf, [256] * (len(branches) + 1), a.t.device)
+        br = [self._cbr(tape, a, f"ASSP.aspp{i + 1}.0", seq[0], seq[1], out=sl[i]) for i, seq in enumerate(branches)]
+        g = tape.avgpool(a, 1)
+        g = self._cbr(tape, g, "ASSP.avg_pool.1", A.avg_pool[1], A.avg_pool[2])
+        br.append(tape.bilinear(g, Hf, Wf, True, out=sl[-1]))
+        tape.bind_slices(cat, br)
+        return self._cbr(tape, cat, "ASSP.conv1", A.conv1, A.bn1, drop_p=A.dropout.p)
+
     def _finish(self, tape):
-        if tape.bn_modules:
-            torch._foreach_add_([m.num_batches_tracked for m in tape.bn_modules], 1)
+        # one count per normalisation: a BN applied twice in a step (PSPDenseNet's block0.4) advances by 2, as the reference's
+        counts = {}
+        for m in tape.bn_modules:
+            counts[m] = counts.get(m, 0) + 1
+        for k in sorted(set(counts.values())):
+            torch._foreach_add_([m.num_batches_tracked for m, c in counts.items() if c == k], k)
 
     def _dp_world(self):
         """Data-parallel replicas taking part in this model's backward (1 = no exchange)."""
@@ -636,42 +761,26 @@ class DeepLab(_EngineModel):
             del self.ASSP, self.decoder
             self.ASSP, self.decoder = assp, dec
             _init_like_reference_head(self.backbone, self.ASSP, self.decoder)
-            if freeze_bn:
-                self.freeze_bn()
-            if freeze_backbone:
-                for p in self.backbone.parameters():
-                    p.requires_grad = False
-            return
-        # deeplabv3_plus.py:35-53: os16 -> layer3 stride 2, layer4 every conv2 d=2 ; os8 -> layer3 d=2, layer4 d=4
-        if output_stride == 16:
-            plan = [(1, 1, 1), (2, 1, 1), (2, 1, 1), (1, 2, 2)]
         else:
-            plan = [(1, 1, 1), (2, 1, 1), (1, 2, 2), (1, 4, 4)]
-        bb = _Holder()
-        c0, b0 = nn.Conv2d(in_channels, 64, 7, stride=2, padding=3, bias=False), nn.BatchNorm2d(64)
-        bb.layer0 = nn.Sequential(c0, b0, nn.ReLU(inplace=True), nn.MaxPool2d(kernel_size=3, stride=2, padding=1))
-        bb.layer1, bb.layer2, bb.layer3, bb.layer4 = _res_layers(RESNET_BLOCKS[backbone], 64, plan)
-        self.backbone = bb
-        self._build_heads(num_classes, output_stride, low_level_channels=256)
-        _init_like_torchvision_trunk(bb.layer1, bb.layer2, bb.layer3, bb.layer4)
-        _init_like_reference_head(bb.layer0, self.ASSP, self.decoder)
+            # deeplabv3_plus.py:35-53: os16 -> layer3 stride 2, layer4 every conv2 d=2 ; os8 -> layer3 d=2, layer4 d=4
+            if output_stride == 16:
+                plan = [(1, 1, 1), (2, 1, 1), (2, 1, 1), (1, 2, 2)]
+            else:
+                plan = [(1, 1, 1), (2, 1, 1), (1, 2, 2), (1, 4, 4)]
+            bb = _Holder()
+            bb.layer0 = _stem7(in_channels)
+            bb.layer1, bb.layer2, bb.layer3, bb.layer4 = _res_layers(RESNET_BLOCKS[backbone], 64, plan)
+            self.backbone = bb
+            self._build_heads(num_classes, output_stride, low_level_channels=256)
+            _init_like_torchvision_trunk(bb.layer1, bb.layer2, bb.layer3, bb.layer4)
+            _init_like_reference_head(bb.layer0, self.ASSP, self.decoder)
         if freeze_bn:
             self.freeze_bn()
         if freeze_backbone:
-            for p in self.backbone.parameters():
-                p.requires_grad = False
+            _freeze(self.backbone.parameters())
 
     def _build_heads(self, num_classes, output_stride, low_level_channels):
-        dil = (1, 6, 12, 18) if output_stride == 16 else (1, 12, 24, 36)
-        a = _Holder()
-        for i, k in zip((1, 2, 3, 4), (1, 3, 3, 3)):
-            c, n = _cbn(2048, 256, k, 1, dil[i - 1])
-            setattr(a, f"aspp{i}", nn.Sequential(c, n, nn.ReLU(inplace=True)))
-        c, n = _cbn(2048, 256, 1)
-        a.avg_pool = nn.Sequential(nn.AdaptiveAvgPool2d((1, 1)), c, n, nn.ReLU(inplace=True))
-        a.conv1, a.bn1 = _cbn(256 * 5, 256, 1)
-        a.relu, a.dropout = nn.ReLU(inplace=True), nn.Dropout(0.5)
-        self.ASSP = a
+        self.ASSP = _aspp_module((1, 6, 12, 18) if output_stride == 16 else (1, 12, 24, 36))
         d = _Holder()
         d.conv1, d.bn1 = _cbn(low_level_channels, 48, 1)
         d.relu = nn.ReLU(inplace=True)
@@ -695,34 +804,6 @@ class DeepLab(_EngineModel):
             a = self._sep_unit(tape, a, f"backbone.conv{n}", getattr(bb, f"conv{n}"), getattr(bb, f"bn{n}"), relu_after=True)
         return a, low
 
-    def _trunk_resnet(self, tape, x):
-        bb = self.backbone
-        a = self._cbr(tape, x, "backbone.layer0.0", bb.layer0[0], bb.layer0[1])
-        a = tape.maxpool(a)
-        low = None
-        for li in (1, 2, 3, 4):
-            layer = getattr(bb, f"layer{li}")
-            for bi, blk in enumerate(layer):
-                a = self._block(tape, a, f"backbone.layer{li}.{bi}.", blk)
-            if li == 1:
-                low = a
-        return a, low
-
-    def _aspp(self, tape, a):
-        """ASSP.forward (deeplabv3_plus.py:286-297): five branches written straight into one 1280-channel buffer."""
-        N, Hf, Wf = a.t.shape[0], a.t.shape[1], a.t.shape[2]
-        A = self.ASSP
-        cat, sl = tape.concat(N, Hf, Wf, [256] * 5, a.t.device)
-        br = []
-        for i in (1, 2, 3, 4):
-            seq = getattr(A, f"aspp{i}")
-            br.append(self._cbr(tape, a, f"ASSP.aspp{i}.0", seq[0], seq[1], out=sl[i - 1]))
-        g = tape.avgpool(a, 1)
-        g = self._cbr(tape, g, "ASSP.avg_pool.1", A.avg_pool[1], A.avg_pool[2])
-        br.append(tape.bilinear(g, Hf, Wf, True, out=sl[4]))
-        tape.bind_slices(cat, br)
-        return self._cbr(tape, cat, "ASSP.conv1", A.conv1, A.bn1, drop_p=A.dropout.p)
-
     def _decoder(self, tape, f, low):
         """Decoder.forward (deeplabv3_plus.py:323-330): concat order (low-level 48, upsampled 256); returns the fp32
         stride-4 logits Act."""
@@ -738,7 +819,10 @@ class DeepLab(_EngineModel):
         return lo
 
     def _features(self, tape, x):
-        a, low = self._trunk_xception(tape, x) if self.backbone_name == "xception" else self._trunk_resnet(tape, x)
+        if self.backbone_name == "xception":
+            a, low = self._trunk_xception(tape, x)
+        else:
+            low, _, _, a = self._trunk(tape, x, "backbone.", "layer0")
         return self._decoder(tape, self._aspp(tape, a), low)
 
     def _forward_heads(self, tape, x):
@@ -765,50 +849,20 @@ class PSPNet(_EngineModel):
         if in_channels != 3:
             raise NotImplementedError("in_channels != 3 swaps the deep stem for a 7x7 conv (pspnet.py:50-51); not built")
         self.num_classes, self.use_aux = num_classes, use_aux
-        s1, n1 = _cbn(3, 64, 3, 2, 1)
-        s2, n2 = _cbn(64, 64, 3, 1, 1)
-        s3 = nn.Conv2d(64, 128, 3, stride=1, padding=1, bias=False)
-        stem = nn.Sequential(s1, n1, nn.ReLU(inplace=True), s2, n2, nn.ReLU(inplace=True), s3)
-        self.initial = nn.Sequential(stem, nn.BatchNorm2d(128), nn.ReLU(inplace=True), nn.MaxPool2d(kernel_size=3, stride=2, padding=1))
+        self.initial = _deep_stem()
         # resnet.py:154-163,190-210: layer3 = [d1, d2, ...], layer4 = [d2, d4, ...], all stride 1 (output stride 8)
         plan = [(1, 1, 1), (2, 1, 1), (1, 1, 2), (1, 2, 4)]
         self.layer1, self.layer2, self.layer3, self.layer4 = _res_layers(RESNET_BLOCKS[backbone], 128, plan)
-        m_out = 2048
-        psp = _Holder()
-        stages = []
-        for b in (1, 2, 3, 6):
-            c, n = _cbn(m_out, m_out // 4, 1)
-            stages.append(nn.Sequential(nn.AdaptiveAvgPool2d(output_size=b), c, n, nn.ReLU(inplace=True)))
-        psp.stages = nn.ModuleList(stages)
-        c, n = _cbn(m_out * 2, m_out // 4, 3)
-        psp.bottleneck = nn.Sequential(c, n, nn.ReLU(inplace=True), nn.Dropout2d(0.1))
-        self.master_branch = nn.Sequential(psp, nn.Conv2d(m_out // 4, num_classes, kernel_size=1))
-        c, n = _cbn(m_out // 2, m_out // 4, 3)
-        self.auxiliary_branch = nn.Sequential(c, n, nn.ReLU(inplace=True), nn.Dropout2d(0.1),
-                                              nn.Conv2d(m_out // 4, num_classes, kernel_size=1))
-        self.bins = (1, 2, 3, 6)
+        self.master_branch, self.auxiliary_branch = _psp_branches(2048, 1024, num_classes)
         _init_like_resnet_s(self.initial, self.layer1, self.layer2, self.layer3, self.layer4)
         _init_like_reference_head(self.master_branch, self.auxiliary_branch)
         if freeze_bn:
             self.freeze_bn()
         if freeze_backbone:
-            for m in (self.initial, self.layer1, self.layer2, self.layer3, self.layer4):
-                for p in m.parameters():
-                    p.requires_grad = False
+            _freeze(self.get_backbone_params())
 
     def _forward_heads(self, tape, x):
-        N = x.shape[0]
-        stem = self.initial[0]
-        a = self._cbr(tape, x, "initial.0.0", stem[0], stem[1])
-        a = self._cbr(tape, a, "initial.0.3", stem[3], stem[4])
-        a = self._cbr(tape, a, "initial.0.6", stem[6], self.initial[1])
-        a = tape.maxpool(a)
-        x_aux = None
-        for li in (1, 2, 3, 4):
-            for bi, blk in enumerate(getattr(self, f"layer{li}")):
-                a = self._block(tape, a, f"layer{li}.{bi}.", blk)
-            if li == 3:
-                x_aux = a
+        _, _, x_aux, a = self._trunk(tape, x, "", "initial")
         lo = self._psp_head(tape, a)
         H, W = x.shape[2], x.shape[3]
         heads = [BilinearHead(lo, False, H, W)]  # pspnet.py:86,91: F.interpolate default align_corners=False; the crop is a no-op
@@ -820,29 +874,9 @@ class PSPNet(_EngineModel):
         return heads
 
     def _psp_head(self, tape, a, cat=None):
-        """_PSPModule.forward + the classifier (pspnet.py:31-38, :66-70): returns the fp32 stride-8 logits Act.  a: the trunk
-        output (m channels; stages of m // 4).  cat: a `dense_buffer` of 2m channels whose first m the trunk wrote in place
-        (PSPDenseNet's block4); otherwise the concat is allocated here."""
-        N, Hf, Wf, m = a.t.shape
-        q = m // 4
-        psp = self.master_branch[0]
-        # pspnet.py:31-38: cat([features, stage1..4]) -> 3x3 bottleneck.  A ResNet trunk's output is copied into slice 0
-        # (it is also the residual-stream tensor, so it cannot simply be produced in place there).
-        if cat is None:
-            cat, sl = tape.concat(N, Hf, Wf, [m, q, q, q, q], a.t.device)
-            feats = tape.copy_into(a, sl[0])
-        else:
-            sl = [cat.t[..., :m]] + [cat.t[..., m + i * q:m + (i + 1) * q] for i in range(4)]
-            feats = a
-        br = [feats]
-        for i, b in enumerate(self.bins):
-            st = psp.stages[i]
-            p = tape.avgpool(a, b)
-            p = self._cbr(tape, p, f"master_branch.0.stages.{i}.1", st[1], st[2])
-            br.append(tape.bilinear(p, Hf, Wf, True, out=sl[i + 1]))
-        tape.bind_slices(cat, br)
-        y = self._cbr(tape, cat, "master_branch.0.bottleneck.0", psp.bottleneck[0], psp.bottleneck[1], drop_p=psp.bottleneck[3].p,
-                      drop_channelwise=True)
+        """master_branch (pspnet.py:85): the PSP module + the classifier; returns the fp32 stride-8 logits Act.  a, cat: as
+        `_ppm`'s."""
+        y = self._ppm(tape, a, self.master_branch[0], "master_branch.0", cat=cat)
         lo, _ = tape.conv(y, self._spec("master_branch.1", self.master_branch[1]), out_dtype=torch.float32)
         return lo
 
@@ -870,21 +904,11 @@ class UperNet(_EngineModel):
         _check_pretrained(self, pretrained)
         self.num_classes = num_classes
         bb = _Holder()
-        c0, b0 = nn.Conv2d(in_channels, 64, 7, stride=2, padding=3, bias=False), nn.BatchNorm2d(64)
-        bb.initial = nn.Sequential(c0, b0, nn.ReLU(inplace=True), nn.MaxPool2d(kernel_size=3, stride=2, padding=1))
+        bb.initial = _stem7(in_channels)
         bb.layer1, bb.layer2, bb.layer3, bb.layer4 = _res_layers(RESNET_BLOCKS[backbone], 64, [(1, 1, 1), (2, 1, 1), (2, 1, 1), (1, 2, 2)])
         self.backbone = bb
         feats = [256, 512, 1024, 2048]
-        ppn = _Holder()
-        self.bins = (1, 2, 4, 6)
-        stages = []
-        for b in self.bins:
-            c, n = _cbn(feats[-1], feats[-1] // 4, 1)
-            stages.append(nn.Sequential(nn.AdaptiveAvgPool2d(output_size=b), c, n, nn.ReLU(inplace=True)))
-        ppn.stages = nn.ModuleList(stages)
-        c, n = _cbn(feats[-1] * 2, feats[-1], 3)
-        ppn.bottleneck = nn.Sequential(c, n, nn.ReLU(inplace=True), nn.Dropout2d(0.1))
-        self.PPN = ppn
+        self.PPN = _psp_module(feats[-1], (1, 2, 4, 6), feats[-1])
         fpn = _Holder()
         fpn.conv1x1 = nn.ModuleList([nn.Conv2d(f, fpn_out, kernel_size=1) for f in feats[1:]])
         fpn.smooth_conv = nn.ModuleList([nn.Conv2d(fpn_out, fpn_out, kernel_size=3, padding=1)] * (len(feats) - 1))
@@ -897,32 +921,12 @@ class UperNet(_EngineModel):
         if freeze_bn:
             self.freeze_bn()
         if freeze_backbone:
-            for p in self.backbone.parameters():
-                p.requires_grad = False
+            _freeze(self.backbone.parameters())
 
     def _forward_heads(self, tape, x):
         N = x.shape[0]
-        bb = self.backbone
-        a = self._cbr(tape, x, "backbone.initial.0", bb.initial[0], bb.initial[1])
-        a = tape.maxpool(a)
-        feats = []
-        for li in (1, 2, 3, 4):
-            for bi, blk in enumerate(getattr(bb, f"layer{li}")):
-                a = self._block(tape, a, f"backbone.layer{li}.{bi}.", blk)
-            feats.append(a)
-        # ---- PPN on the last feature map (upernet.py:31-38) ----
-        f4 = feats[-1]
-        Hf, Wf = f4.t.shape[1], f4.t.shape[2]
-        cat, sl = tape.concat(N, Hf, Wf, [2048, 512, 512, 512, 512], f4.t.device)
-        br = [tape.copy_into(f4, sl[0])]
-        for i, b in enumerate(self.bins):
-            st = self.PPN.stages[i]
-            p = tape.avgpool(f4, b)
-            p = self._cbr(tape, p, f"PPN.stages.{i}.1", st[1], st[2])
-            br.append(tape.bilinear(p, Hf, Wf, True, out=sl[i + 1]))
-        tape.bind_slices(cat, br)
-        pb = self.PPN.bottleneck
-        feats[-1] = self._cbr(tape, cat, "PPN.bottleneck.0", pb[0], pb[1], drop_p=pb[3].p, drop_channelwise=True)
+        feats = self._trunk(tape, x, "backbone.", "initial")
+        feats[-1] = self._ppm(tape, feats[-1], self.PPN, "PPN")  # PPN on the last feature map (upernet.py:31-38)
         # ---- FPN_fuse (upernet.py:103-117) ----
         F_ = self.FPN
         lat = [feats[0]]
@@ -986,20 +990,11 @@ class DeepLab_DUC_HDC(_EngineModel):
         assert output_stride in (4, 8), "Only output strides of 8 or 16 are suported"
         self.num_classes, self.output_stride = num_classes, output_stride
         bb = _Holder()
-        c0, b0 = nn.Conv2d(in_channels, 64, 7, stride=2 if output_stride == 8 else 1, padding=3, bias=False), nn.BatchNorm2d(64)
-        bb.layer0 = nn.Sequential(c0, b0, nn.ReLU(inplace=True), nn.MaxPool2d(kernel_size=3, stride=2, padding=1))
+        bb.layer0 = _stem7(in_channels, stride=2 if output_stride == 8 else 1)
         plan = [(1, [1] * 3), (2, [1] * 4), (1, [1, 2, 3] * 7 + [2, 2]), (1, [3, 4, 5])]
         bb.layer1, bb.layer2, bb.layer3, bb.layer4 = _res_layers(RESNET_BLOCKS["resnet101"], 64, plan)
         self.backbone = bb
-        a = _Holder()
-        for i, d in enumerate((1, 6, 12, 18, 24, 36), 1):
-            c, n = _cbn(2048, 256, 1 if i == 1 else 3, 1, d)
-            setattr(a, f"aspp{i}", nn.Sequential(c, n, nn.ReLU(inplace=True)))
-        c, n = _cbn(2048, 256, 1)
-        a.avg_pool = nn.Sequential(nn.AdaptiveAvgPool2d((1, 1)), c, n, nn.ReLU(inplace=True))
-        a.conv1, a.bn1 = _cbn(256 * 7, 256, 1)
-        a.relu, a.dropout = nn.ReLU(inplace=True), nn.Dropout(0.5)
-        self.ASSP = a
+        self.ASSP = _aspp_module((1, 6, 12, 18, 24, 36))
         d = _Holder()
         d.conv1, d.bn1 = _cbn(256, 48, 1)
         d.relu = nn.ReLU(inplace=True)
@@ -1016,8 +1011,7 @@ class DeepLab_DUC_HDC(_EngineModel):
         if freeze_bn:
             self.freeze_bn()
         if freeze_backbone:
-            for p in self.backbone.parameters():
-                p.requires_grad = False
+            _freeze(self.backbone.parameters())
 
     def _decoder(self, tape, f, low):
         """Decoder.forward (duc_hdc.py:200-208): the DUC output is shuffled and cropped straight into the concat buffer
@@ -1036,31 +1030,8 @@ class DeepLab_DUC_HDC(_EngineModel):
         lo, _ = tape.conv(y, self._spec("decoder.output.7", D.output[7]), out=buf)
         return lo
 
-    def _aspp(self, tape, a):
-        """ASSP.forward (duc_hdc.py:157-174): six branches + image pooling written straight into one 1792-channel buffer."""
-        N, Hf, Wf = a.t.shape[0], a.t.shape[1], a.t.shape[2]
-        A = self.ASSP
-        cat, sl = tape.concat(N, Hf, Wf, [256] * 7, a.t.device)
-        br = []
-        for i in range(1, 7):
-            seq = getattr(A, f"aspp{i}")
-            br.append(self._cbr(tape, a, f"ASSP.aspp{i}.0", seq[0], seq[1], out=sl[i - 1]))
-        g = tape.avgpool(a, 1)
-        g = self._cbr(tape, g, "ASSP.avg_pool.1", A.avg_pool[1], A.avg_pool[2])
-        br.append(tape.bilinear(g, Hf, Wf, True, out=sl[6]))
-        tape.bind_slices(cat, br)
-        return self._cbr(tape, cat, "ASSP.conv1", A.conv1, A.bn1, drop_p=A.dropout.p)
-
     def _forward_heads(self, tape, x):
-        bb = self.backbone
-        a = self._cbr(tape, x, "backbone.layer0.0", bb.layer0[0], bb.layer0[1])
-        a = tape.maxpool(a)
-        low = None
-        for li in (1, 2, 3, 4):
-            for bi, blk in enumerate(getattr(bb, f"layer{li}")):
-                a = self._block(tape, a, f"backbone.layer{li}.{bi}.", blk)
-            if li == 1:
-                low = a
+        low, _, _, a = self._trunk(tape, x, "backbone.", "layer0")
         y = self._decoder(tape, self._aspp(tape, a), low)
         z = self._cbr(tape, y, "DUC_out.conv", self.DUC_out.conv, self.DUC_out.bn)
         return [ShuffleHead(z, 4)]
@@ -1100,11 +1071,7 @@ class UNetResnet(_EngineModel):
             raise NotImplementedError("in_channels != 3 swaps the deep stem for a 64-channel 7x7 conv that bn1 cannot take "
                                       "(unet.py:131-132); not built")
         self.num_classes = num_classes
-        s1, n1 = _cbn(3, 64, 3, 2, 1)
-        s2, n2 = _cbn(64, 64, 3, 1, 1)
-        s3 = nn.Conv2d(64, 128, 3, stride=1, padding=1, bias=False)
-        stem = nn.Sequential(s1, n1, nn.ReLU(inplace=True), s2, n2, nn.ReLU(inplace=True), s3)
-        self.initial = nn.Sequential(stem, nn.BatchNorm2d(128), nn.ReLU(inplace=True), nn.MaxPool2d(kernel_size=3, stride=2, padding=1))
+        self.initial = _deep_stem()
         plan = [(1, 1, 1), (2, 1, 1), (1, 1, 2), (1, 2, 4)]  # resnet.py:190-210, as PSPNet
         self.layer1, self.layer2, self.layer3, self.layer4 = _res_layers(RESNET_BLOCKS[backbone], 128, plan)
         for name, cin, cout in self.DECODER:
@@ -1117,8 +1084,7 @@ class UNetResnet(_EngineModel):
         if freeze_bn:
             self.freeze_bn()
         if freeze_backbone:
-            for p in self.get_backbone_params():
-                p.requires_grad = False
+            _freeze(self.get_backbone_params())
 
     def _conv(self, tape, x, name):
         y, _ = tape.conv(x, self._spec(name, getattr(self, name)))
@@ -1135,11 +1101,7 @@ class UNetResnet(_EngineModel):
     def _forward_heads(self, tape, x):
         N, H, W = x.shape[0], x.shape[2], x.shape[3]
         dev = x.device
-        stem = self.initial[0]
-        a = self._cbr(tape, x, "initial.0.0", stem[0], stem[1])
-        a = self._cbr(tape, a, "initial.0.3", stem[3], stem[4])
-        a = self._cbr(tape, a, "initial.0.6", stem[6], self.initial[1])
-        a = tape.maxpool(a)
+        a = self._stem(tape, x, "initial", self.initial)
         # concat buffers (upsampled, skip) at the sizes of x1, x2, x3: the last block of layers 1-3 writes its output into
         # the skip slice, and the next layer reads it from there
         cats, skips = {}, {}
@@ -1206,6 +1168,7 @@ class SegNet(_EngineModel):
     ENCODER = ((64, 64), (128, 128), (256, 256, 256), (512, 512, 512), (512, 512, 512))
     DECODER = ((512, (512, 512, 512)), (512, (512, 512, 256)), (256, (256, 256, 128)), (128, (128, 64)), (64, (64, 64)))
     MIN_SIZE = 32
+    IM2COL_CONV = "stage1_encoder.0"
 
     def __init__(self, num_classes, in_channels=3, pretrained=None, freeze_bn=False, freeze_backbone=False, **_):
         super().__init__()
@@ -1240,17 +1203,7 @@ class SegNet(_EngineModel):
         if freeze_bn:
             self.freeze_bn()
         if freeze_backbone:
-            for i in range(1, 6):
-                for p in getattr(self, f"stage{i}_encoder").parameters():
-                    p.requires_grad = False
-
-    def _spec(self, name, module):
-        # the network input (NCHW fp32, any channel count) always goes through the explicit im2col conv
-        s = self._specs.get(name)
-        if s is None or s.m is not module:
-            s = ConvSpec(name, module, explicit_im2col=(name == "stage1_encoder.0"))
-            self._specs[name] = s
-        return s
+            _freeze(chain(*(getattr(self, f"stage{i}_encoder").parameters() for i in range(1, 6))))
 
     def _check_size(self, x):
         H, W = x.shape[-2], x.shape[-1]
@@ -1352,8 +1305,7 @@ class FCN8(_EngineModel):
         if freeze_bn:
             self.freeze_bn()
         if freeze_backbone:
-            for p in chain(self.pool3.parameters(), self.pool4.parameters(), self.pool5.parameters()):
-                p.requires_grad = False
+            _freeze(chain(self.pool3.parameters(), self.pool4.parameters(), self.pool5.parameters()))
 
     def all_conv_specs(self):
         # the frozen upsamplers run on the score kernels, not the conv path: no packed weight or weight gradient
@@ -1449,6 +1401,8 @@ class PSPDenseNet(_EngineModel):
     there.  densenet161 raises NotImplementedError: its block1 expects 96 channels and the reference cannot train it from
     scratch."""
 
+    IM2COL_CONV = "block0.0"
+
     def __init__(self, num_classes, in_channels=3, backbone="densenet201", pretrained=None, use_aux=True, freeze_bn=False, **_):
         super().__init__()
         if backbone == "densenet161":
@@ -1480,20 +1434,7 @@ class PSPDenseNet(_EngineModel):
         for k in (2, 3):
             cin, cout = widths[k - 1][1], widths[k][0]
             setattr(self, f"transition{k}", nn.Sequential(nn.BatchNorm2d(cin), nn.ReLU(inplace=True), nn.Conv2d(cin, cout, 1, bias=False)))
-        m_out, aux_in = widths[3][1], widths[3][0]
-        psp = _Holder()
-        stages = []
-        for b in (1, 2, 3, 6):
-            cv, bn = _cbn(m_out, m_out // 4, 1)
-            stages.append(nn.Sequential(nn.AdaptiveAvgPool2d(output_size=b), cv, bn, nn.ReLU(inplace=True)))
-        psp.stages = nn.ModuleList(stages)
-        cv, bn = _cbn(m_out * 2, m_out // 4, 3)
-        psp.bottleneck = nn.Sequential(cv, bn, nn.ReLU(inplace=True), nn.Dropout2d(0.1))
-        self.master_branch = nn.Sequential(psp, nn.Conv2d(m_out // 4, num_classes, kernel_size=1))
-        cv, bn = _cbn(aux_in, m_out // 4, 3)
-        self.auxiliary_branch = nn.Sequential(cv, bn, nn.ReLU(inplace=True), nn.Dropout2d(0.1),
-                                              nn.Conv2d(m_out // 4, num_classes, kernel_size=1))
-        self.bins = (1, 2, 3, 6)
+        self.master_branch, self.auxiliary_branch = _psp_branches(widths[3][1], widths[3][0], num_classes)
         for mod in (self.block1, self.block2, self.block3, self.block4, self.transition1, self.transition2, self.transition3):
             for m in mod.modules():  # torchvision DenseNet.__init__
                 if isinstance(m, nn.Conv2d):
@@ -1505,24 +1446,6 @@ class PSPDenseNet(_EngineModel):
         _init_like_reference_head(self.master_branch, self.auxiliary_branch)
         if freeze_bn:
             self.freeze_bn()
-
-    _psp_head = PSPNet._psp_head
-
-    def _spec(self, name, module):
-        # the network input (NCHW fp32, any channel count) always goes through the explicit im2col conv
-        s = self._specs.get(name)
-        if s is None or s.m is not module:
-            s = ConvSpec(name, module, explicit_im2col=(name == "block0.0"))
-            self._specs[name] = s
-        return s
-
-    def _finish(self, tape):
-        # block0.4 normalises twice per step: its num_batches_tracked rises by 2, as the reference's
-        counts = {}
-        for m in tape.bn_modules:
-            counts[m] = counts.get(m, 0) + 1
-        for k in sorted(set(counts.values())):
-            torch._foreach_add_([m.num_batches_tracked for m, c in counts.items() if c == k], k)
 
     def _dense(self, tape, buf, table, bi, c0, dil):
         """Block bi's layers over its buffer (slice [0, c0) already written, its record in table[:2 c0])."""
@@ -1588,7 +1511,9 @@ class PSPDenseNet(_EngineModel):
             ya = self._cbr(tape, x_aux, "auxiliary_branch.0", ab[0], ab[1], drop_p=ab[3].p, drop_channelwise=True)
             la, _ = tape.conv(ya, self._spec("auxiliary_branch.4", ab[4]), out_dtype=torch.float32)
             heads.append(BilinearHead(la, False, H, W))
-        lo = self._psp_head(tape, tape.prefix(buf, 0, m_out), cat=buf)
+        mb = self.master_branch
+        y = self._ppm(tape, tape.prefix(buf, 0, m_out), mb[0], "master_branch.0", cat=buf)
+        lo, _ = tape.conv(y, self._spec("master_branch.1", mb[1]), out_dtype=torch.float32)
         return [BilinearHead(lo, False, H, W)] + heads
 
     def get_backbone_params(self):
