@@ -453,6 +453,13 @@ typedef struct seg_aug_scale_entry {
 int seg_aug_scale_entry_bytes(void);
 int seg_augment_scale_batch_u8(const uint8_t* arena, const seg_aug_scale_entry* table, int B, int crop_h, int crop_w,
                                const float* mean3, const float* std3, float* out_nchw, int64_t* out_labels, void* stream);
+/* The validation tail of base/base_dataset.py:40-61 (resize so the short side is the crop, centre crop, np.uint8,
+ * ToTensor, Normalize) with the same records: the image arithmetic is seg_augment_scale_batch_u8's, flip = 0 and (y0, x0)
+ * the centre origin.  The label follows PIL's Image.resize(NEAREST) instead of cv2's INTER_NEAREST: Pillow accumulates its
+ * float64 source coordinate pixel by pixel, so the host computes the indices and appends them to the label map in the
+ * arena, at lbl_off + (src_h * src_w * lbl_bytes rounded up to 4): int32 x index [w], then int32 y index [h]. */
+int seg_augment_val_batch_u8(const uint8_t* arena, const seg_aug_scale_entry* table, int B, int crop_h, int crop_w,
+                             const float* mean3, const float* std3, float* out_nchw, int64_t* out_labels, void* stream);
 /* the same with the rotation of base/base_dataset.py:77-83
  * between the resize and the tail.  (a11 a12 b1; a21 a22 b2) = the INVERSE of cv2.getRotationMatrix2D((w/2, h/2), angle, 1)
  * computed by the host in float64 exactly as cv::warpAffine does (oracle/data.py::cv_warp_affine); identity = no rotation. */
@@ -470,6 +477,13 @@ typedef struct seg_aug_full_entry {
 int seg_aug_full_entry_bytes(void);
 int seg_augment_full_batch_u8(const uint8_t* arena, const seg_aug_full_entry* table, int B, int crop_h, int crop_w,
                               const float* mean3, const float* std3, float* out_nchw, int64_t* out_labels, void* stream);
+/* the same with the Gaussian blur of base/base_dataset.py:114-119 after the flip, on the float crop before np.uint8:
+ * cv2.GaussianBlur(k = 3, BORDER_REFLECT_101 at the crop's border), OpenCV's separable fp32 filter (row pass, then column
+ * pass, no fma).  blur_taps: DEVICE memory, B x (centre tap, side tap) float32 = getGaussianKernel(3, sigma) in float64
+ * rounded to float32, computed by the host; (1, 0) = k = 1 (no blur), bit-identical to seg_augment_full_batch_u8. */
+int seg_augment_full_blur_batch_u8(const uint8_t* arena, const seg_aug_full_entry* table, const float* blur_taps, int B, int crop_h,
+                                   int crop_w, const float* mean3, const float* std3, float* out_nchw, int64_t* out_labels,
+                                   void* stream);
 /* ---- inference-side resampling (SURVEY.md §8f row 3; inference.py:26-79), fp32 NCHW score maps, `planes` = N*C ----
  * resize: dst = beta*dst + alpha*flip_x?(bilinear resize of src to Hd x Wd).  mode 0 / 1 = ATen bilinear with
  * align_corners False / True (1 = nn.Upsample(align_corners=True), inference.py:60; same size + flip_x = tensor.flip(-1),

@@ -111,6 +111,14 @@ __device__ __forceinline__ void cv_linear_coord(int d, double scale, int src, bo
   }
 }
 
+// PilLabels = false: the training tail's label rule above (cv2.resize INTER_NEAREST).
+// PilLabels = true: the validation tail's (base_dataset.py:40-61), which resizes the label with PIL's Image.resize(NEAREST).
+// Pillow walks the destination with a float64 source coordinate that it ACCUMULATES (xo = a/2, then xo += a per pixel,
+// a = src / dst; Geometry.c ImagingScaleAffine) and truncates, so the index is not a closed-form function of d: for about
+// half of the size pairs some index differs from floor((d + 0.5) * a).  The host runs the same additions and appends the
+// two int32 index tables (x: w entries, then y: h entries) to the label map in the arena, 4-byte aligned; the kernel looks
+// them up.  The image arithmetic is the same in both instantiations.
+template <bool PilLabels>
 __global__ void __launch_bounds__(256) augment_scale_u8_kernel(const uint8_t* __restrict__ arena,
                                                                const seg_aug_scale_entry* __restrict__ table, int crop_h, int crop_w,
                                                                AugParams prm, float* __restrict__ out, int64_t* __restrict__ labels) {
@@ -157,9 +165,17 @@ __global__ void __launch_bounds__(256) augment_scale_u8_kernel(const uint8_t* __
       g = res[1];
       bl = res[2];
       if (lbl != nullptr) {
-        int lx = (int)floor(__dmul_rn((double)dx, e.scale_x)), ly = (int)floor(__dmul_rn((double)dy, e.scale_y));
-        lx = lx < e.src_w - 1 ? lx : e.src_w - 1;
-        ly = ly < e.src_h - 1 ? ly : e.src_h - 1;
+        int lx, ly;
+        if constexpr (PilLabels) {
+          const int32_t* tab = reinterpret_cast<const int32_t*>(lbl + ((int64_t)e.src_h * e.src_w * e.lbl_bytes + 3) / 4 * 4);
+          lx = tab[dx];
+          ly = tab[e.w + dy];
+        } else {
+          lx = (int)floor(__dmul_rn((double)dx, e.scale_x));
+          ly = (int)floor(__dmul_rn((double)dy, e.scale_y));
+          lx = lx < e.src_w - 1 ? lx : e.src_w - 1;
+          ly = ly < e.src_h - 1 ? ly : e.src_h - 1;
+        }
         const int64_t k = (int64_t)ly * e.src_w + lx;
         lab = e.lbl_bytes == 1 ? (int)lbl[k] : reinterpret_cast<const int32_t*>(lbl)[k];
       }
@@ -214,6 +230,49 @@ __device__ __forceinline__ int resized_label(const uint8_t* __restrict__ lbl, co
 // INTER_NEAREST uses delta = AB_SCALE / 2 on the same rounded row / column terms
 __device__ __forceinline__ long long rowX_nearest_fix(long long row_term, long long col_term) { return row_term + 512 + col_term; }
 
+// Fixed-point source coordinates in the resized image of rotated pixel (dy, dx): the two rounded terms are added as
+// integers, as OpenCV does.
+struct RotCoords {
+  long long colX, colY, rowX, rowY;
+};
+__device__ __forceinline__ RotCoords rot_coords(const seg_aug_full_entry& e, int dy, int dx) {
+  RotCoords q;
+  q.colX = __double2ll_rn(__dmul_rn(__dmul_rn(e.a11, (double)dx), 1024.0));
+  q.colY = __double2ll_rn(__dmul_rn(__dmul_rn(e.a21, (double)dx), 1024.0));
+  q.rowX = __double2ll_rn(__dmul_rn(__dadd_rn(__dmul_rn(e.a12, (double)dy), e.b1), 1024.0));
+  q.rowY = __double2ll_rn(__dmul_rn(__dadd_rn(__dmul_rn(e.a22, (double)dy), e.b2), 1024.0));
+  return q;
+}
+
+// The float (pre-np.uint8) value of rotated pixel (dy, dx), inside the h x w image: INTER_LINEAR over four resized taps.
+__device__ __forceinline__ void rotated_pixel_f32(const uint8_t* __restrict__ img, const seg_aug_full_entry& e, const RotCoords& q,
+                                                  float* v3) {
+  const long long X = q.rowX + 16 + q.colX, Y = q.rowY + 16 + q.colY;  // delta = AB_SCALE / INTER_TAB_SIZE / 2
+  const long long Xf = X >> 5, Yf = Y >> 5;                            // 5 fractional bits left
+  const int xi = (int)(Xf >> 5), yi = (int)(Yf >> 5);
+  const float fx = __fdiv_rn((float)(int)(Xf & 31), 32.f), fy = __fdiv_rn((float)(int)(Yf & 31), 32.f);
+  const float one_fx = __fsub_rn(1.f, fx), one_fy = __fsub_rn(1.f, fy);
+  const float w00 = __fmul_rn(one_fy, one_fx), w01 = __fmul_rn(one_fy, fx), w10 = __fmul_rn(fy, one_fx), w11 = __fmul_rn(fy, fx);
+  float p00[3], p01[3], p10[3], p11[3];
+  resized_pixel_f32(img, e, yi, xi, p00);
+  resized_pixel_f32(img, e, yi, xi + 1, p01);
+  resized_pixel_f32(img, e, yi + 1, xi, p10);
+  resized_pixel_f32(img, e, yi + 1, xi + 1, p11);
+#pragma unroll
+  for (int c = 0; c < 3; ++c)
+    v3[c] = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(p00[c], w00), __fmul_rn(p01[c], w01)), __fmul_rn(p10[c], w10)), __fmul_rn(p11[c], w11));
+}
+
+__device__ __forceinline__ unsigned trunc_u8(float v) {
+  unsigned r = v > 0.f ? (unsigned)v : 0u;  // np.uint8(float) truncates
+  return r > 255u ? 255u : r;
+}
+
+__device__ __forceinline__ int rotated_label(const uint8_t* __restrict__ lbl, const seg_aug_full_entry& e, const RotCoords& q) {
+  const long long X = rowX_nearest_fix(q.rowX, q.colX), Y = rowX_nearest_fix(q.rowY, q.colY);
+  return resized_label(lbl, e, (int)(Y >> 10), (int)(X >> 10));
+}
+
 __global__ void __launch_bounds__(256) augment_full_u8_kernel(const uint8_t* __restrict__ arena, const seg_aug_full_entry* __restrict__ table,
                                                               int crop_h, int crop_w, AugParams prm, float* __restrict__ out,
                                                               int64_t* __restrict__ labels) {
@@ -238,44 +297,96 @@ __global__ void __launch_bounds__(256) augment_full_u8_kernel(const uint8_t* __r
     unsigned r = 0, g = 0, bl = 0;
     int lab = 0;
     if (dy < e.h && dx < e.w) {
-      // fixed-point source coordinates in the resized image (the two rounded terms are added as integers, as OpenCV does)
-      const long long colX = __double2ll_rn(__dmul_rn(__dmul_rn(e.a11, (double)dx), 1024.0));
-      const long long colY = __double2ll_rn(__dmul_rn(__dmul_rn(e.a21, (double)dx), 1024.0));
-      const long long rowX = __double2ll_rn(__dmul_rn(__dadd_rn(__dmul_rn(e.a12, (double)dy), e.b1), 1024.0));
-      const long long rowY = __double2ll_rn(__dmul_rn(__dadd_rn(__dmul_rn(e.a22, (double)dy), e.b2), 1024.0));
-      {
-        const long long X = rowX + 16 + colX, Y = rowY + 16 + colY;  // delta = AB_SCALE / INTER_TAB_SIZE / 2
-        const long long Xf = X >> 5, Yf = Y >> 5;                    // 5 fractional bits left
-        const int xi = (int)(Xf >> 5), yi = (int)(Yf >> 5);
-        const float fx = __fdiv_rn((float)(int)(Xf & 31), 32.f), fy = __fdiv_rn((float)(int)(Yf & 31), 32.f);
-        const float one_fx = __fsub_rn(1.f, fx), one_fy = __fsub_rn(1.f, fy);
-        const float w00 = __fmul_rn(one_fy, one_fx), w01 = __fmul_rn(one_fy, fx), w10 = __fmul_rn(fy, one_fx), w11 = __fmul_rn(fy, fx);
-        float p00[3], p01[3], p10[3], p11[3];
-        resized_pixel_f32(img, e, yi, xi, p00);
-        resized_pixel_f32(img, e, yi, xi + 1, p01);
-        resized_pixel_f32(img, e, yi + 1, xi, p10);
-        resized_pixel_f32(img, e, yi + 1, xi + 1, p11);
-        unsigned res[3];
-#pragma unroll
-        for (int c = 0; c < 3; ++c) {
-          const float v = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(p00[c], w00), __fmul_rn(p01[c], w01)), __fmul_rn(p10[c], w10)),
-                                    __fmul_rn(p11[c], w11));
-          res[c] = v > 0.f ? (unsigned)v : 0u;  // np.uint8(float) truncates
-          if (res[c] > 255u) res[c] = 255u;
-        }
-        r = res[0];
-        g = res[1];
-        bl = res[2];
-      }
-      if (lbl != nullptr) {
-        const long long X = rowX_nearest_fix(rowX, colX), Y = rowX_nearest_fix(rowY, colY);
-        lab = resized_label(lbl, e, (int)(Y >> 10), (int)(X >> 10));
-      }
+      const RotCoords q = rot_coords(e, dy, dx);
+      float v[3];
+      rotated_pixel_f32(img, e, q, v);
+      r = trunc_u8(v[0]);
+      g = trunc_u8(v[1]);
+      bl = trunc_u8(v[2]);
+      if (lbl != nullptr) lab = rotated_label(lbl, e, q);
     }
     o[i] = lut[0][r];
     o[plane + i] = lut[1][g];
     o[2 * (int64_t)plane + i] = lut[2][bl];
     if (lo != nullptr) lo[i] = (int64_t)lab;
+  }
+}
+
+// ------------------------------------------------------------------ scale + rotate + tail + GAUSSIAN BLUR
+// base_dataset.py:114-119 blurs the float32 crop AFTER the flip, BEFORE np.uint8: cv2.GaussianBlur(image, (k, k), sigma,
+// sigma, BORDER_REFLECT_101) with k = 1 (a copy) or 3.  OpenCV's float path for k = 3 (smooth.dispatch.cpp -> sepFilter2D,
+// filter.simd.hpp SymmRowSmallFilter / SymmColumnSmallFilter), restated bit-exactly in the tests' blur oracle:
+//   taps  k0 (centre), k1 (side): getGaussianKernel in float64 rounded to float32 — computed by the HOST, passed per sample;
+//   row   R = C*k0 + (C[x-1] + C[x+1])*k1    then    column   B = (R[y-1] + R[y+1])*k1 + R*k0    (fp32, no fma);
+//   reflect-101 at the CROP's border (index -1 -> 1, n -> n-2);  an axis of length 1 is not filtered (OpenCV's kernel
+//   size drops to 1 there);  taps (1, 0) are an exact identity (C*1 + (..)*0 == C for the finite values here).
+// The 3-tap kernel is symmetric and a + b == b + a in IEEE arithmetic, so blurring the unflipped crop and flipping the
+// result is bit-identical to the reference's flip-then-blur.  Each block stages a TY x TX tile of the pre-truncation crop
+// values plus a one-pixel halo (recomputed from the raw image: 16 raw taps per staged pixel, 1.2x the tile) in shared
+// memory, runs the row pass into a second buffer, then the column pass, np.uint8, ToTensor and Normalize.
+constexpr int BLUR_TY = 16, BLUR_TX = 32;
+
+__device__ __forceinline__ int reflect101(int i, int n) { return n == 1 ? 0 : (i < 0 ? -i : (i >= n ? 2 * n - 2 - i : i)); }
+
+__global__ void __launch_bounds__(256) augment_full_blur_u8_kernel(const uint8_t* __restrict__ arena,
+                                                                   const seg_aug_full_entry* __restrict__ table,
+                                                                   const float* __restrict__ blur_taps, int crop_h, int crop_w,
+                                                                   int tiles_x, AugParams prm, float* __restrict__ out,
+                                                                   int64_t* __restrict__ labels) {
+  __shared__ float lut[3][256];
+  __shared__ float cs[3][BLUR_TY + 2][BLUR_TX + 2];  // crop values, halo included
+  __shared__ float rs[3][BLUR_TY + 2][BLUR_TX];      // after the row pass
+  for (int t = threadIdx.x; t < 768; t += blockDim.x) {
+    const int c = t >> 8, v = t & 255;
+    lut[c][v] = __fdiv_rn(__fsub_rn(__fdiv_rn((float)v, 255.f), prm.mean[c]), prm.stdv[c]);
+  }
+  const int b = blockIdx.y;
+  const seg_aug_full_entry e = table[b];
+  const uint8_t* img = arena + e.img_off;
+  const int ty0 = (int)(blockIdx.x / tiles_x) * BLUR_TY, tx0 = (int)(blockIdx.x % tiles_x) * BLUR_TX;
+  // the unflipped crop at (y, xs): rotated-image pixel (y + y0, xs + x0), zero padding outside h x w
+  for (int t = threadIdx.x; t < (BLUR_TY + 2) * (BLUR_TX + 2); t += blockDim.x) {
+    const int hy = t / (BLUR_TX + 2), hx = t - hy * (BLUR_TX + 2);
+    const int y = ty0 + hy - 1, xs = tx0 + hx - 1;
+    float v[3] = {0.f, 0.f, 0.f};
+    if (y <= crop_h && xs <= crop_w) {  // beyond that only pixels outside the crop would read the value
+      const int dy = reflect101(y, crop_h) + e.y0, dx = reflect101(xs, crop_w) + e.x0;
+      if (dy < e.h && dx < e.w) rotated_pixel_f32(img, e, rot_coords(e, dy, dx), v);
+    }
+#pragma unroll
+    for (int c = 0; c < 3; ++c) cs[c][hy][hx] = v[c];
+  }
+  __syncthreads();
+  const float k0 = blur_taps[2 * b], k1 = blur_taps[2 * b + 1];
+  const float kx0 = crop_w > 1 ? k0 : 1.f, kx1 = crop_w > 1 ? k1 : 0.f;
+  const float ky0 = crop_h > 1 ? k0 : 1.f, ky1 = crop_h > 1 ? k1 : 0.f;
+  for (int t = threadIdx.x; t < (BLUR_TY + 2) * BLUR_TX; t += blockDim.x) {
+    const int hy = t / BLUR_TX, x = t - hy * BLUR_TX;
+#pragma unroll
+    for (int c = 0; c < 3; ++c)
+      rs[c][hy][x] = __fadd_rn(__fmul_rn(cs[c][hy][x + 1], kx0), __fmul_rn(__fadd_rn(cs[c][hy][x], cs[c][hy][x + 2]), kx1));
+  }
+  __syncthreads();
+  const uint8_t* lbl = (e.lbl_off >= 0 && labels != nullptr) ? arena + e.lbl_off : nullptr;
+  const int plane = crop_h * crop_w;
+  float* o = out + (int64_t)b * 3 * plane;
+  int64_t* lo = labels != nullptr ? labels + (int64_t)b * plane : nullptr;
+  for (int t = threadIdx.x; t < BLUR_TY * BLUR_TX; t += blockDim.x) {
+    const int ty = t / BLUR_TX, tx = t - ty * BLUR_TX;
+    const int y = ty0 + ty, xs = tx0 + tx;
+    if (y >= crop_h || xs >= crop_w) continue;
+    unsigned u[3];
+#pragma unroll
+    for (int c = 0; c < 3; ++c)
+      u[c] = trunc_u8(__fadd_rn(__fmul_rn(__fadd_rn(rs[c][ty][tx], rs[c][ty + 2][tx]), ky1), __fmul_rn(rs[c][ty + 1][tx], ky0)));
+    const int i = y * crop_w + (e.flip ? crop_w - 1 - xs : xs);
+    o[i] = lut[0][u[0]];
+    o[plane + i] = lut[1][u[1]];
+    o[2 * (int64_t)plane + i] = lut[2][u[2]];
+    if (lo != nullptr) {
+      const int dy = y + e.y0, dx = xs + e.x0;
+      lo[i] = (dy < e.h && dx < e.w && lbl != nullptr) ? (int64_t)rotated_label(lbl, e, rot_coords(e, dy, dx)) : 0;
+    }
   }
 }
 
@@ -444,8 +555,27 @@ int seg_augment_scale_batch_u8(const uint8_t* arena, const seg_aug_scale_entry* 
   if (per_image > need) per_image = need;
   if (per_image < 1) per_image = 1;
   dim3 grid((unsigned)per_image, (unsigned)B, 1);
-  augment_scale_u8_kernel<<<grid, 256, 0, ST(stream)>>>(arena, table, crop_h, crop_w, prm, out_nchw, out_labels);
+  augment_scale_u8_kernel<false><<<grid, 256, 0, ST(stream)>>>(arena, table, crop_h, crop_w, prm, out_nchw, out_labels);
   return check_launch("augment_scale_batch_u8");
+}
+
+int seg_augment_val_batch_u8(const uint8_t* arena, const seg_aug_scale_entry* table, int B, int crop_h, int crop_w,
+                             const float* mean3, const float* std3, float* out_nchw, int64_t* out_labels, void* stream) {
+  SEG_REQUIRE(arena != nullptr && table != nullptr && out_nchw != nullptr && mean3 != nullptr && std3 != nullptr, "augment_val: null pointer");
+  SEG_REQUIRE(B > 0 && B <= 65535 && crop_h > 0 && crop_w > 0 && (int64_t)crop_h * crop_w < (1ll << 30), "augment_val: bad batch / crop size");
+  AugParams prm;
+  for (int c = 0; c < 3; ++c) {
+    prm.mean[c] = mean3[c];
+    prm.stdv[c] = std3[c];
+    SEG_REQUIRE(std3[c] != 0.f, "augment_val: std must be non-zero");
+  }
+  int64_t per_image = ((int64_t)num_sms() * 8 + B - 1) / B;
+  const int64_t need = ceil_div64((int64_t)crop_h * crop_w, 256);
+  if (per_image > need) per_image = need;
+  if (per_image < 1) per_image = 1;
+  dim3 grid((unsigned)per_image, (unsigned)B, 1);
+  augment_scale_u8_kernel<true><<<grid, 256, 0, ST(stream)>>>(arena, table, crop_h, crop_w, prm, out_nchw, out_labels);
+  return check_launch("augment_val_batch_u8");
 }
 
 int seg_aug_full_entry_bytes(void) { return (int)sizeof(seg_aug_full_entry); }
@@ -467,6 +597,24 @@ int seg_augment_full_batch_u8(const uint8_t* arena, const seg_aug_full_entry* ta
   dim3 grid((unsigned)per_image, (unsigned)B, 1);
   augment_full_u8_kernel<<<grid, 256, 0, ST(stream)>>>(arena, table, crop_h, crop_w, prm, out_nchw, out_labels);
   return check_launch("augment_full_batch_u8");
+}
+
+int seg_augment_full_blur_batch_u8(const uint8_t* arena, const seg_aug_full_entry* table, const float* blur_taps, int B, int crop_h,
+                                   int crop_w, const float* mean3, const float* std3, float* out_nchw, int64_t* out_labels,
+                                   void* stream) {
+  SEG_REQUIRE(arena != nullptr && table != nullptr && blur_taps != nullptr && out_nchw != nullptr && mean3 != nullptr && std3 != nullptr,
+              "augment_full_blur: null pointer");
+  SEG_REQUIRE(B > 0 && B <= 65535 && crop_h > 0 && crop_w > 0 && (int64_t)crop_h * crop_w < (1ll << 30), "augment_full_blur: bad batch / crop size");
+  AugParams prm;
+  for (int c = 0; c < 3; ++c) {
+    prm.mean[c] = mean3[c];
+    prm.stdv[c] = std3[c];
+    SEG_REQUIRE(std3[c] != 0.f, "augment_full_blur: std must be non-zero");
+  }
+  const int64_t tiles_x = ceil_div64(crop_w, BLUR_TX), tiles = tiles_x * ceil_div64(crop_h, BLUR_TY);  // < 2^31 for crop_h * crop_w < 2^30
+  dim3 grid((unsigned)tiles, (unsigned)B, 1);
+  augment_full_blur_u8_kernel<<<grid, 256, 0, ST(stream)>>>(arena, table, blur_taps, crop_h, crop_w, (int)tiles_x, prm, out_nchw, out_labels);
+  return check_launch("augment_full_blur_batch_u8");
 }
 
 int seg_resize_nchw_f32(const float* src, int64_t planes, int Hs, int Ws, float* dst, int Hd, int Wd, int mode, int flip_x,

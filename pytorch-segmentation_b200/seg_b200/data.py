@@ -8,9 +8,10 @@ for the whole batch, bit-exactly (same fp32 operations).  The random draws stay 
 (crop row, crop column, flip), so a seeded run is reproducible against the reference.
 
     DeviceBatcher(mean, std, crop_size, device)      — stage(samples) -> (images fp32 [B,3,crop,crop], labels int64 [B,crop,crop])
-    DevicePrefetcher(loader, device, stop_after=None, batcher=None) — drop-in for the reference's DataPrefetcher;
+    DevicePrefetcher(loader, device, stop_after=None, batcher=None, val=False) — drop-in for the reference's DataPrefetcher;
         a loader that yields ready (float image batch, long label batch) pairs is passed through exactly as the reference
-        does, a loader that yields lists of raw samples goes through the batcher.
+        does, a loader that yields lists of raw samples goes through the batcher (stage, or stage_val for a validation
+        loader's raw (image, label) pairs when val=True).
 """
 import math
 import random
@@ -54,6 +55,49 @@ def inverse_rotation(w, h, angle):
     return a11, a12, -a11 * m02 - a12 * m12, a21, a22, -a21 * m02 - a22 * m12
 
 
+def draw_blur(blur=True, rng=random):
+    """The Gaussian-blur sigma of base_dataset.py:114-119 (drawn after the flip); None when blur is off."""
+    return rng.random() if blur else None
+
+
+def gaussian_taps(sigma):
+    """(centre, side) float32 taps of cv2.GaussianBlur(image, (k, k), sigma, sigma) with the reference's kernel size
+    k = int(3.3 * sigma) made odd: (1, 0) for k = 1 (no blur, also for sigma None), else getGaussianKernel(3, sigma, CV_32F)
+    as OpenCV computes it (float64: t = exp(4 * (-0.125 / sigma^2)), normalised by 1 / (2t + 1), rounded to float32)."""
+    if sigma is None:
+        return 1.0, 0.0
+    k = int(3.3 * sigma)
+    k = k + 1 if k % 2 == 0 else k
+    if k == 1:
+        return 1.0, 0.0
+    if k != 3:
+        raise ValueError(f"blur: sigma {sigma} gives a {k}x{k} kernel; the device blur implements 3x3 (sigma < 1.2121...)")
+    t = math.exp(4.0 * (-0.125 / (sigma * sigma)))
+    mul = 1.0 / (t * 2.0 + 1.0)
+    return float(np.float32(1.0 * mul)), float(np.float32(t * mul))
+
+
+def val_geometry(h, w, crop_size):
+    """(h', w', y0, x0) of _val_augmentation (base_dataset.py:40-61): the size whose short side is crop_size, in the
+    reference's Python arithmetic, and the centre crop's origin."""
+    if not crop_size:
+        raise ValueError("validation tail: crop_size None / 0 means no resize and no crop (variable-size batches), which the "
+                         "device tail does not build; set a crop_size")
+    crop = int(crop_size)
+    h2, w2 = (crop, int(crop * w / h)) if h < w else (int(crop * h / w), crop)
+    return h2, w2, (h2 - crop) // 2, (w2 - crop) // 2
+
+
+def pil_nearest_index(src, dst):
+    """Source index per destination index of PIL's Image.resize(NEAREST) (Geometry.c ImagingScaleAffine): a float64
+    coordinate that starts at a/2 and ACCUMULATES a = src / dst per pixel, truncated (np.add.accumulate adds in order)."""
+    a = float(src) / dst
+    xo = np.add.accumulate(np.concatenate([[0.0 + a * 0.5], np.full(dst - 1, a)]))
+    idx = xo.astype(np.int64)
+    assert idx.min() >= 0 and idx.max() < src
+    return idx.astype(np.int32)
+
+
 def draw_scale(h, w, base_size, scale=True, rng=random):
     """Size after the random-scale resize of base_dataset.py:66-72 (the long side becomes a draw in [0.5, 2] x base_size)."""
     if not base_size:
@@ -84,6 +128,9 @@ def check_crop_origins(crop, dims):
 class DeviceBatcher:
     def __init__(self, mean, std, crop_size, device, max_bytes=64 << 20):
         assert _ENTRY.itemsize == lib.load().seg_aug_entry_bytes()
+        if not crop_size:
+            raise ValueError("DeviceBatcher: crop_size None / 0 means the reference neither pads nor crops (and its validation "
+                             "tail does not resize), so batches would have variable sizes; the device tails need a crop_size")
         self.mean, self.std = [float(v) for v in mean], [float(v) for v in std]
         self.crop = int(crop_size)
         self.device = torch.device(device)
@@ -136,6 +183,57 @@ class DeviceBatcher:
         tab = dev[:B * _ENTRY.itemsize]
         return ops.augment_batch_u8(dev, tab, B, self.crop, self.crop, self.mean, self.std, want_labels=want_labels)
 
+    def _stage_raw(self, samples, dtype, record, head=None, tail=None):
+        """Packs RAW samples (image uint8 [H,W,3], label uint8|int32 [H,W] or None, ...) into the pinned staging buffer and
+        copies it to the device once: the B `dtype` records first, then `head` (a float32 array, e.g. per-sample blur taps),
+        then every image and label map 4-byte aligned, each label map followed by `tail(b, H, W)` (an int32 array) when given.
+        record(b, img_off, lbl_off, H, W, lbl_bytes) -> the record of sample b.  Returns (device arena, head offset)."""
+        B = len(samples)
+        slot = self._slot
+        self._slot ^= 1
+        if self._events[slot] is not None:
+            self._events[slot].synchronize()
+        host = self._host[slot].numpy()
+        table = np.zeros(B, dtype=dtype)
+        head_off = off = B * dtype.itemsize
+        if head is not None:
+            head = np.ascontiguousarray(head, dtype=np.float32)
+            host[off:off + head.nbytes] = head.reshape(-1).view(np.uint8)
+            off += head.nbytes
+        for b, s in enumerate(samples):
+            img, lbl = np.ascontiguousarray(s[0], dtype=np.uint8), s[1]
+            H, W = img.shape[:2]
+            assert img.shape == (H, W, 3), "images are HWC uint8 with 3 channels"
+            n = img.size
+            lb, lbl_off, extra = 1, -1, None
+            if lbl is not None:
+                lbl = np.ascontiguousarray(lbl)
+                assert lbl.shape == (H, W) and lbl.dtype in (np.uint8, np.int32), "labels are uint8 or int32 [H,W]"
+                lb = lbl.dtype.itemsize
+                extra = tail(b, H, W) if tail is not None else None
+            need = off + n + 8 + (H * W * lb if lbl is not None else 0) + (extra.nbytes if extra is not None else 0)
+            if need > self.capacity:
+                raise RuntimeError(f"DeviceBatcher: batch needs more than max_bytes={self.capacity} of staging memory")
+            host[off:off + n] = img.reshape(-1)
+            img_off = off
+            off += (n + 3) // 4 * 4
+            if lbl is not None:
+                nb = H * W * lb
+                host[off:off + nb] = lbl.reshape(-1).view(np.uint8)
+                lbl_off = off
+                off += (nb + 3) // 4 * 4
+                if extra is not None:
+                    host[off:off + extra.nbytes] = np.ascontiguousarray(extra, dtype=np.int32).view(np.uint8)
+                    off += extra.nbytes
+            table[b] = record(b, img_off, lbl_off, H, W, lb)
+        host[:B * dtype.itemsize] = table.view(np.uint8)
+        self.last_staged_bytes = off
+        dev = self._host[slot][:off].to(self.device, non_blocking=True)
+        ev = torch.cuda.Event()
+        ev.record()
+        self._events[slot] = ev
+        return dev, head_off
+
     def stage_scaled(self, samples):
         """samples: sequence of (RAW image uint8 [H,W,3], RAW label uint8|int32 [H,W] or None, h, w, y0, x0, flip): the sample
         is resized to h x w (cv2.resize arithmetic, base_dataset.py:66-75) and then padded / cropped / flipped / normalised
@@ -143,90 +241,77 @@ class DeviceBatcher:
         assert _SCALE_ENTRY.itemsize == lib.load().seg_aug_scale_entry_bytes()
         B = len(samples)
         check_crop_origins(self.crop, [(s[2], s[3], s[4], s[5]) for s in samples])
-        slot = self._slot
-        self._slot ^= 1
-        if self._events[slot] is not None:
-            self._events[slot].synchronize()
-        host = self._host[slot].numpy()
-        table = np.zeros(B, dtype=_SCALE_ENTRY)
-        off = B * _SCALE_ENTRY.itemsize
-        want_labels = samples[0][1] is not None
-        for b, (img, lbl, h, w, y0, x0, flip) in enumerate(samples):
-            img = np.ascontiguousarray(img, dtype=np.uint8)
-            H, W = img.shape[:2]
-            assert img.shape == (H, W, 3), "images are HWC uint8 with 3 channels"
-            n = img.size
-            lb, lbl_off = 1, -1
-            if lbl is not None:
-                lbl = np.ascontiguousarray(lbl)
-                assert lbl.shape == (H, W) and lbl.dtype in (np.uint8, np.int32), "labels are uint8 or int32 [H,W]"
-                lb = lbl.dtype.itemsize
-            if off + n + 8 + (H * W * lb if lbl is not None else 0) > self.capacity:
-                raise RuntimeError(f"DeviceBatcher: batch needs more than max_bytes={self.capacity} of staging memory")
-            host[off:off + n] = img.reshape(-1)
-            img_off = off
-            off += (n + 3) // 4 * 4
-            if lbl is not None:
-                nb = H * W * lb
-                host[off:off + nb] = lbl.reshape(-1).view(np.uint8)
-                lbl_off = off
-                off += (nb + 3) // 4 * 4
-            # cv::resize: inv_scale = dsize / ssize, scale = 1. / inv_scale — float64, computed here so the kernel sees the same bits
-            table[b] = (img_off, lbl_off, 1.0 / (int(w) / W), 1.0 / (int(h) / H), H, W, int(h), int(w), int(y0), int(x0), int(bool(flip)), lb)
-        host[:B * _SCALE_ENTRY.itemsize] = table.view(np.uint8)
-        self.last_staged_bytes = off
-        dev = self._host[slot][:off].to(self.device, non_blocking=True)
-        ev = torch.cuda.Event()
-        ev.record()
-        self._events[slot] = ev
-        return ops.augment_scale_batch_u8(dev, dev[:B * _SCALE_ENTRY.itemsize], B, self.crop, self.crop, self.mean, self.std,
-                                          want_labels=want_labels)
 
-    def stage_full(self, samples):
+        def record(b, img_off, lbl_off, H, W, lb):
+            _, _, h, w, y0, x0, flip = samples[b]
+            # cv::resize: inv_scale = dsize / ssize, scale = 1. / inv_scale — float64, computed here so the kernel sees the same bits
+            return (img_off, lbl_off, 1.0 / (int(w) / W), 1.0 / (int(h) / H), H, W, int(h), int(w), int(y0), int(x0), int(bool(flip)), lb)
+
+        dev, _ = self._stage_raw(samples, _SCALE_ENTRY, record)
+        return ops.augment_scale_batch_u8(dev, dev[:B * _SCALE_ENTRY.itemsize], B, self.crop, self.crop, self.mean, self.std,
+                                          want_labels=samples[0][1] is not None)
+
+    def stage_full(self, samples, sigmas=None):
         """(bit-exact against the staged oracle, tests/test_data_tail_gpu.py.)  samples: sequence of
         (RAW image, RAW label or None, h, w, angle or None, y0, x0, flip): resize to h x w, rotate by `angle` degrees about the
-        centre (base_dataset.py:77-83), pad / crop / flip / normalise — one kernel (`seg_augment_full_batch_u8`)."""
+        centre (base_dataset.py:77-83), pad / crop / flip / normalise — one kernel (`seg_augment_full_batch_u8`).
+        sigmas: per-sample Gaussian blur sigma or None (draw_blur; base_dataset.py:114-119), applied after the flip; when any
+        sample's kernel size is 3 the batch runs `seg_augment_full_blur_batch_u8`, whose k = 1 samples are bit-identical
+        to the unblurred kernel's."""
         assert _FULL_ENTRY.itemsize == lib.load().seg_aug_full_entry_bytes()
         B = len(samples)
         check_crop_origins(self.crop, [(s[2], s[3], s[5], s[6]) for s in samples])
-        slot = self._slot
-        self._slot ^= 1
-        if self._events[slot] is not None:
-            self._events[slot].synchronize()
-        host = self._host[slot].numpy()
-        table = np.zeros(B, dtype=_FULL_ENTRY)
-        off = B * _FULL_ENTRY.itemsize
-        want_labels = samples[0][1] is not None
-        for b, (img, lbl, h, w, angle, y0, x0, flip) in enumerate(samples):
-            img = np.ascontiguousarray(img, dtype=np.uint8)
-            H, W = img.shape[:2]
-            assert img.shape == (H, W, 3), "images are HWC uint8 with 3 channels"
-            n = img.size
-            lb, lbl_off = 1, -1
-            if lbl is not None:
-                lbl = np.ascontiguousarray(lbl)
-                assert lbl.shape == (H, W) and lbl.dtype in (np.uint8, np.int32), "labels are uint8 or int32 [H,W]"
-                lb = lbl.dtype.itemsize
-            if off + n + 8 + (H * W * lb if lbl is not None else 0) > self.capacity:
-                raise RuntimeError(f"DeviceBatcher: batch needs more than max_bytes={self.capacity} of staging memory")
-            host[off:off + n] = img.reshape(-1)
-            img_off = off
-            off += (n + 3) // 4 * 4
-            if lbl is not None:
-                nb = H * W * lb
-                host[off:off + nb] = lbl.reshape(-1).view(np.uint8)
-                lbl_off = off
-                off += (nb + 3) // 4 * 4
-            table[b] = (img_off, lbl_off, 1.0 / (int(w) / W), 1.0 / (int(h) / H)) + inverse_rotation(int(w), int(h), angle) + \
-                       (H, W, int(h), int(w), int(y0), int(x0), int(bool(flip)), lb)
-        host[:B * _FULL_ENTRY.itemsize] = table.view(np.uint8)
-        self.last_staged_bytes = off
-        dev = self._host[slot][:off].to(self.device, non_blocking=True)
-        ev = torch.cuda.Event()
-        ev.record()
-        self._events[slot] = ev
-        return ops.augment_full_batch_u8(dev, dev[:B * _FULL_ENTRY.itemsize], B, self.crop, self.crop, self.mean, self.std,
-                                         want_labels=want_labels)
+        taps = None
+        if sigmas is not None:
+            if len(sigmas) != B:
+                raise ValueError(f"DeviceBatcher: {len(sigmas)} blur sigmas for {B} samples")
+            taps = np.array([gaussian_taps(s) for s in sigmas], dtype=np.float32)
+            if (taps[:, 1] == 0).all():
+                taps = None  # nothing to blur: the unblurred kernel gives the same bytes
+
+        def record(b, img_off, lbl_off, H, W, lb):
+            _, _, h, w, angle, y0, x0, flip = samples[b]
+            return (img_off, lbl_off, 1.0 / (int(w) / W), 1.0 / (int(h) / H)) + inverse_rotation(int(w), int(h), angle) + \
+                (H, W, int(h), int(w), int(y0), int(x0), int(bool(flip)), lb)
+
+        dev, head_off = self._stage_raw(samples, _FULL_ENTRY, record, head=taps)
+        tab, want_labels = dev[:B * _FULL_ENTRY.itemsize], samples[0][1] is not None
+        if taps is None:
+            return ops.augment_full_batch_u8(dev, tab, B, self.crop, self.crop, self.mean, self.std, want_labels=want_labels)
+        dtaps = dev[head_off:head_off + taps.nbytes].view(torch.float32)
+        return ops.augment_full_blur_batch_u8(dev, tab, dtaps, B, self.crop, self.crop, self.mean, self.std, want_labels=want_labels)
+
+    def stage_val(self, samples):
+        """The validation tail of base_dataset.py:40-61 and :129-136.  samples: sequence of (RAW image uint8 [H,W,3], RAW label
+        uint8|int32 [H,W] or None).  Each sample is resized so that its short side is crop_size (cv2.resize INTER_LINEAR on
+        the image, PIL's NEAREST on the label, negative labels kept), centre-cropped, truncated to uint8 and normalised — one
+        kernel (`seg_augment_val_batch_u8`), no resized intermediate."""
+        assert _SCALE_ENTRY.itemsize == lib.load().seg_aug_scale_entry_bytes()
+        B = len(samples)
+        for b, s in enumerate(samples):
+            if len(s) != 2:
+                raise ValueError(f"DeviceBatcher.stage_val: sample {b} is not an (image, label) pair")
+            im, lb = s
+            if np.ndim(im) != 3 or np.shape(im)[2] != 3 or min(np.shape(im)[:2]) < 1:
+                raise ValueError(f"DeviceBatcher.stage_val: sample {b}: image of shape {np.shape(im)} is not [H, W, 3]")
+            if lb is not None and tuple(np.shape(lb)) != tuple(np.shape(im)[:2]):
+                raise ValueError(f"DeviceBatcher.stage_val: sample {b}: label of shape {np.shape(lb)} for a {np.shape(im)} image")
+            if (lb is None) != (samples[0][1] is None):
+                raise ValueError("DeviceBatcher.stage_val: either every sample has a label or none has")
+        geom = [val_geometry(np.shape(s[0])[0], np.shape(s[0])[1], self.crop) for s in samples]
+        check_crop_origins(self.crop, [(h, w, y0, x0) for h, w, y0, x0 in geom])
+
+        def record(b, img_off, lbl_off, H, W, lb):
+            h, w, y0, x0 = geom[b]
+            return (img_off, lbl_off, 1.0 / (w / W), 1.0 / (h / H), H, W, h, w, y0, x0, 0, lb)
+
+        def tables(b, H, W):
+            h, w = geom[b][:2]
+            return np.concatenate([pil_nearest_index(W, w), pil_nearest_index(H, h)])
+
+        dev, _ = self._stage_raw(samples, _SCALE_ENTRY, record, tail=tables)
+        return ops.augment_val_batch_u8(dev, dev[:B * _SCALE_ENTRY.itemsize], B, self.crop, self.crop, self.mean, self.std,
+                                        want_labels=samples[0][1] is not None)
 
     def stage_random(self, raw, flip=True, rng=random):
         """raw: sequence of (image, label).  Draws crop origin / flip per sample like the reference's worker would."""
@@ -237,8 +322,9 @@ class DevicePrefetcher:
     """base/base_dataloader.py:49-85 with the same protocol (`len`, iteration yields (input, target) on the device, the
     next batch is staged on a side stream while the current one is consumed, `stop_after`)."""
 
-    def __init__(self, loader, device, stop_after=None, batcher=None):
+    def __init__(self, loader, device, stop_after=None, batcher=None, val=False):
         self.loader = loader
+        self.val = val  # raw batches are (image, label) pairs of a validation loader: batcher.stage_val
         self.dataset = getattr(loader, "dataset", None)
         self.stream = torch.cuda.Stream()
         self.stop_after = stop_after
@@ -264,7 +350,7 @@ class DevicePrefetcher:
             else:
                 if self.batcher is None:
                     raise RuntimeError("DevicePrefetcher: the loader yields raw uint8 samples but no DeviceBatcher was given")
-                self.next_input, self.next_target = self.batcher.stage(item)
+                self.next_input, self.next_target = (self.batcher.stage_val if self.val else self.batcher.stage)(item)
 
     def __iter__(self):
         count = 0

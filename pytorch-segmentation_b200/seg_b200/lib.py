@@ -138,6 +138,9 @@ _SIGS = {
     "seg_augment_scale_batch_u8": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, POINTER(c_float), POINTER(c_float), c_void_p, c_void_p, c_void_p]),
     "seg_aug_full_entry_bytes": (c_int, []),
     "seg_augment_full_batch_u8": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, POINTER(c_float), POINTER(c_float), c_void_p, c_void_p, c_void_p]),
+    "seg_augment_val_batch_u8": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, POINTER(c_float), POINTER(c_float), c_void_p, c_void_p, c_void_p]),
+    "seg_augment_full_blur_batch_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, POINTER(c_float), POINTER(c_float), c_void_p,
+                                               c_void_p, c_void_p]),
     "seg_resize_nchw_f32": (c_int, [c_void_p, c_int64, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int, c_float, c_float, c_void_p]),
     "seg_window_add_nchw_f32": (c_int, [c_void_p, c_int64, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "seg_div_by_count_nchw_f32": (c_int, [c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p]),

@@ -932,3 +932,29 @@ def augment_full_batch_u8(arena, table, B, crop_h, crop_w, mean, std, want_label
     s3 = (ctypes.c_float * 3)(*[float(v) for v in std])
     call("seg_augment_full_batch_u8", ptr(arena), ptr(table), int(B), int(crop_h), int(crop_w), m3, s3, ptr(out), ptr(labels))
     return out, labels
+
+
+def augment_val_batch_u8(arena, table, B, crop_h, crop_w, mean, std, want_labels=True):
+    """The validation tail (resize so the short side is the crop, centre crop, ToTensor, Normalize) on B seg_aug_scale_entry
+    records; each label map in the arena is followed by its PIL NEAREST index tables (x then y, int32)."""
+    assert arena.dtype == torch.uint8 and table.dtype == torch.uint8 and table.numel() == B * lib.load().seg_aug_scale_entry_bytes()
+    out = torch.empty((B, 3, crop_h, crop_w), dtype=torch.float32, device=arena.device)
+    labels = torch.empty((B, crop_h, crop_w), dtype=torch.int64, device=arena.device) if want_labels else None
+    m3 = (ctypes.c_float * 3)(*[float(v) for v in mean])
+    s3 = (ctypes.c_float * 3)(*[float(v) for v in std])
+    call("seg_augment_val_batch_u8", ptr(arena), ptr(table), int(B), int(crop_h), int(crop_w), m3, s3, ptr(out), ptr(labels))
+    return out, labels
+
+
+def augment_full_blur_batch_u8(arena, table, taps, B, crop_h, crop_w, mean, std, want_labels=True):
+    """augment_full_batch_u8 with the Gaussian blur after the flip; taps: float32 device tensor [B, 2] of (centre, side)
+    taps, (1, 0) for a sample that is not blurred."""
+    assert arena.dtype == torch.uint8 and table.dtype == torch.uint8 and table.numel() == B * lib.load().seg_aug_full_entry_bytes()
+    assert taps.dtype == torch.float32 and taps.is_contiguous() and taps.numel() == 2 * B and taps.device == arena.device
+    out = torch.empty((B, 3, crop_h, crop_w), dtype=torch.float32, device=arena.device)
+    labels = torch.empty((B, crop_h, crop_w), dtype=torch.int64, device=arena.device) if want_labels else None
+    m3 = (ctypes.c_float * 3)(*[float(v) for v in mean])
+    s3 = (ctypes.c_float * 3)(*[float(v) for v in std])
+    call("seg_augment_full_blur_batch_u8", ptr(arena), ptr(table), ptr(taps), int(B), int(crop_h), int(crop_w), m3, s3, ptr(out),
+         ptr(labels))
+    return out, labels
