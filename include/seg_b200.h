@@ -484,6 +484,25 @@ int seg_augment_full_batch_u8(const uint8_t* arena, const seg_aug_full_entry* ta
 int seg_augment_full_blur_batch_u8(const uint8_t* arena, const seg_aug_full_entry* table, const float* blur_taps, int B, int crop_h,
                                    int crop_w, const float* mean3, const float* std3, float* out_nchw, int64_t* out_labels,
                                    void* stream);
+/* ---- label maps: the *_mapped twins of the five augmentation entry points take the same arguments and records and also
+ * accept lbl_bytes = 1 | SEG_AUG_LABEL_MAP: the sample's uint8 label map is followed, at the next 4-byte boundary, by 256
+ * int32 entries `map`, and every label read from the raw map is map[raw] (a dataset's id -> train-id table, applied where
+ * the reference applies it: before the resize, rotation and padding).  Fill values — the zero padding of copyMakeBorder and
+ * warpAffine's constant-0 border — are post-map values and stay 0.  The validation kernel's PIL index tables follow the
+ * map.  The flag is valid with 1-byte labels only (the host packer refuses anything else); records without it read their
+ * labels exactly as the entry points above do. */
+#define SEG_AUG_LABEL_MAP 256
+int seg_augment_mapped_batch_u8(const uint8_t* arena, const seg_aug_entry* table, int B, int crop_h, int crop_w, const float* mean3,
+                                const float* std3, float* out_nchw, int64_t* out_labels, void* stream);
+int seg_augment_scale_mapped_batch_u8(const uint8_t* arena, const seg_aug_scale_entry* table, int B, int crop_h, int crop_w,
+                                      const float* mean3, const float* std3, float* out_nchw, int64_t* out_labels, void* stream);
+int seg_augment_val_mapped_batch_u8(const uint8_t* arena, const seg_aug_scale_entry* table, int B, int crop_h, int crop_w,
+                                    const float* mean3, const float* std3, float* out_nchw, int64_t* out_labels, void* stream);
+int seg_augment_full_mapped_batch_u8(const uint8_t* arena, const seg_aug_full_entry* table, int B, int crop_h, int crop_w,
+                                     const float* mean3, const float* std3, float* out_nchw, int64_t* out_labels, void* stream);
+int seg_augment_full_blur_mapped_batch_u8(const uint8_t* arena, const seg_aug_full_entry* table, const float* blur_taps, int B,
+                                          int crop_h, int crop_w, const float* mean3, const float* std3, float* out_nchw,
+                                          int64_t* out_labels, void* stream);
 /* ---- inference-side resampling (SURVEY.md §8f row 3; inference.py:26-79), fp32 NCHW score maps, `planes` = N*C ----
  * resize: dst = beta*dst + alpha*flip_x?(bilinear resize of src to Hd x Wd).  mode 0 / 1 = ATen bilinear with
  * align_corners False / True (1 = nn.Upsample(align_corners=True), inference.py:60; same size + flip_x = tensor.flip(-1),

@@ -25,6 +25,25 @@ struct AugParams {
   float mean[3];
   float stdv[3];
 };
+
+// Label maps (SEG_AUG_LABEL_MAP in a record's lbl_bytes): a raw uint8 label map of n pixels is followed, at the next
+// 4-byte boundary, by 256 int32 entries, and the label read at index k is map[raw[k]] (a dataset's id -> train-id table,
+// cityscapes.py:53-54, applied where the reference applies it: in _load_data, before any resize, rotation or padding).
+// Fill values (the zero padding, the rotation's constant border) are post-map values and never go through the map.
+// LabelMap = false instantiates exactly the reads the kernels had before label maps existed.
+template <bool LabelMap>
+__device__ __forceinline__ const int32_t* label_map_of(const uint8_t* lbl, int lbl_bytes, int64_t n) {
+  if constexpr (LabelMap)
+    return (lbl != nullptr && (lbl_bytes & SEG_AUG_LABEL_MAP)) ? reinterpret_cast<const int32_t*>(lbl + (n + 3) / 4 * 4) : nullptr;
+  return nullptr;
+}
+template <bool LabelMap>
+__device__ __forceinline__ int read_label(const uint8_t* lbl, const int32_t* lmap, int lbl_bytes, int64_t k) {
+  if constexpr (LabelMap)
+    if (lmap != nullptr) return __ldg(lmap + lbl[k]);
+  return lbl_bytes == 1 ? (int)lbl[k] : reinterpret_cast<const int32_t*>(lbl)[k];
+}
+template <bool LabelMap>
 __global__ void __launch_bounds__(256) augment_u8_kernel(const uint8_t* __restrict__ arena, const seg_aug_entry* __restrict__ table,
                                                          int crop_h, int crop_w, AugParams prm, float* __restrict__ out,
                                                          int64_t* __restrict__ labels) {
@@ -41,6 +60,7 @@ __global__ void __launch_bounds__(256) augment_u8_kernel(const uint8_t* __restri
   const seg_aug_entry e = table[b];
   const uint8_t* img = arena + e.img_off;
   const uint8_t* lbl = (e.lbl_off >= 0 && labels != nullptr) ? arena + e.lbl_off : nullptr;
+  const int32_t* lmap = label_map_of<LabelMap>(lbl, e.lbl_bytes, (int64_t)e.h * e.w);
   const int plane = crop_h * crop_w;  // < 2^31 (checked on the host)
   float* o = out + (int64_t)b * 3 * plane;
   int64_t* lo = labels != nullptr ? labels + (int64_t)b * plane : nullptr;
@@ -65,7 +85,7 @@ __global__ void __launch_bounds__(256) augment_u8_kernel(const uint8_t* __restri
           r[u] = p[0];
           g[u] = p[1];
           bl[u] = p[2];
-          if (lbl != nullptr) lab[u] = e.lbl_bytes == 1 ? (int)lbl[k] : reinterpret_cast<const int32_t*>(lbl)[k];
+          if (lbl != nullptr) lab[u] = read_label<LabelMap>(lbl, lmap, e.lbl_bytes, k);
         }
       }
     }
@@ -118,7 +138,7 @@ __device__ __forceinline__ void cv_linear_coord(int d, double scale, int src, bo
 // half of the size pairs some index differs from floor((d + 0.5) * a).  The host runs the same additions and appends the
 // two int32 index tables (x: w entries, then y: h entries) to the label map in the arena, 4-byte aligned; the kernel looks
 // them up.  The image arithmetic is the same in both instantiations.
-template <bool PilLabels>
+template <bool PilLabels, bool LabelMap>
 __global__ void __launch_bounds__(256) augment_scale_u8_kernel(const uint8_t* __restrict__ arena,
                                                                const seg_aug_scale_entry* __restrict__ table, int crop_h, int crop_w,
                                                                AugParams prm, float* __restrict__ out, int64_t* __restrict__ labels) {
@@ -132,6 +152,7 @@ __global__ void __launch_bounds__(256) augment_scale_u8_kernel(const uint8_t* __
   const seg_aug_scale_entry e = table[b];
   const uint8_t* img = arena + e.img_off;
   const uint8_t* lbl = (e.lbl_off >= 0 && labels != nullptr) ? arena + e.lbl_off : nullptr;
+  const int32_t* lmap = label_map_of<LabelMap>(lbl, e.lbl_bytes, (int64_t)e.src_h * e.src_w);
   const int plane = crop_h * crop_w;
   float* o = out + (int64_t)b * 3 * plane;
   int64_t* lo = labels != nullptr ? labels + (int64_t)b * plane : nullptr;
@@ -167,7 +188,9 @@ __global__ void __launch_bounds__(256) augment_scale_u8_kernel(const uint8_t* __
       if (lbl != nullptr) {
         int lx, ly;
         if constexpr (PilLabels) {
-          const int32_t* tab = reinterpret_cast<const int32_t*>(lbl + ((int64_t)e.src_h * e.src_w * e.lbl_bytes + 3) / 4 * 4);
+          // the index tables follow the label map, and its 256-entry id table when there is one
+          const int32_t* tab = (LabelMap && lmap != nullptr) ? lmap + 256
+                                                             : reinterpret_cast<const int32_t*>(lbl + ((int64_t)e.src_h * e.src_w * e.lbl_bytes + 3) / 4 * 4);
           lx = tab[dx];
           ly = tab[e.w + dy];
         } else {
@@ -177,7 +200,7 @@ __global__ void __launch_bounds__(256) augment_scale_u8_kernel(const uint8_t* __
           ly = ly < e.src_h - 1 ? ly : e.src_h - 1;
         }
         const int64_t k = (int64_t)ly * e.src_w + lx;
-        lab = e.lbl_bytes == 1 ? (int)lbl[k] : reinterpret_cast<const int32_t*>(lbl)[k];
+        lab = read_label<LabelMap>(lbl, lmap, e.lbl_bytes, k);
       }
     }
     o[i] = lut[0][r];
@@ -218,13 +241,15 @@ __device__ __forceinline__ void resized_pixel_f32(const uint8_t* __restrict__ im
   }
 }
 
-__device__ __forceinline__ int resized_label(const uint8_t* __restrict__ lbl, const seg_aug_full_entry& e, int ry, int rx) {
+template <bool LabelMap>
+__device__ __forceinline__ int resized_label(const uint8_t* __restrict__ lbl, const int32_t* lmap, const seg_aug_full_entry& e, int ry,
+                                             int rx) {
   if (ry < 0 || ry >= e.h || rx < 0 || rx >= e.w) return 0;
   int lx = (int)floor(__dmul_rn((double)rx, e.scale_x)), ly = (int)floor(__dmul_rn((double)ry, e.scale_y));
   lx = lx < e.src_w - 1 ? lx : e.src_w - 1;
   ly = ly < e.src_h - 1 ? ly : e.src_h - 1;
   const int64_t k = (int64_t)ly * e.src_w + lx;
-  return e.lbl_bytes == 1 ? (int)lbl[k] : reinterpret_cast<const int32_t*>(lbl)[k];
+  return read_label<LabelMap>(lbl, lmap, e.lbl_bytes, k);
 }
 
 // INTER_NEAREST uses delta = AB_SCALE / 2 on the same rounded row / column terms
@@ -268,11 +293,14 @@ __device__ __forceinline__ unsigned trunc_u8(float v) {
   return r > 255u ? 255u : r;
 }
 
-__device__ __forceinline__ int rotated_label(const uint8_t* __restrict__ lbl, const seg_aug_full_entry& e, const RotCoords& q) {
+template <bool LabelMap>
+__device__ __forceinline__ int rotated_label(const uint8_t* __restrict__ lbl, const int32_t* lmap, const seg_aug_full_entry& e,
+                                             const RotCoords& q) {
   const long long X = rowX_nearest_fix(q.rowX, q.colX), Y = rowX_nearest_fix(q.rowY, q.colY);
-  return resized_label(lbl, e, (int)(Y >> 10), (int)(X >> 10));
+  return resized_label<LabelMap>(lbl, lmap, e, (int)(Y >> 10), (int)(X >> 10));
 }
 
+template <bool LabelMap>
 __global__ void __launch_bounds__(256) augment_full_u8_kernel(const uint8_t* __restrict__ arena, const seg_aug_full_entry* __restrict__ table,
                                                               int crop_h, int crop_w, AugParams prm, float* __restrict__ out,
                                                               int64_t* __restrict__ labels) {
@@ -286,6 +314,7 @@ __global__ void __launch_bounds__(256) augment_full_u8_kernel(const uint8_t* __r
   const seg_aug_full_entry e = table[b];
   const uint8_t* img = arena + e.img_off;
   const uint8_t* lbl = (e.lbl_off >= 0 && labels != nullptr) ? arena + e.lbl_off : nullptr;
+  const int32_t* lmap = label_map_of<LabelMap>(lbl, e.lbl_bytes, (int64_t)e.src_h * e.src_w);
   const int plane = crop_h * crop_w;
   float* o = out + (int64_t)b * 3 * plane;
   int64_t* lo = labels != nullptr ? labels + (int64_t)b * plane : nullptr;
@@ -303,7 +332,7 @@ __global__ void __launch_bounds__(256) augment_full_u8_kernel(const uint8_t* __r
       r = trunc_u8(v[0]);
       g = trunc_u8(v[1]);
       bl = trunc_u8(v[2]);
-      if (lbl != nullptr) lab = rotated_label(lbl, e, q);
+      if (lbl != nullptr) lab = rotated_label<LabelMap>(lbl, lmap, e, q);
     }
     o[i] = lut[0][r];
     o[plane + i] = lut[1][g];
@@ -328,6 +357,7 @@ constexpr int BLUR_TY = 16, BLUR_TX = 32;
 
 __device__ __forceinline__ int reflect101(int i, int n) { return n == 1 ? 0 : (i < 0 ? -i : (i >= n ? 2 * n - 2 - i : i)); }
 
+template <bool LabelMap>
 __global__ void __launch_bounds__(256) augment_full_blur_u8_kernel(const uint8_t* __restrict__ arena,
                                                                    const seg_aug_full_entry* __restrict__ table,
                                                                    const float* __restrict__ blur_taps, int crop_h, int crop_w,
@@ -368,6 +398,7 @@ __global__ void __launch_bounds__(256) augment_full_blur_u8_kernel(const uint8_t
   }
   __syncthreads();
   const uint8_t* lbl = (e.lbl_off >= 0 && labels != nullptr) ? arena + e.lbl_off : nullptr;
+  const int32_t* lmap = label_map_of<LabelMap>(lbl, e.lbl_bytes, (int64_t)e.src_h * e.src_w);
   const int plane = crop_h * crop_w;
   float* o = out + (int64_t)b * 3 * plane;
   int64_t* lo = labels != nullptr ? labels + (int64_t)b * plane : nullptr;
@@ -385,7 +416,7 @@ __global__ void __launch_bounds__(256) augment_full_blur_u8_kernel(const uint8_t
     o[2 * (int64_t)plane + i] = lut[2][u[2]];
     if (lo != nullptr) {
       const int dy = y + e.y0, dx = xs + e.x0;
-      lo[i] = (dy < e.h && dx < e.w && lbl != nullptr) ? (int64_t)rotated_label(lbl, e, rot_coords(e, dy, dx)) : 0;
+      lo[i] = (dy < e.h && dx < e.w && lbl != nullptr) ? (int64_t)rotated_label<LabelMap>(lbl, lmap, e, rot_coords(e, dy, dx)) : 0;
     }
   }
 }
@@ -517,16 +548,35 @@ using namespace seg;
 extern "C" {
 
 int seg_aug_entry_bytes(void) { return (int)sizeof(seg_aug_entry); }
+int seg_aug_scale_entry_bytes(void) { return (int)sizeof(seg_aug_scale_entry); }
+int seg_aug_full_entry_bytes(void) { return (int)sizeof(seg_aug_full_entry); }
 
-int seg_augment_batch_u8(const uint8_t* arena, const seg_aug_entry* table, int B, int crop_h, int crop_w, const float* mean3,
-                         const float* std3, float* out_nchw, int64_t* out_labels, void* stream) {
-  SEG_REQUIRE(arena != nullptr && table != nullptr && out_nchw != nullptr && mean3 != nullptr && std3 != nullptr, "augment: null pointer");
-  SEG_REQUIRE(B > 0 && B <= 65535 && crop_h > 0 && crop_w > 0 && (int64_t)crop_h * crop_w < (1ll << 30), "augment: bad batch / crop size");
+}  // extern "C"
+
+namespace {
+
+// Kernel launches of the augmentation entry points; LabelMap = true only for the *_mapped twins.
+enum AugKind { AUG_PLAIN, AUG_SCALE, AUG_VAL, AUG_FULL, AUG_FULL_BLUR };
+
+template <bool LabelMap>
+int launch_augment(AugKind kind, const char* name, const uint8_t* arena, const void* table, const float* blur_taps, int B, int crop_h,
+                   int crop_w, const float* mean3, const float* std3, float* out_nchw, int64_t* out_labels, void* stream) {
+  SEG_REQUIRE(arena != nullptr && table != nullptr && out_nchw != nullptr && mean3 != nullptr && std3 != nullptr &&
+                  (kind != AUG_FULL_BLUR || blur_taps != nullptr),
+              "%s: null pointer", name);
+  SEG_REQUIRE(B > 0 && B <= 65535 && crop_h > 0 && crop_w > 0 && (int64_t)crop_h * crop_w < (1ll << 30), "%s: bad batch / crop size", name);
   AugParams prm;
   for (int c = 0; c < 3; ++c) {
     prm.mean[c] = mean3[c];  // host pointers: six floats by value into the kernel arguments
     prm.stdv[c] = std3[c];
-    SEG_REQUIRE(std3[c] != 0.f, "augment: std must be non-zero");
+    SEG_REQUIRE(std3[c] != 0.f, "%s: std must be non-zero", name);
+  }
+  if (kind == AUG_FULL_BLUR) {
+    const int64_t tiles_x = ceil_div64(crop_w, BLUR_TX), tiles = tiles_x * ceil_div64(crop_h, BLUR_TY);  // < 2^31 for crop_h * crop_w < 2^30
+    dim3 grid((unsigned)tiles, (unsigned)B, 1);
+    augment_full_blur_u8_kernel<LabelMap><<<grid, 256, 0, ST(stream)>>>(arena, static_cast<const seg_aug_full_entry*>(table), blur_taps,
+                                                                        crop_h, crop_w, (int)tiles_x, prm, out_nchw, out_labels);
+    return check_launch(name);
   }
   // blockIdx.y = image; the B images share ~8 blocks per SM between them
   int64_t per_image = ((int64_t)num_sms() * 8 + B - 1) / B;
@@ -534,87 +584,57 @@ int seg_augment_batch_u8(const uint8_t* arena, const seg_aug_entry* table, int B
   if (per_image > need) per_image = need;
   if (per_image < 1) per_image = 1;
   dim3 grid((unsigned)per_image, (unsigned)B, 1);
-  augment_u8_kernel<<<grid, 256, 0, ST(stream)>>>(arena, table, crop_h, crop_w, prm, out_nchw, out_labels);
-  return check_launch("augment_batch_u8");
-}
-
-int seg_aug_scale_entry_bytes(void) { return (int)sizeof(seg_aug_scale_entry); }
-
-int seg_augment_scale_batch_u8(const uint8_t* arena, const seg_aug_scale_entry* table, int B, int crop_h, int crop_w,
-                               const float* mean3, const float* std3, float* out_nchw, int64_t* out_labels, void* stream) {
-  SEG_REQUIRE(arena != nullptr && table != nullptr && out_nchw != nullptr && mean3 != nullptr && std3 != nullptr, "augment_scale: null pointer");
-  SEG_REQUIRE(B > 0 && B <= 65535 && crop_h > 0 && crop_w > 0 && (int64_t)crop_h * crop_w < (1ll << 30), "augment_scale: bad batch / crop size");
-  AugParams prm;
-  for (int c = 0; c < 3; ++c) {
-    prm.mean[c] = mean3[c];
-    prm.stdv[c] = std3[c];
-    SEG_REQUIRE(std3[c] != 0.f, "augment_scale: std must be non-zero");
+  switch (kind) {
+    case AUG_PLAIN:
+      augment_u8_kernel<LabelMap><<<grid, 256, 0, ST(stream)>>>(arena, static_cast<const seg_aug_entry*>(table), crop_h, crop_w, prm,
+                                                                out_nchw, out_labels);
+      break;
+    case AUG_SCALE:
+      augment_scale_u8_kernel<false, LabelMap><<<grid, 256, 0, ST(stream)>>>(arena, static_cast<const seg_aug_scale_entry*>(table), crop_h,
+                                                                             crop_w, prm, out_nchw, out_labels);
+      break;
+    case AUG_VAL:
+      augment_scale_u8_kernel<true, LabelMap><<<grid, 256, 0, ST(stream)>>>(arena, static_cast<const seg_aug_scale_entry*>(table), crop_h,
+                                                                            crop_w, prm, out_nchw, out_labels);
+      break;
+    default:
+      augment_full_u8_kernel<LabelMap><<<grid, 256, 0, ST(stream)>>>(arena, static_cast<const seg_aug_full_entry*>(table), crop_h, crop_w,
+                                                                     prm, out_nchw, out_labels);
   }
-  int64_t per_image = ((int64_t)num_sms() * 8 + B - 1) / B;
-  const int64_t need = ceil_div64((int64_t)crop_h * crop_w, 256);
-  if (per_image > need) per_image = need;
-  if (per_image < 1) per_image = 1;
-  dim3 grid((unsigned)per_image, (unsigned)B, 1);
-  augment_scale_u8_kernel<false><<<grid, 256, 0, ST(stream)>>>(arena, table, crop_h, crop_w, prm, out_nchw, out_labels);
-  return check_launch("augment_scale_batch_u8");
+  return check_launch(name);
 }
 
-int seg_augment_val_batch_u8(const uint8_t* arena, const seg_aug_scale_entry* table, int B, int crop_h, int crop_w,
-                             const float* mean3, const float* std3, float* out_nchw, int64_t* out_labels, void* stream) {
-  SEG_REQUIRE(arena != nullptr && table != nullptr && out_nchw != nullptr && mean3 != nullptr && std3 != nullptr, "augment_val: null pointer");
-  SEG_REQUIRE(B > 0 && B <= 65535 && crop_h > 0 && crop_w > 0 && (int64_t)crop_h * crop_w < (1ll << 30), "augment_val: bad batch / crop size");
-  AugParams prm;
-  for (int c = 0; c < 3; ++c) {
-    prm.mean[c] = mean3[c];
-    prm.stdv[c] = std3[c];
-    SEG_REQUIRE(std3[c] != 0.f, "augment_val: std must be non-zero");
+}  // namespace
+
+extern "C" {
+
+#define SEG_AUG_ENTRY(fn, kind, rec, mapped)                                                                                       \
+  int fn(const uint8_t* arena, const rec* table, int B, int crop_h, int crop_w, const float* mean3, const float* std3, float* out_nchw, \
+         int64_t* out_labels, void* stream) {                                                                                         \
+    return launch_augment<mapped>(kind, #fn, arena, table, nullptr, B, crop_h, crop_w, mean3, std3, out_nchw, out_labels, stream);   \
   }
-  int64_t per_image = ((int64_t)num_sms() * 8 + B - 1) / B;
-  const int64_t need = ceil_div64((int64_t)crop_h * crop_w, 256);
-  if (per_image > need) per_image = need;
-  if (per_image < 1) per_image = 1;
-  dim3 grid((unsigned)per_image, (unsigned)B, 1);
-  augment_scale_u8_kernel<true><<<grid, 256, 0, ST(stream)>>>(arena, table, crop_h, crop_w, prm, out_nchw, out_labels);
-  return check_launch("augment_val_batch_u8");
-}
-
-int seg_aug_full_entry_bytes(void) { return (int)sizeof(seg_aug_full_entry); }
-
-int seg_augment_full_batch_u8(const uint8_t* arena, const seg_aug_full_entry* table, int B, int crop_h, int crop_w,
-                              const float* mean3, const float* std3, float* out_nchw, int64_t* out_labels, void* stream) {
-  SEG_REQUIRE(arena != nullptr && table != nullptr && out_nchw != nullptr && mean3 != nullptr && std3 != nullptr, "augment_full: null pointer");
-  SEG_REQUIRE(B > 0 && B <= 65535 && crop_h > 0 && crop_w > 0 && (int64_t)crop_h * crop_w < (1ll << 30), "augment_full: bad batch / crop size");
-  AugParams prm;
-  for (int c = 0; c < 3; ++c) {
-    prm.mean[c] = mean3[c];
-    prm.stdv[c] = std3[c];
-    SEG_REQUIRE(std3[c] != 0.f, "augment_full: std must be non-zero");
-  }
-  int64_t per_image = ((int64_t)num_sms() * 8 + B - 1) / B;
-  const int64_t need = ceil_div64((int64_t)crop_h * crop_w, 256);
-  if (per_image > need) per_image = need;
-  if (per_image < 1) per_image = 1;
-  dim3 grid((unsigned)per_image, (unsigned)B, 1);
-  augment_full_u8_kernel<<<grid, 256, 0, ST(stream)>>>(arena, table, crop_h, crop_w, prm, out_nchw, out_labels);
-  return check_launch("augment_full_batch_u8");
-}
+SEG_AUG_ENTRY(seg_augment_batch_u8, AUG_PLAIN, seg_aug_entry, false)
+SEG_AUG_ENTRY(seg_augment_scale_batch_u8, AUG_SCALE, seg_aug_scale_entry, false)
+SEG_AUG_ENTRY(seg_augment_val_batch_u8, AUG_VAL, seg_aug_scale_entry, false)
+SEG_AUG_ENTRY(seg_augment_full_batch_u8, AUG_FULL, seg_aug_full_entry, false)
+SEG_AUG_ENTRY(seg_augment_mapped_batch_u8, AUG_PLAIN, seg_aug_entry, true)
+SEG_AUG_ENTRY(seg_augment_scale_mapped_batch_u8, AUG_SCALE, seg_aug_scale_entry, true)
+SEG_AUG_ENTRY(seg_augment_val_mapped_batch_u8, AUG_VAL, seg_aug_scale_entry, true)
+SEG_AUG_ENTRY(seg_augment_full_mapped_batch_u8, AUG_FULL, seg_aug_full_entry, true)
+#undef SEG_AUG_ENTRY
 
 int seg_augment_full_blur_batch_u8(const uint8_t* arena, const seg_aug_full_entry* table, const float* blur_taps, int B, int crop_h,
                                    int crop_w, const float* mean3, const float* std3, float* out_nchw, int64_t* out_labels,
                                    void* stream) {
-  SEG_REQUIRE(arena != nullptr && table != nullptr && blur_taps != nullptr && out_nchw != nullptr && mean3 != nullptr && std3 != nullptr,
-              "augment_full_blur: null pointer");
-  SEG_REQUIRE(B > 0 && B <= 65535 && crop_h > 0 && crop_w > 0 && (int64_t)crop_h * crop_w < (1ll << 30), "augment_full_blur: bad batch / crop size");
-  AugParams prm;
-  for (int c = 0; c < 3; ++c) {
-    prm.mean[c] = mean3[c];
-    prm.stdv[c] = std3[c];
-    SEG_REQUIRE(std3[c] != 0.f, "augment_full_blur: std must be non-zero");
-  }
-  const int64_t tiles_x = ceil_div64(crop_w, BLUR_TX), tiles = tiles_x * ceil_div64(crop_h, BLUR_TY);  // < 2^31 for crop_h * crop_w < 2^30
-  dim3 grid((unsigned)tiles, (unsigned)B, 1);
-  augment_full_blur_u8_kernel<<<grid, 256, 0, ST(stream)>>>(arena, table, blur_taps, crop_h, crop_w, (int)tiles_x, prm, out_nchw, out_labels);
-  return check_launch("augment_full_blur_batch_u8");
+  return launch_augment<false>(AUG_FULL_BLUR, "seg_augment_full_blur_batch_u8", arena, table, blur_taps, B, crop_h, crop_w, mean3, std3,
+                               out_nchw, out_labels, stream);
+}
+
+int seg_augment_full_blur_mapped_batch_u8(const uint8_t* arena, const seg_aug_full_entry* table, const float* blur_taps, int B,
+                                          int crop_h, int crop_w, const float* mean3, const float* std3, float* out_nchw,
+                                          int64_t* out_labels, void* stream) {
+  return launch_augment<true>(AUG_FULL_BLUR, "seg_augment_full_blur_mapped_batch_u8", arena, table, blur_taps, B, crop_h, crop_w, mean3,
+                              std3, out_nchw, out_labels, stream);
 }
 
 int seg_resize_nchw_f32(const float* src, int64_t planes, int Hs, int Ws, float* dst, int Hd, int Wd, int mode, int flip_x,

@@ -23,3 +23,4 @@ def _find_reference_utils():
 REFERENCE_UTILS = _find_reference_utils()
 if REFERENCE_UTILS is not None:
     __path__.append(REFERENCE_UTILS)
+    from .logger import Logger  # noqa: E402,F401  the reference package's own export (train.py:9 `from utils import Logger`)

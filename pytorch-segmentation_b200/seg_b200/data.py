@@ -11,7 +11,9 @@ for the whole batch, bit-exactly (same fp32 operations).  The random draws stay 
     DevicePrefetcher(loader, device, stop_after=None, batcher=None, val=False) — drop-in for the reference's DataPrefetcher;
         a loader that yields ready (float image batch, long label batch) pairs is passed through exactly as the reference
         does, a loader that yields lists of raw samples goes through the batcher (stage, or stage_val for a validation
-        loader's raw (image, label) pairs when val=True).
+        loader's raw (image, label) pairs when val=True), and a PackedBatch (device_collate, packed in the loader's
+        workers) is copied once and run by the kernel its records call for.
+    pack_arena(...) — the one packer (records, optional head, images, labels, optional label map and tail) behind both.
 """
 import math
 import random
@@ -125,9 +127,203 @@ def check_crop_origins(crop, dims):
                              f"for a {h} x {w} image and crop {crop}")
 
 
+def check_label_map(label_map):
+    """A dataset's id -> train-id table as the kernels read it: 256 int32 entries, indexed by the raw uint8 label."""
+    t = np.ascontiguousarray(label_map, dtype=np.int32).reshape(-1)
+    if t.shape != (256,):
+        raise ValueError(f"label map: {t.size} entries, a uint8 label needs 256")
+    return t
+
+
+def pack_arena(samples, dtype, record, head=None, tail=None, label_map=None, out=None):
+    """The one packer of the device input pipeline: the B `dtype` records first, then `head` (a float32 array, e.g.
+    per-sample blur taps), then every image (HWC uint8) and label map (uint8|int32 [H,W] or None) 4-byte aligned.  After a
+    label map come, in this order: the 256 int32 entries of `label_map` (when given; the label must then be uint8 and its
+    record's lbl_bytes is 1 | lib.AUG_LABEL_MAP), and `tail(b, H, W)` (an int32 array, e.g. the PIL index tables of the
+    validation tail).  record(b, img_off, lbl_off, H, W, lbl_bytes) -> the record of sample b.
+    Writes into `out` (a uint8 tensor, e.g. pinned staging memory; RuntimeError when the batch does not fit) or into a new
+    CPU tensor, and returns the packed prefix: a uint8 tensor of exactly the arena's bytes."""
+    B = len(samples)
+    lmap = check_label_map(label_map) if label_map is not None else None
+    parts, off = [], B * dtype.itemsize
+    if head is not None:
+        head = np.ascontiguousarray(head, dtype=np.float32)
+        off += head.nbytes
+    capacity = out.numel() if out is not None else None
+    for b, s in enumerate(samples):   # sizes and offsets first: nothing is written for a batch that does not fit
+        img, lbl = np.ascontiguousarray(s[0], dtype=np.uint8), s[1]
+        H, W = img.shape[:2]
+        assert img.shape == (H, W, 3), "images are HWC uint8 with 3 channels"
+        n = img.size
+        lb, lbl_off, extra = 1, -1, None
+        if lbl is not None:
+            lbl = np.ascontiguousarray(lbl)
+            assert lbl.shape == (H, W) and lbl.dtype in (np.uint8, np.int32), "labels are uint8 or int32 [H,W]"
+            lb = lbl.dtype.itemsize
+            if lmap is not None and lb != 1:
+                raise ValueError(f"pack_arena: sample {b}: a label map applies to uint8 labels, not {lbl.dtype}")
+            extra = tail(b, H, W) if tail is not None else None
+        need = off + n + 8 + (H * W * lb if lbl is not None else 0) + (extra.nbytes if extra is not None else 0) + \
+            (lmap.nbytes if lmap is not None and lbl is not None else 0)
+        if capacity is not None and need > capacity:
+            raise RuntimeError(f"DeviceBatcher: batch needs more than max_bytes={capacity} of staging memory")
+        img_off = off
+        off += (n + 3) // 4 * 4  # keep int32 label maps 4-byte aligned
+        if lbl is not None:
+            lbl_off = off
+            off += (H * W * lb + 3) // 4 * 4
+            if lmap is not None:
+                off += lmap.nbytes
+                lb |= lib.AUG_LABEL_MAP
+            if extra is not None:
+                extra = np.ascontiguousarray(extra, dtype=np.int32)
+                off += extra.nbytes
+        rec = record(b, img_off, lbl_off, H, W, lb)
+        if rec[-1] not in (1, 4, 1 | lib.AUG_LABEL_MAP) or (rec[-1] == 1 | lib.AUG_LABEL_MAP) != (lmap is not None and lbl is not None):
+            raise ValueError(f"pack_arena: sample {b}: lbl_bytes {rec[-1]} is not 1, 4 or 1 | AUG_LABEL_MAP with a label map")
+        parts.append((img, img_off, lbl, lbl_off, extra, rec))
+    arena = (out if out is not None else torch.zeros(off, dtype=torch.uint8))[:off]  # zeros: alignment gaps are defined
+    host = arena.numpy()
+    table = np.zeros(B, dtype=dtype)
+    if head is not None:
+        host[B * dtype.itemsize:B * dtype.itemsize + head.nbytes] = head.reshape(-1).view(np.uint8)
+    for b, (img, img_off, lbl, lbl_off, extra, rec) in enumerate(parts):
+        host[img_off:img_off + img.size] = img.reshape(-1)
+        if lbl is not None:
+            nb = lbl.nbytes
+            host[lbl_off:lbl_off + nb] = lbl.reshape(-1).view(np.uint8)
+            e = lbl_off + (nb + 3) // 4 * 4
+            if lmap is not None:
+                host[e:e + lmap.nbytes] = lmap.view(np.uint8)
+                e += lmap.nbytes
+            if extra is not None:
+                host[e:e + extra.nbytes] = extra.view(np.uint8)
+        table[b] = rec
+    host[:B * dtype.itemsize] = table.view(np.uint8)
+    return arena
+
+
+class PackedBatch:
+    """One batch packed for one kernel launch: `arena` (pack_arena's uint8 tensor) and what the launch needs.  kind is
+    "plain" (pad / crop / flip / normalise), "scale" (+ random-scale resize), "full" (+ rotation), "full_blur" (+ Gaussian
+    blur) or "val" (validation resize + centre crop).  DataLoader's pin_memory=True pins the arena (`pin_memory`)."""
+
+    __slots__ = ("arena", "kind", "B", "crop", "want_labels", "label_map", "head_bytes")
+
+    def __init__(self, arena, kind, B, crop, want_labels, label_map, head_bytes=0):
+        self.arena, self.kind, self.B, self.crop = arena, kind, int(B), int(crop)
+        self.want_labels, self.label_map, self.head_bytes = bool(want_labels), bool(label_map), int(head_bytes)
+
+    def pin_memory(self, *args):
+        return PackedBatch(self.arena.pin_memory(*args), self.kind, self.B, self.crop, self.want_labels, self.label_map, self.head_bytes)
+
+    def __len__(self):
+        return self.B
+
+
+_RECORD = {"plain": _ENTRY, "scale": _SCALE_ENTRY, "val": _SCALE_ENTRY, "full": _FULL_ENTRY, "full_blur": _FULL_ENTRY}
+
+
+def pack_plain(samples, crop, label_map=None, out=None):
+    """samples: sequence of (image uint8 [h,w,3], label uint8|int32 [h,w] or None, y0, x0, flip)."""
+    check_crop_origins(crop, [(np.shape(s[0])[0], np.shape(s[0])[1], s[2], s[3]) for s in samples])
+
+    def record(b, img_off, lbl_off, h, w, lb):
+        _, _, y0, x0, flip = samples[b]
+        return (img_off, lbl_off, h, w, int(y0), int(x0), int(bool(flip)), lb)
+
+    arena = pack_arena(samples, _ENTRY, record, label_map=label_map, out=out)
+    return PackedBatch(arena, "plain", len(samples), crop, samples[0][1] is not None, label_map is not None)
+
+
+def pack_scaled(samples, crop, label_map=None, out=None):
+    """samples: sequence of (RAW image, RAW label or None, h, w, y0, x0, flip)."""
+    check_crop_origins(crop, [(s[2], s[3], s[4], s[5]) for s in samples])
+
+    def record(b, img_off, lbl_off, H, W, lb):
+        _, _, h, w, y0, x0, flip = samples[b]
+        # cv::resize: inv_scale = dsize / ssize, scale = 1. / inv_scale — float64, computed here so the kernel sees the same bits
+        return (img_off, lbl_off, 1.0 / (int(w) / W), 1.0 / (int(h) / H), H, W, int(h), int(w), int(y0), int(x0), int(bool(flip)), lb)
+
+    arena = pack_arena(samples, _SCALE_ENTRY, record, label_map=label_map, out=out)
+    return PackedBatch(arena, "scale", len(samples), crop, samples[0][1] is not None, label_map is not None)
+
+
+def pack_full(samples, crop, sigmas=None, label_map=None, out=None):
+    """samples: sequence of (RAW image, RAW label or None, h, w, angle or None, y0, x0, flip); sigmas: per-sample blur sigma
+    or None.  kind "full_blur" when any sample's kernel size is 3, else "full"."""
+    B = len(samples)
+    check_crop_origins(crop, [(s[2], s[3], s[5], s[6]) for s in samples])
+    taps = None
+    if sigmas is not None:
+        if len(sigmas) != B:
+            raise ValueError(f"DeviceBatcher: {len(sigmas)} blur sigmas for {B} samples")
+        taps = np.array([gaussian_taps(s) for s in sigmas], dtype=np.float32)
+        if (taps[:, 1] == 0).all():
+            taps = None  # nothing to blur: the unblurred kernel gives the same bytes
+
+    def record(b, img_off, lbl_off, H, W, lb):
+        _, _, h, w, angle, y0, x0, flip = samples[b]
+        return (img_off, lbl_off, 1.0 / (int(w) / W), 1.0 / (int(h) / H)) + inverse_rotation(int(w), int(h), angle) + \
+            (H, W, int(h), int(w), int(y0), int(x0), int(bool(flip)), lb)
+
+    arena = pack_arena(samples, _FULL_ENTRY, record, head=taps, label_map=label_map, out=out)
+    return PackedBatch(arena, "full" if taps is None else "full_blur", B, crop, samples[0][1] is not None, label_map is not None,
+                       0 if taps is None else taps.nbytes)
+
+
+def pack_val(samples, crop, label_map=None, out=None):
+    """samples: sequence of (RAW image uint8 [H,W,3], RAW label uint8|int32 [H,W] or None)."""
+    for b, s in enumerate(samples):
+        if len(s) != 2:
+            raise ValueError(f"DeviceBatcher.stage_val: sample {b} is not an (image, label) pair")
+        im, lb = s
+        if np.ndim(im) != 3 or np.shape(im)[2] != 3 or min(np.shape(im)[:2]) < 1:
+            raise ValueError(f"DeviceBatcher.stage_val: sample {b}: image of shape {np.shape(im)} is not [H, W, 3]")
+        if lb is not None and tuple(np.shape(lb)) != tuple(np.shape(im)[:2]):
+            raise ValueError(f"DeviceBatcher.stage_val: sample {b}: label of shape {np.shape(lb)} for a {np.shape(im)} image")
+        if (lb is None) != (samples[0][1] is None):
+            raise ValueError("DeviceBatcher.stage_val: either every sample has a label or none has")
+    geom = [val_geometry(np.shape(s[0])[0], np.shape(s[0])[1], crop) for s in samples]
+    check_crop_origins(crop, [(h, w, y0, x0) for h, w, y0, x0 in geom])
+
+    def record(b, img_off, lbl_off, H, W, lb):
+        h, w, y0, x0 = geom[b]
+        return (img_off, lbl_off, 1.0 / (w / W), 1.0 / (h / H), H, W, h, w, y0, x0, 0, lb)
+
+    def tables(b, H, W):
+        h, w = geom[b][:2]
+        return np.concatenate([pil_nearest_index(W, w), pil_nearest_index(H, h)])
+
+    arena = pack_arena(samples, _SCALE_ENTRY, record, tail=tables, label_map=label_map, out=out)
+    return PackedBatch(arena, "val", len(samples), crop, samples[0][1] is not None, label_map is not None)
+
+
+def launch_packed(batch, dev, mean, std):
+    """Runs the kernel of `batch` (a PackedBatch) on `dev`, its arena already on the device.  Returns (images, labels)."""
+    B, c = batch.B, batch.crop
+    tab = dev[:B * _RECORD[batch.kind].itemsize]
+    kw = dict(want_labels=batch.want_labels, label_map=batch.label_map)
+    if batch.kind == "plain":
+        return ops.augment_batch_u8(dev, tab, B, c, c, mean, std, **kw)
+    if batch.kind == "scale":
+        return ops.augment_scale_batch_u8(dev, tab, B, c, c, mean, std, **kw)
+    if batch.kind == "val":
+        return ops.augment_val_batch_u8(dev, tab, B, c, c, mean, std, **kw)
+    if batch.kind == "full":
+        return ops.augment_full_batch_u8(dev, tab, B, c, c, mean, std, **kw)
+    if batch.kind == "full_blur":
+        o = tab.numel()
+        taps = dev[o:o + batch.head_bytes].view(torch.float32)
+        return ops.augment_full_blur_batch_u8(dev, tab, taps, B, c, c, mean, std, **kw)
+    raise ValueError(f"launch_packed: unknown batch kind {batch.kind!r}")
+
+
 class DeviceBatcher:
     def __init__(self, mean, std, crop_size, device, max_bytes=64 << 20):
         assert _ENTRY.itemsize == lib.load().seg_aug_entry_bytes()
+        assert _SCALE_ENTRY.itemsize == lib.load().seg_aug_scale_entry_bytes()
+        assert _FULL_ENTRY.itemsize == lib.load().seg_aug_full_entry_bytes()
         if not crop_size:
             raise ValueError("DeviceBatcher: crop_size None / 0 means the reference neither pads nor crops (and its validation "
                              "tail does not resize), so batches would have variable sizes; the device tails need a crop_size")
@@ -139,179 +335,56 @@ class DeviceBatcher:
         self._slot = 0
         self._events = [None, None]
 
-    def stage(self, samples):
-        """samples: sequence of (image uint8 [h,w,3], label uint8|int32 [h,w] or None, y0, x0, flip).  Packs them into
-        pinned memory, copies once, launches the kernel on the current stream.  Returns (images, labels)."""
-        B = len(samples)
-        check_crop_origins(self.crop, [(np.shape(s[0])[0], np.shape(s[0])[1], s[2], s[3]) for s in samples])
+    def _stage(self, pack, samples, *args, **kw):
+        """Packs with `pack` into the next pinned staging buffer, copies the arena once and launches its kernel on the
+        current stream."""
         slot = self._slot
         self._slot ^= 1
         if self._events[slot] is not None:
             self._events[slot].synchronize()  # the previous H2D copy out of this staging buffer has finished
-        host = self._host[slot].numpy()
-        table = np.zeros(B, dtype=_ENTRY)
-        off = B * _ENTRY.itemsize
-        want_labels = samples[0][1] is not None
-        for b, (img, lbl, y0, x0, flip) in enumerate(samples):
-            img = np.ascontiguousarray(img, dtype=np.uint8)
-            h, w = img.shape[:2]
-            assert img.shape == (h, w, 3), "images are HWC uint8 with 3 channels"
-            n = img.size
-            lb, lbl_off = 1, -1
-            if lbl is not None:
-                lbl = np.ascontiguousarray(lbl)
-                assert lbl.shape == (h, w) and lbl.dtype in (np.uint8, np.int32), "labels are uint8 or int32 [h,w]"
-                lb = lbl.dtype.itemsize
-            need = off + n + 8 + (h * w * lb if lbl is not None else 0)
-            if need > self.capacity:
-                raise RuntimeError(f"DeviceBatcher: batch needs more than max_bytes={self.capacity} of staging memory")
-            host[off:off + n] = img.reshape(-1)
-            img_off = off
-            off += (n + 3) // 4 * 4  # keep int32 label maps 4-byte aligned
-            if lbl is not None:
-                nb = h * w * lb
-                host[off:off + nb] = lbl.reshape(-1).view(np.uint8)
-                lbl_off = off
-                off += (nb + 3) // 4 * 4
-            table[b] = (img_off, lbl_off, h, w, int(y0), int(x0), int(bool(flip)), lb)
-        host[:B * _ENTRY.itemsize] = table.view(np.uint8)
-        self.last_staged_bytes = off
-        dev = self._host[slot][:off].to(self.device, non_blocking=True)
-        ev = torch.cuda.Event()
-        ev.record()
-        self._events[slot] = ev
-        tab = dev[:B * _ENTRY.itemsize]
-        return ops.augment_batch_u8(dev, tab, B, self.crop, self.crop, self.mean, self.std, want_labels=want_labels)
+        batch = pack(samples, self.crop, *args, out=self._host[slot], **kw)
+        return self.launch(batch, slot)
 
-    def _stage_raw(self, samples, dtype, record, head=None, tail=None):
-        """Packs RAW samples (image uint8 [H,W,3], label uint8|int32 [H,W] or None, ...) into the pinned staging buffer and
-        copies it to the device once: the B `dtype` records first, then `head` (a float32 array, e.g. per-sample blur taps),
-        then every image and label map 4-byte aligned, each label map followed by `tail(b, H, W)` (an int32 array) when given.
-        record(b, img_off, lbl_off, H, W, lbl_bytes) -> the record of sample b.  Returns (device arena, head offset)."""
-        B = len(samples)
-        slot = self._slot
-        self._slot ^= 1
-        if self._events[slot] is not None:
-            self._events[slot].synchronize()
-        host = self._host[slot].numpy()
-        table = np.zeros(B, dtype=dtype)
-        head_off = off = B * dtype.itemsize
-        if head is not None:
-            head = np.ascontiguousarray(head, dtype=np.float32)
-            host[off:off + head.nbytes] = head.reshape(-1).view(np.uint8)
-            off += head.nbytes
-        for b, s in enumerate(samples):
-            img, lbl = np.ascontiguousarray(s[0], dtype=np.uint8), s[1]
-            H, W = img.shape[:2]
-            assert img.shape == (H, W, 3), "images are HWC uint8 with 3 channels"
-            n = img.size
-            lb, lbl_off, extra = 1, -1, None
-            if lbl is not None:
-                lbl = np.ascontiguousarray(lbl)
-                assert lbl.shape == (H, W) and lbl.dtype in (np.uint8, np.int32), "labels are uint8 or int32 [H,W]"
-                lb = lbl.dtype.itemsize
-                extra = tail(b, H, W) if tail is not None else None
-            need = off + n + 8 + (H * W * lb if lbl is not None else 0) + (extra.nbytes if extra is not None else 0)
-            if need > self.capacity:
-                raise RuntimeError(f"DeviceBatcher: batch needs more than max_bytes={self.capacity} of staging memory")
-            host[off:off + n] = img.reshape(-1)
-            img_off = off
-            off += (n + 3) // 4 * 4
-            if lbl is not None:
-                nb = H * W * lb
-                host[off:off + nb] = lbl.reshape(-1).view(np.uint8)
-                lbl_off = off
-                off += (nb + 3) // 4 * 4
-                if extra is not None:
-                    host[off:off + extra.nbytes] = np.ascontiguousarray(extra, dtype=np.int32).view(np.uint8)
-                    off += extra.nbytes
-            table[b] = record(b, img_off, lbl_off, H, W, lb)
-        host[:B * dtype.itemsize] = table.view(np.uint8)
-        self.last_staged_bytes = off
-        dev = self._host[slot][:off].to(self.device, non_blocking=True)
-        ev = torch.cuda.Event()
-        ev.record()
-        self._events[slot] = ev
-        return dev, head_off
+    def launch(self, batch, slot=None):
+        """Copies a PackedBatch's arena to the device (non-blocking when it is pinned) and runs its kernel.  slot: the
+        staging buffer it was packed into, whose reuse then waits for this copy."""
+        if batch.crop != self.crop:
+            raise ValueError(f"DeviceBatcher: a batch packed for crop {batch.crop} given to a batcher with crop {self.crop}")
+        self.last_staged_bytes = batch.arena.numel()
+        dev = batch.arena.to(self.device, non_blocking=True)
+        if slot is not None:
+            ev = torch.cuda.Event()
+            ev.record()
+            self._events[slot] = ev
+        return launch_packed(batch, dev, self.mean, self.std)
 
-    def stage_scaled(self, samples):
+    def stage(self, samples, label_map=None):
+        """samples: sequence of (image uint8 [h,w,3], label uint8|int32 [h,w] or None, y0, x0, flip).  Packs them into
+        pinned memory, copies once, launches the kernel on the current stream.  Returns (images, labels).
+        label_map: a dataset's 256-entry id -> train-id table for uint8 labels (SEG_AUG_LABEL_MAP), or None."""
+        return self._stage(pack_plain, samples, label_map=label_map)
+
+    def stage_scaled(self, samples, label_map=None):
         """samples: sequence of (RAW image uint8 [H,W,3], RAW label uint8|int32 [H,W] or None, h, w, y0, x0, flip): the sample
         is resized to h x w (cv2.resize arithmetic, base_dataset.py:66-75) and then padded / cropped / flipped / normalised
         — in one kernel, without a resized intermediate (`seg_augment_scale_batch_u8`)."""
-        assert _SCALE_ENTRY.itemsize == lib.load().seg_aug_scale_entry_bytes()
-        B = len(samples)
-        check_crop_origins(self.crop, [(s[2], s[3], s[4], s[5]) for s in samples])
+        return self._stage(pack_scaled, samples, label_map=label_map)
 
-        def record(b, img_off, lbl_off, H, W, lb):
-            _, _, h, w, y0, x0, flip = samples[b]
-            # cv::resize: inv_scale = dsize / ssize, scale = 1. / inv_scale — float64, computed here so the kernel sees the same bits
-            return (img_off, lbl_off, 1.0 / (int(w) / W), 1.0 / (int(h) / H), H, W, int(h), int(w), int(y0), int(x0), int(bool(flip)), lb)
-
-        dev, _ = self._stage_raw(samples, _SCALE_ENTRY, record)
-        return ops.augment_scale_batch_u8(dev, dev[:B * _SCALE_ENTRY.itemsize], B, self.crop, self.crop, self.mean, self.std,
-                                          want_labels=samples[0][1] is not None)
-
-    def stage_full(self, samples, sigmas=None):
+    def stage_full(self, samples, sigmas=None, label_map=None):
         """(bit-exact against the staged oracle, tests/test_data_tail_gpu.py.)  samples: sequence of
         (RAW image, RAW label or None, h, w, angle or None, y0, x0, flip): resize to h x w, rotate by `angle` degrees about the
         centre (base_dataset.py:77-83), pad / crop / flip / normalise — one kernel (`seg_augment_full_batch_u8`).
         sigmas: per-sample Gaussian blur sigma or None (draw_blur; base_dataset.py:114-119), applied after the flip; when any
         sample's kernel size is 3 the batch runs `seg_augment_full_blur_batch_u8`, whose k = 1 samples are bit-identical
         to the unblurred kernel's."""
-        assert _FULL_ENTRY.itemsize == lib.load().seg_aug_full_entry_bytes()
-        B = len(samples)
-        check_crop_origins(self.crop, [(s[2], s[3], s[5], s[6]) for s in samples])
-        taps = None
-        if sigmas is not None:
-            if len(sigmas) != B:
-                raise ValueError(f"DeviceBatcher: {len(sigmas)} blur sigmas for {B} samples")
-            taps = np.array([gaussian_taps(s) for s in sigmas], dtype=np.float32)
-            if (taps[:, 1] == 0).all():
-                taps = None  # nothing to blur: the unblurred kernel gives the same bytes
+        return self._stage(pack_full, samples, sigmas, label_map=label_map)
 
-        def record(b, img_off, lbl_off, H, W, lb):
-            _, _, h, w, angle, y0, x0, flip = samples[b]
-            return (img_off, lbl_off, 1.0 / (int(w) / W), 1.0 / (int(h) / H)) + inverse_rotation(int(w), int(h), angle) + \
-                (H, W, int(h), int(w), int(y0), int(x0), int(bool(flip)), lb)
-
-        dev, head_off = self._stage_raw(samples, _FULL_ENTRY, record, head=taps)
-        tab, want_labels = dev[:B * _FULL_ENTRY.itemsize], samples[0][1] is not None
-        if taps is None:
-            return ops.augment_full_batch_u8(dev, tab, B, self.crop, self.crop, self.mean, self.std, want_labels=want_labels)
-        dtaps = dev[head_off:head_off + taps.nbytes].view(torch.float32)
-        return ops.augment_full_blur_batch_u8(dev, tab, dtaps, B, self.crop, self.crop, self.mean, self.std, want_labels=want_labels)
-
-    def stage_val(self, samples):
+    def stage_val(self, samples, label_map=None):
         """The validation tail of base_dataset.py:40-61 and :129-136.  samples: sequence of (RAW image uint8 [H,W,3], RAW label
         uint8|int32 [H,W] or None).  Each sample is resized so that its short side is crop_size (cv2.resize INTER_LINEAR on
         the image, PIL's NEAREST on the label, negative labels kept), centre-cropped, truncated to uint8 and normalised — one
         kernel (`seg_augment_val_batch_u8`), no resized intermediate."""
-        assert _SCALE_ENTRY.itemsize == lib.load().seg_aug_scale_entry_bytes()
-        B = len(samples)
-        for b, s in enumerate(samples):
-            if len(s) != 2:
-                raise ValueError(f"DeviceBatcher.stage_val: sample {b} is not an (image, label) pair")
-            im, lb = s
-            if np.ndim(im) != 3 or np.shape(im)[2] != 3 or min(np.shape(im)[:2]) < 1:
-                raise ValueError(f"DeviceBatcher.stage_val: sample {b}: image of shape {np.shape(im)} is not [H, W, 3]")
-            if lb is not None and tuple(np.shape(lb)) != tuple(np.shape(im)[:2]):
-                raise ValueError(f"DeviceBatcher.stage_val: sample {b}: label of shape {np.shape(lb)} for a {np.shape(im)} image")
-            if (lb is None) != (samples[0][1] is None):
-                raise ValueError("DeviceBatcher.stage_val: either every sample has a label or none has")
-        geom = [val_geometry(np.shape(s[0])[0], np.shape(s[0])[1], self.crop) for s in samples]
-        check_crop_origins(self.crop, [(h, w, y0, x0) for h, w, y0, x0 in geom])
-
-        def record(b, img_off, lbl_off, H, W, lb):
-            h, w, y0, x0 = geom[b]
-            return (img_off, lbl_off, 1.0 / (w / W), 1.0 / (h / H), H, W, h, w, y0, x0, 0, lb)
-
-        def tables(b, H, W):
-            h, w = geom[b][:2]
-            return np.concatenate([pil_nearest_index(W, w), pil_nearest_index(H, h)])
-
-        dev, _ = self._stage_raw(samples, _SCALE_ENTRY, record, tail=tables)
-        return ops.augment_val_batch_u8(dev, dev[:B * _SCALE_ENTRY.itemsize], B, self.crop, self.crop, self.mean, self.std,
-                                        want_labels=samples[0][1] is not None)
+        return self._stage(pack_val, samples, label_map=label_map)
 
     def stage_random(self, raw, flip=True, rng=random):
         """raw: sequence of (image, label).  Draws crop origin / flip per sample like the reference's worker would."""
@@ -332,6 +405,9 @@ class DevicePrefetcher:
         self.next_target = None
         self.device = device
         self.batcher = batcher
+        # a PackedBatch (packed by device_collate in the loader's workers) is normalised with the dataset's mean / std
+        self.mean = getattr(loader, "MEAN", None) or getattr(self.dataset, "mean", None)
+        self.std = getattr(loader, "STD", None) or getattr(self.dataset, "std", None)
 
     def __len__(self):
         return len(self.loader)
@@ -344,7 +420,12 @@ class DevicePrefetcher:
             self.next_target = None
             return
         with torch.cuda.stream(self.stream):
-            if isinstance(item, (tuple, list)) and len(item) == 2 and isinstance(item[0], torch.Tensor) and item[0].is_floating_point():
+            if isinstance(item, PackedBatch):   # the kernel comes from the batch's own records, not from the loader
+                if self.mean is None or self.std is None:
+                    raise RuntimeError("DevicePrefetcher: a packed batch needs the loader's MEAN / STD (or the dataset's mean / std)")
+                dev = item.arena.to(self.device, non_blocking=True)  # the one H2D copy of the batch
+                self.next_input, self.next_target = launch_packed(item, dev, self.mean, self.std)
+            elif isinstance(item, (tuple, list)) and len(item) == 2 and isinstance(item[0], torch.Tensor) and item[0].is_floating_point():
                 self.next_input = item[0].cuda(device=self.device, non_blocking=True)   # the reference's path, unchanged
                 self.next_target = item[1].cuda(device=self.device, non_blocking=True)
             else:
@@ -367,3 +448,57 @@ class DevicePrefetcher:
             yield input, target
             if type(self.stop_after) is int and (count > self.stop_after):
                 break
+
+
+# ------------------------------------------------------------------ the reference's datasets in device mode
+class DeviceSample(tuple):
+    """What a dataset in device mode returns per sample: (image uint8 [H,W,3], raw label uint8|int32 [H,W], draws, crop,
+    label_map).  draws is None for the validation tail, else (h, w, angle, y0, x0, flip, sigma) in the reference's draw
+    order, h = w = None when the sample is not resized (no base_size)."""
+
+    __slots__ = ()
+
+    def __new__(cls, image, label, draws, crop, label_map):
+        return tuple.__new__(cls, (image, label, draws, crop, label_map))
+
+    def __getnewargs__(self):
+        return tuple(self)
+
+
+def draw_augmentation(h, w, crop, base_size=None, scale=True, rotate=False, flip=True, blur=False, rng=random):
+    """The draws of base_dataset.py:63-119 for an h x w sample, with the reference's Python `random` calls in its order:
+    scale, angle, crop row, crop column, flip, blur sigma."""
+    h2, w2 = draw_scale(h, w, base_size, scale, rng)
+    angle = draw_rotate(rotate, rng)
+    y0, x0, f = draw_crop_flip(h2, w2, crop, flip, rng)
+    sigma = draw_blur(blur, rng)
+    return (h2, w2) if base_size else (None, None), angle, y0, x0, f, sigma
+
+
+def device_collate(batch):
+    """collate_fn of the device-mode loaders: packs a list of DeviceSample into one PackedBatch in the DataLoader worker
+    (pack_arena; the loader's pin_memory=True then pins it) and picks the kernel from the samples' own draws: validation
+    -> val; any rotation or 3 x 3 blur -> full (+ blur); any resize -> scale; else the plain tail.  Anything else (a dataset
+    on the reference's path) goes to torch's default_collate."""
+    if not isinstance(batch[0], DeviceSample):
+        from torch.utils.data import default_collate
+        return default_collate(batch)
+    crop, lmap = batch[0][3], batch[0][4]
+    if any(s[3] != crop for s in batch):
+        raise ValueError("device_collate: samples packed for different crop sizes")
+    vals = [s[2] is None for s in batch]
+    if all(vals):
+        return pack_val([(s[0], s[1]) for s in batch], crop, label_map=lmap)
+    if any(vals):
+        raise ValueError("device_collate: a batch mixes validation samples and training draws")
+    d = [s[2] for s in batch]
+    full = any(a is not None for (_, _, a, _, _, _, _) in d) or any(gaussian_taps(sg)[1] != 0 for (*_, sg) in d)
+    scaled = any(h is not None for (h, *_) in d)
+    hw = [(h, w) if h is not None else np.shape(s[0])[:2] for s, (h, w, *_) in zip(batch, d)]
+    if full:
+        return pack_full([(s[0], s[1], h, w, a, y0, x0, f) for s, (h, w), (_, _, a, y0, x0, f, _) in zip(batch, hw, d)], crop,
+                         sigmas=[sg for (*_, sg) in d], label_map=lmap)
+    if scaled:
+        return pack_scaled([(s[0], s[1], h, w, y0, x0, f) for s, (h, w), (_, _, _, y0, x0, f, _) in zip(batch, hw, d)], crop,
+                           label_map=lmap)
+    return pack_plain([(s[0], s[1], y0, x0, f) for s, (_, _, _, y0, x0, f, _) in zip(batch, d)], crop, label_map=lmap)

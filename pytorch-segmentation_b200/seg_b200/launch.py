@@ -28,7 +28,7 @@ def setup_paths(reference_root):
         sys.path.insert(0, p)
     # anything of the reference imported before the path was ordered must be re-resolved through the overlay
     for name in list(sys.modules):
-        if name.split(".")[0] in ("models", "utils", "base"):
+        if name.split(".")[0] in ("models", "utils", "base", "dataloaders"):
             del sys.modules[name]
     # utils/transforms.py:4 imports skimage, which this image lacks; the trainer never calls it (SURVEY.md §8c shim 1)
     try:

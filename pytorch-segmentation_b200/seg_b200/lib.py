@@ -16,6 +16,7 @@ LIB_PATH = os.path.join(os.path.dirname(_HERE), "libseg_b200.so")
 DT_BF16, DT_F32 = 0, 1
 IMPL_AUTO, IMPL_SIMT, IMPL_TC = 0, 1, 2
 LOSS_CE, LOSS_WCE, LOSS_FOCAL = 0, 1, 2  # SEG_LOSS_* (the `kind` of the seg_loss_* / seg_upsample_loss_* entry points)
+AUG_LABEL_MAP = 256  # SEG_AUG_LABEL_MAP: flag in an augmentation record's lbl_bytes (read by the *_mapped entry points)
 
 
 class SyncDesc(Structure):
@@ -141,6 +142,12 @@ _SIGS = {
     "seg_augment_val_batch_u8": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, POINTER(c_float), POINTER(c_float), c_void_p, c_void_p, c_void_p]),
     "seg_augment_full_blur_batch_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, POINTER(c_float), POINTER(c_float), c_void_p,
                                                c_void_p, c_void_p]),
+    "seg_augment_mapped_batch_u8": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, POINTER(c_float), POINTER(c_float), c_void_p, c_void_p, c_void_p]),
+    "seg_augment_scale_mapped_batch_u8": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, POINTER(c_float), POINTER(c_float), c_void_p, c_void_p, c_void_p]),
+    "seg_augment_val_mapped_batch_u8": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, POINTER(c_float), POINTER(c_float), c_void_p, c_void_p, c_void_p]),
+    "seg_augment_full_mapped_batch_u8": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, POINTER(c_float), POINTER(c_float), c_void_p, c_void_p, c_void_p]),
+    "seg_augment_full_blur_mapped_batch_u8": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, POINTER(c_float), POINTER(c_float), c_void_p,
+                                                      c_void_p, c_void_p]),
     "seg_resize_nchw_f32": (c_int, [c_void_p, c_int64, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int, c_float, c_float, c_void_p]),
     "seg_window_add_nchw_f32": (c_int, [c_void_p, c_int64, c_int, c_int, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p]),
     "seg_div_by_count_nchw_f32": (c_int, [c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p]),

@@ -900,61 +900,50 @@ def argmax_nchw(scores):
     return labels
 
 
-def augment_batch_u8(arena, table, B, crop_h, crop_w, mean, std, want_labels=True):
+def _augment(name, table_bytes, arena, table, taps, B, crop_h, crop_w, mean, std, want_labels, label_map):
+    assert arena.dtype == torch.uint8 and table.dtype == torch.uint8 and table.numel() == B * table_bytes
+    out = torch.empty((B, 3, crop_h, crop_w), dtype=torch.float32, device=arena.device)
+    labels = torch.empty((B, crop_h, crop_w), dtype=torch.int64, device=arena.device) if want_labels else None
+    m3 = (ctypes.c_float * 3)(*[float(v) for v in mean])
+    s3 = (ctypes.c_float * 3)(*[float(v) for v in std])
+    name = name.replace("_batch_u8", "_mapped_batch_u8") if label_map else name
+    head = (ptr(arena), ptr(table)) if taps is None else (ptr(arena), ptr(table), ptr(taps))
+    call(name, *head, int(B), int(crop_h), int(crop_w), m3, s3, ptr(out), ptr(labels))
+    return out, labels
+
+
+# label_map=True runs the *_mapped twin of each entry point, which also reads records whose lbl_bytes carries
+# lib.AUG_LABEL_MAP (a uint8 label map followed by its 256-entry int32 id table); records without the flag give the same
+# output under either kernel.
+def augment_batch_u8(arena, table, B, crop_h, crop_w, mean, std, want_labels=True, label_map=False):
     """arena: uint8 device tensor (images + labels back to back), table: uint8 device tensor of B seg_aug_entry records."""
-    assert arena.dtype == torch.uint8 and table.dtype == torch.uint8 and table.numel() == B * lib.load().seg_aug_entry_bytes()
-    out = torch.empty((B, 3, crop_h, crop_w), dtype=torch.float32, device=arena.device)
-    labels = torch.empty((B, crop_h, crop_w), dtype=torch.int64, device=arena.device) if want_labels else None
-    m3 = (ctypes.c_float * 3)(*[float(v) for v in mean])
-    s3 = (ctypes.c_float * 3)(*[float(v) for v in std])
-    call("seg_augment_batch_u8", ptr(arena), ptr(table), int(B), int(crop_h), int(crop_w), m3, s3, ptr(out), ptr(labels))
-    return out, labels
+    return _augment("seg_augment_batch_u8", lib.load().seg_aug_entry_bytes(), arena, table, None, B, crop_h, crop_w, mean, std,
+                    want_labels, label_map)
 
 
-def augment_scale_batch_u8(arena, table, B, crop_h, crop_w, mean, std, want_labels=True):
+def augment_scale_batch_u8(arena, table, B, crop_h, crop_w, mean, std, want_labels=True, label_map=False):
     """As augment_batch_u8 with the random-scale resize fused in front; table = B seg_aug_scale_entry records."""
-    assert arena.dtype == torch.uint8 and table.dtype == torch.uint8 and table.numel() == B * lib.load().seg_aug_scale_entry_bytes()
-    out = torch.empty((B, 3, crop_h, crop_w), dtype=torch.float32, device=arena.device)
-    labels = torch.empty((B, crop_h, crop_w), dtype=torch.int64, device=arena.device) if want_labels else None
-    m3 = (ctypes.c_float * 3)(*[float(v) for v in mean])
-    s3 = (ctypes.c_float * 3)(*[float(v) for v in std])
-    call("seg_augment_scale_batch_u8", ptr(arena), ptr(table), int(B), int(crop_h), int(crop_w), m3, s3, ptr(out), ptr(labels))
-    return out, labels
+    return _augment("seg_augment_scale_batch_u8", lib.load().seg_aug_scale_entry_bytes(), arena, table, None, B, crop_h, crop_w, mean,
+                    std, want_labels, label_map)
 
 
-def augment_full_batch_u8(arena, table, B, crop_h, crop_w, mean, std, want_labels=True):
+def augment_full_batch_u8(arena, table, B, crop_h, crop_w, mean, std, want_labels=True, label_map=False):
     """augment_scale_batch_u8 with the rotation (cv2.getRotationMatrix2D + warpAffine arithmetic) fused in; table = B
     seg_aug_full_entry records."""
-    assert arena.dtype == torch.uint8 and table.dtype == torch.uint8 and table.numel() == B * lib.load().seg_aug_full_entry_bytes()
-    out = torch.empty((B, 3, crop_h, crop_w), dtype=torch.float32, device=arena.device)
-    labels = torch.empty((B, crop_h, crop_w), dtype=torch.int64, device=arena.device) if want_labels else None
-    m3 = (ctypes.c_float * 3)(*[float(v) for v in mean])
-    s3 = (ctypes.c_float * 3)(*[float(v) for v in std])
-    call("seg_augment_full_batch_u8", ptr(arena), ptr(table), int(B), int(crop_h), int(crop_w), m3, s3, ptr(out), ptr(labels))
-    return out, labels
+    return _augment("seg_augment_full_batch_u8", lib.load().seg_aug_full_entry_bytes(), arena, table, None, B, crop_h, crop_w, mean,
+                    std, want_labels, label_map)
 
 
-def augment_val_batch_u8(arena, table, B, crop_h, crop_w, mean, std, want_labels=True):
+def augment_val_batch_u8(arena, table, B, crop_h, crop_w, mean, std, want_labels=True, label_map=False):
     """The validation tail (resize so the short side is the crop, centre crop, ToTensor, Normalize) on B seg_aug_scale_entry
     records; each label map in the arena is followed by its PIL NEAREST index tables (x then y, int32)."""
-    assert arena.dtype == torch.uint8 and table.dtype == torch.uint8 and table.numel() == B * lib.load().seg_aug_scale_entry_bytes()
-    out = torch.empty((B, 3, crop_h, crop_w), dtype=torch.float32, device=arena.device)
-    labels = torch.empty((B, crop_h, crop_w), dtype=torch.int64, device=arena.device) if want_labels else None
-    m3 = (ctypes.c_float * 3)(*[float(v) for v in mean])
-    s3 = (ctypes.c_float * 3)(*[float(v) for v in std])
-    call("seg_augment_val_batch_u8", ptr(arena), ptr(table), int(B), int(crop_h), int(crop_w), m3, s3, ptr(out), ptr(labels))
-    return out, labels
+    return _augment("seg_augment_val_batch_u8", lib.load().seg_aug_scale_entry_bytes(), arena, table, None, B, crop_h, crop_w, mean,
+                    std, want_labels, label_map)
 
 
-def augment_full_blur_batch_u8(arena, table, taps, B, crop_h, crop_w, mean, std, want_labels=True):
+def augment_full_blur_batch_u8(arena, table, taps, B, crop_h, crop_w, mean, std, want_labels=True, label_map=False):
     """augment_full_batch_u8 with the Gaussian blur after the flip; taps: float32 device tensor [B, 2] of (centre, side)
     taps, (1, 0) for a sample that is not blurred."""
-    assert arena.dtype == torch.uint8 and table.dtype == torch.uint8 and table.numel() == B * lib.load().seg_aug_full_entry_bytes()
     assert taps.dtype == torch.float32 and taps.is_contiguous() and taps.numel() == 2 * B and taps.device == arena.device
-    out = torch.empty((B, 3, crop_h, crop_w), dtype=torch.float32, device=arena.device)
-    labels = torch.empty((B, crop_h, crop_w), dtype=torch.int64, device=arena.device) if want_labels else None
-    m3 = (ctypes.c_float * 3)(*[float(v) for v in mean])
-    s3 = (ctypes.c_float * 3)(*[float(v) for v in std])
-    call("seg_augment_full_blur_batch_u8", ptr(arena), ptr(table), ptr(taps), int(B), int(crop_h), int(crop_w), m3, s3, ptr(out),
-         ptr(labels))
-    return out, labels
+    return _augment("seg_augment_full_blur_batch_u8", lib.load().seg_aug_full_entry_bytes(), arena, table, taps, B, crop_h, crop_w,
+                    mean, std, want_labels, label_map)
